@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # CPU restatement of the Go PS path
+    python bench.py --steps K --dump-outputs DIR             # also write what the last timed step computed
 
 One step = one pass of the PS hot path over one synthetic Criteo-shaped batch
 (BASELINE.json configs[1]): pull dense -> unique -> pull rows of 76 tables -> tower
@@ -12,7 +13,7 @@ fwd/bwd -> dedup-sum -> push with fused Adam -> version++.  Prints ONE JSON line
 `e2e`     : same metric with the step's ids/features/labels copied from pinned host
             memory and the loss copied back every step, inside the timed region
 `roofline`: the dominant PS kernel's algorithmic bytes / CUDA-event duration vs the
-            measured HBM copy bandwidth (MEASURED_PEAKS.json)
+            measured HBM copy bandwidth (MEASURED_PEAKS.json; else the H100 SXM data sheet's 3.35 TB/s)
 `cpu_baseline`: the oracle's C restatement of the Go PS path on the host cores
 """
 import argparse
@@ -28,21 +29,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 ADAM_ARGS = "learning_rate=0.001;beta_1=0.9;beta_2=0.999;epsilon=1e-07;amsgrad=false;"  # dac_ctr/elasticdl_train.py:47-48
-FALLBACK_HBM_GBS = 6650.0  # B200_PROFILING.md fallback
-
-
-def ncu_traffic(kernel, world):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the named kernel from the committed
-    `ncu --set full` capture of this workload at N=1 (profiles/ncu_traffic.json); None when the capture
-    does not cover the configuration (a number taken under ncu is never measured live by the bench)."""
-    if world != 1:
-        return None
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as f:
-            k = json.load(f)["kernels"][kernel]
-        return k["dram_read_bytes"] + k["dram_write_bytes"]
-    except (OSError, KeyError, ValueError):
-        return None
+FALLBACK_HBM_GBS = 3350.0  # H100 SXM data sheet (HBM3), a bound rather than a measured rate
 
 
 def measured_peak():
@@ -171,6 +158,36 @@ def cpu_reference(batch, steps, warmup, dist_kind, threads=None):
                     % ("the reference's own compiled Adam (oracle/_ref = kernel_api.cc built unmodified), one call per row "
                        "as kernel.go:119-138 does" if ref is not None else "the restated Adam (oracle/_ref not built)",
                        cands, T, batch, steps, dist_kind, ncpu))
+
+
+def dump_outputs(out_dir, engine, group, group_rows, seed=0, sample=512):
+    """After the last timed step: its loss, the dense parameters and a fixed sample of embedding rows (per id group
+    its first `sample` ids, the Zipf-hot ones, plus `sample` seeded draws) as .npy files, ~1.5 MB in all.  With
+    N > 1 GPUs this is rank 0's view: its own loss, and the rows and dense parameters of every shard as rank 0
+    reads them through the group (peer reads of the other ranks' shards) while the other ranks wait."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize(group.device)
+    np.save(os.path.join(out_dir, "loss.npy"), engine.loss_buf.detach().cpu().numpy().astype(np.float32))
+    names = [n for n, _ in engine.params]
+    for n, t in group.pull_dense(names).items():
+        np.save(os.path.join(out_dir, "dense__%s.npy" % n.replace("/", "_").replace(":", "_")),
+                t.cpu().numpy().astype(np.float32))
+    rng = np.random.RandomState(seed)
+    sample_ids = [np.unique(np.concatenate([np.arange(min(r, sample)), rng.randint(0, r, sample)])) for r in group_rows]
+    deep, wide = [], []
+    for g, ids in enumerate(sample_ids):
+        idt = torch.from_numpy(ids.astype(np.int64)).to(group.device)
+        d, w = group.pull_rows([(engine.deep_names[g], idt), (engine.wide_names[g], idt)])
+        deep.append(d.cpu().numpy())
+        wide.append(w.cpu().numpy().reshape(-1))
+    np.save(os.path.join(out_dir, "row_group.npy"),
+            np.concatenate([np.full(len(ids), g, dtype=np.float64) for g, ids in enumerate(sample_ids)]))
+    np.save(os.path.join(out_dir, "row_id.npy"), np.concatenate(sample_ids).astype(np.float64))
+    np.save(os.path.join(out_dir, "deep_rows.npy"), np.concatenate(deep).astype(np.float32))
+    np.save(os.path.join(out_dir, "wide_rows.npy"), np.concatenate(wide).astype(np.float32))
 
 
 def parity_check_multi(engine, group, rank, world, dev, lr=1e-3):
@@ -363,7 +380,12 @@ def main():
     ap.add_argument("--no-parity-check", action="store_true", help="skip the post-timing N>1 parity self-check")
     ap.add_argument("--ids", default="narrow", choices=["narrow", "int32"],
                     help="id transport of the packed batches: 1/2/4 bytes per id by table size, or int32")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (rank 0's view when N > 1; "
+                         "not available with --impl reference)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU path; --impl reference computes no outputs to dump")
     cpu_batch = args.cpu_batch or args.batch
 
     rank = int(os.environ.get("RANK", "0"))
@@ -405,7 +427,7 @@ def main():
 
     from elasticdl_b200 import _lib
     from elasticdl_b200.ps import PSGroup
-    from elasticdl_b200.workloads.deepfm import DeepFMPSEngine, N_DENSE, pack_batch, synthetic_batch
+    from elasticdl_b200.workloads.deepfm import GROUP_ROWS, DeepFMPSEngine, N_DENSE, pack_batch, synthetic_batch
 
     group = PSGroup(world, "Adam", ADAM_ARGS, device=local_rank,
                     local_shards=[rank] if world > 1 else None)
@@ -441,7 +463,7 @@ def main():
     rows_mb = u_mean * (96 + 16) / 1e6  # Adam records touched per step: 96 B (dim 8) + 16 B (dim 1) per unique id
     config["l2_policy"] = ("pool of %d distinct batches cycled: a batch's rows (%.0f MB of records per step, plus "
                            "~%.0f MB of id / dedup / row buffers) recur after %d other steps, i.e. after > %.0f MB of "
-                           "other traffic vs the 126 MB L2; Zipf-hot rows recur every step by construction of the workload"
+                           "other traffic vs the 50 MB L2; Zipf-hot rows recur every step by construction of the workload"
                            % (args.pool, rows_mb, 12 * G * B * 4 / 1e6, args.pool - 1, (args.pool - 1) * rows_mb))
 
     def sync_all():
@@ -484,6 +506,10 @@ def main():
     ms_eager = max_over_ranks(e0.elapsed_time(e1))
     launches = my_launches() - launches0
     group.check()
+    if args.dump_outputs and not use_graph:
+        if rank == 0:
+            dump_outputs(args.dump_outputs, engine, group, GROUP_ROWS)
+        sync_all()
     # per-kernel device times: the same eager steps with CUDA-event pairs around the named kernels.  The host
     # needs ~10 us per launch, more than some of these kernels run, so each step is queued behind a spin
     # kernel (torch.cuda._sleep) that keeps the GPU busy while the host enqueues the whole step: the kernels
@@ -519,6 +545,10 @@ def main():
         sync_all()
         ms = max_over_ranks(e0.elapsed_time(e1))
         group.check()
+        if args.dump_outputs:
+            if rank == 0:
+                dump_outputs(args.dump_outputs, engine, group, GROUP_ROWS)
+            sync_all()
     clocks = sampler.stop() if rank == 0 else None
 
     # ---- per-kernel durations from the CUDA events recorded inside the timed region ----
@@ -569,8 +599,8 @@ def main():
             engine.step(*packed_views(hb, G, B, engine.widths))
         # the D2H read of the step's loss: the last kernel of every step stores it into a ring in pinned host
         # memory (engine.loss_ring, 4 bytes over PCIe per step; b200_deepfm_publish_loss) -- a cudaMemcpyAsync of the
-        # scalar between two graph launches put a copy-engine round trip on the critical path of every step
-        # (tools/e2e_probe.py: 198 us per step without it, 222-237 us with it)
+        # scalar between two graph launches puts a copy-engine round trip on the critical path of every step
+        # (tools/e2e_probe.py measures both)
     e3.record()
     sync_all()
     ms_e2e = max_over_ranks(e2.elapsed_time(e3))
@@ -614,7 +644,6 @@ def main():
         step_ms = ms / args.steps
         line["roofline"] = {"kernel": top, "bound": "hbm", "achieved": k["gbs"], "peak": peak, "unit": "GB/s",
                             "frac": k["gbs"] / peak,
-                            "traffic": ncu_traffic(top, world) if (args.batch == 32768 and args.dist == "zipf") else None,
                             "peak_kind": peak_kind, "algorithmic_bytes_per_launch": k["bytes"], "us_per_launch": k["ms"] * 1e3,
                             "step_algorithmic_bytes": step_bytes, "step_gbs": step_bytes / step_ms / 1e6,
                             "step_frac": step_bytes / step_ms / 1e6 / peak,
@@ -622,17 +651,6 @@ def main():
                             "note": "achieved = algorithmic bytes (SURVEY 8d) / CUDA-event time of the launch (eager pass, GPU kept "
                                     "busy so that the event pairs bracket device time); "
                                     "step_frac = sum of the step's algorithmic bytes / graph ms_per_step / peak"}
-        # NOT measured in this run (labelled as such): where the row kernels sit once the launch is big enough to be
-        # bandwidth-bound, and the roof a bare random-row gather / read-modify-write reaches on the same memory system
-        line["roofline"]["row_kernels_at_scale"] = {
-            "not_measured_in_this_run": True,
-            "source": "profiles/r2_13_kernel_roofline_sweep_rows_final.jsonl (bench_kernels.py, graph-timed, 4 M unique "
-                      "random rows, table >> L2) and profiles/r2_01_gather_roof.jsonl (tools/probes/gather_roof.cu)",
-            "frac_of_copy_peak": {"pull_dim8": 0.376, "push_adam_dim8": 0.385, "pull_dim64": 0.675, "push_adam_dim64": 0.533,
-                                  "pull_dim1": 0.131, "push_adam_dim1": 0.154},
-            "bare_probe_frac_of_copy_peak": {"gather_dim8": 0.374, "rmw_adam_dim8": 0.465, "gather_dim64": 0.954,
-                                             "gather_dim1": 0.108},
-        }
         pk = "pull" if "pull" in kern else ("pull_deep" if "pull_deep" in kern else None)
         if pk:
             line["pull_gbs"] = kern[pk]["gbs"]

@@ -2,7 +2,7 @@
 """Kernel-level roofline sweep of the PS kernels (not the driver's bench: see bench.py).
 
 For each kernel: algorithmic bytes (SURVEY.md 8d) / CUDA-event time on the launching stream,
-against MEASURED_PEAKS.json:hbm_gbs.  Working sets exceed the 126 MB L2 (5.5 M-row tables,
+against MEASURED_PEAKS.json:hbm_gbs.  Working sets exceed the 50 MB L2 (5.5 M-row tables,
 ResNet-50-sized dense parameter), ids are unique and uniformly random.  One JSON line per case.
 """
 import json

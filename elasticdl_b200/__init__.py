@@ -1,4 +1,4 @@
-"""elasticdl_b200: B200-native parameter-server hot path behind ElasticDL's worker API.
+"""elasticdl_b200: H100-native parameter-server hot path behind ElasticDL's worker API.
 
 Only what the path needs (SURVEY.md section 8): the C-ABI CUDA library
 (csrc/, include/b200ps.h), the PS group wrapper (ps/), and host-side mirrors of

@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA C-ABI library (sm_100a only, no JIT cache)."""
+"""In-tree build of the CUDA C-ABI library (sm_90a only, no JIT cache)."""
 import os
 import subprocess
 
@@ -10,7 +10,7 @@ HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "
            os.path.join("..", "..", "include", "b200_deepfm.h"),
            os.path.join("..", "..", "include", "b200_features.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

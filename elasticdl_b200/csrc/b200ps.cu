@@ -119,7 +119,7 @@ struct b200ps {
   unsigned long long* d_count = nullptr;
   long long* d_state = nullptr;
   long long launches = 0;
-  int n_sm = 148;
+  int n_sm = 132;
   // owner-computes exchange (b200ps_xchg_*)
   int x_table = -1, x_G = 0, x_B = 0, x_me = -1;
   long long x_cap = 0, x_off_ids = 0, x_off_resp = 0, x_off_upd = 0, x_off_served = 0;
@@ -239,7 +239,7 @@ void count_launch(b200ps_t* ps, int n) {
 
 int grid_for(b200ps_t* ps, long long work_items, int per_block = 256) {
   long long blocks = (work_items + per_block - 1) / per_block;
-  long long cap = (long long)(ps ? ps->n_sm : 148) * 16;  // 16 CTAs of 256 threads per SM keep ~2 waves resident
+  long long cap = (long long)(ps ? ps->n_sm : 132) * 16;  // 16 CTAs of 256 threads per SM keep ~2 waves resident
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;
@@ -438,15 +438,14 @@ int for_each_class(b200ps_t* ps, Split& sp, F&& launch) {
 // Persistent grid of the flat kernels.  The grid must not exceed what is RESIDENT at once: a block that waits for
 // a free slot starts after the first wave has finished and pays the block prologue (76 device-side counts ->
 // scan -> barrier) and the launch ramp again.  Sized for 8 blocks per SM the 48-register kernels (5 resident)
-// ran 1.6 waves: push 34.8 -> 29.4 us, pull 20.4 -> 16.4 us, step 168.6 -> 162-164 us once the grid follows
-// cudaOccupancyMaxActiveBlocksPerMultiprocessor of the kernel actually launched (profiles/r2_13_*).
+// would run 1.6 waves, so the grid follows cudaOccupancyMaxActiveBlocksPerMultiprocessor of the kernel actually
+// launched.
 // U rows in flight per thread only once the work is several times what the resident threads cover.
 void flat_shape(b200ps_t* ps, long long items, int* U, int* grid, bool copy = false) {
   static const int force_u = [] { const char* e = getenv("B200_FLAT_U"); return e ? atoi(e) : 0; }();      // tuning knobs
   const long long resident1 = (long long)ps->n_sm * 6 * 256;  // about what the U = 1 kernels keep resident
   *U = items >= resident1 * 8 ? 2 : 1;
-  // (U = 4 is reachable through B200_FLAT_U only: measured on 1 M / 4 M dim-64 rows it LOSES to U = 2 --
-  //  41 % vs 49-51 % of the copy peak -- its 80 registers cost more resident warps than the unroll adds.)
+  // (U = 4 is reachable through B200_FLAT_U only: its 80 registers cost more resident warps than the unroll adds.)
   if (force_u == 1 || force_u == 2 || (copy && force_u == 4)) *U = force_u;
   *grid = 0;  // set by flat_grid() for the kernel instance that is launched
 }
@@ -909,10 +908,9 @@ static int rows_copy(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
   GroupView gv = group_view(ps);
   cudaStream_t st = (cudaStream_t)stream;
   // The shared-memory staged gather (cp.async in, one bulk async copy out per warp: bytes in flight bounded by
-  // shared memory instead of registers) is OPT-IN (B200_STAGED_MIN = lane-items from which it is taken): measured
-  // at 4 M random dim-8 rows it reaches 28 % of the copy peak where the register path reaches 35 % and the bare
-  // gather probe (tools/probes/gather_roof.cu) 37 % -- random 32 B sectors are bound by the memory system's
-  // request rate, not by bytes in flight, so the extra shared-memory round trip only costs.
+  // shared memory instead of registers) is OPT-IN (B200_STAGED_MIN = lane-items from which it is taken): random
+  // 32 B sectors are bound by the memory system's request rate, not by bytes in flight, so the extra
+  // shared-memory round trip only costs (compare with tools/probes/gather_roof.cu).
   const char* staged_env = getenv("B200_STAGED_MIN");
   const long long staged_min = staged_env ? atoll(staged_env) : (1LL << 62);
   if (sp.flat_n && !write && sp.flat_items >= staged_min) {

@@ -563,7 +563,7 @@ int b200_deepfm_fwd_bwd(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, true)) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = layout(args->G);
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const size_t smem = tower_a_smem(args->G);
@@ -603,7 +603,7 @@ int b200_deepfm_forward(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, false) || !args->logits) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = layout(args->G);
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const size_t smem = tower_a_smem(args->G);

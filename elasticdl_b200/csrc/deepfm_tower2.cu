@@ -1,7 +1,7 @@
 // DeepFM tower, tile version (include/b200_deepfm.h: b200_deepfm_fwd_bwd_tile / b200_deepfm_forward_tile).
 //
 // Round 1's tower gathered every embedding row three times (forward, backward, parameter-gradient
-// kernel) with one dependent global gather chain per lane at ~20 % occupancy: 113 us of a 198 us
+// kernel) with one dependent global gather chain per lane at low occupancy, most of the
 // step.  Here a CTA owns a tile of 32 samples and gathers the tile's 38 x 32 rows ONCE, with
 // cp.async (16 B, L2 -> shared memory, no registers held while in flight), into
 //     X[s] = [ deep 38 x 8 | dense 13 | 1 (bias column) | 0 0 | pad ]     (row stride 324 floats = 81 x 16 B,
@@ -81,6 +81,10 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// Two hidden units per call: two independent round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 // Tile column c of W1x -> index into the flat parameter / gradient layout, or -1 (padding).
 __host__ __device__ inline int w1x_src(const Layout& l, int G, int c, int j) {
@@ -259,10 +263,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
           const float4* w4 = reinterpret_cast<const float4*>(W1x + (c + d) * H1);
           const float2 xx = make_float2(xv[d], xv[d]);
 #pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {  // packed fp32 FMA (FFMA2, sm_100): two hidden units per instruction
+          for (int qd = 0; qd < 4; ++qd) {  // two hidden units per ffma2 call
             const float4 w = w4[qd];
-            h2[2 * qd] = __ffma2_rn(make_float2(w.x, w.y), xx, h2[2 * qd]);
-            h2[2 * qd + 1] = __ffma2_rn(make_float2(w.z, w.w), xx, h2[2 * qd + 1]);
+            h2[2 * qd] = ffma2(make_float2(w.x, w.y), xx, h2[2 * qd]);
+            h2[2 * qd + 1] = ffma2(make_float2(w.z, w.w), xx, h2[2 * qd + 1]);
           }
         }
       }
@@ -367,8 +371,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
 #pragma unroll
           for (int qd = 0; qd < 4; ++qd) {
             const float4 w = w4[qd];
-            dt2 = __ffma2_rn(make_float2(w.x, w.y), make_float2(dh1[4 * qd + 0], dh1[4 * qd + 1]), dt2);
-            dt2 = __ffma2_rn(make_float2(w.z, w.w), make_float2(dh1[4 * qd + 2], dh1[4 * qd + 3]), dt2);
+            dt2 = ffma2(make_float2(w.x, w.y), make_float2(dh1[4 * qd + 0], dh1[4 * qd + 1]), dt2);
+            dt2 = ffma2(make_float2(w.z, w.w), make_float2(dh1[4 * qd + 2], dh1[4 * qd + 3]), dt2);
           }
           x[d] = fmaf(dz, sd[d] - ev[d], dt2.x + dt2.y);
         }
@@ -415,9 +419,9 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
           const float4 dq = jsel == 0 ? q0 : (jsel == 1 ? q1 : (jsel == 2 ? q2 : q3));
           const float2 xx0 = make_float2(x0, x0), xx1 = make_float2(x1, x1);
 #pragma unroll
-          for (int j = 0; j < H1 / 2; ++j) acc0[j] = __ffma2_rn(make_float2(dh[2 * j], dh[2 * j + 1]), xx0, acc0[j]);
-          acc1[0] = __ffma2_rn(make_float2(dq.x, dq.y), xx1, acc1[0]);
-          acc1[1] = __ffma2_rn(make_float2(dq.z, dq.w), xx1, acc1[1]);
+          for (int j = 0; j < H1 / 2; ++j) acc0[j] = ffma2(make_float2(dh[2 * j], dh[2 * j + 1]), xx0, acc0[j]);
+          acc1[0] = ffma2(make_float2(dq.x, dq.y), xx1, acc1[0]);
+          acc1[1] = ffma2(make_float2(dq.z, dq.w), xx1, acc1[1]);
         }
         if (t < H2 * H1 + 2 * H2 + ND) {
           const int o = t;
@@ -486,7 +490,7 @@ int check_args(const b200_deepfm_args_t* a, bool backward) {
 template <bool BACKWARD>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
   cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   static bool attr_done[64][2] = {};

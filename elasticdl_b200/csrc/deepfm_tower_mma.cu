@@ -1,7 +1,7 @@
 // Tensor-core variant of the fused DeepFM tower (include/b200_deepfm.h: b200_deepfm_fwd_bwd_mma).
 //
 // The SIMT tower (deepfm_tower.cu) gathers every embedding row three times (forward, backward to
-// the rows, parameter gradients) and is bound by those latency chains at ~20 % occupancy.  Here a
+// the rows, parameter gradients) and is bound by those latency chains at low occupancy.  Here a
 // CTA gathers the rows of MT samples ONCE, asynchronously (cp.async), into a shared-memory tile
 //     X [MT][ deep 8G | dense 13 | 1.0 | 0-pad ]          (row stride = 4 mod 32 floats)
 // and the three contractions of the first layer share it, as m16n8k8 TF32 `mma.sync`:
@@ -438,7 +438,7 @@ int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
       !a->gsum_deep || !a->loss || !a->n_unique)
     return -1;
   cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const size_t smem = mma_smem_bytes(a->G);

@@ -198,9 +198,18 @@ __global__ void __launch_bounds__(256) k_fingerprint(const uint8_t* __restrict__
   }
 }
 
+// 8 resident blocks of 256 threads per SM of the current device
+int max_blocks() {
+  int dev = 0, n_sm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  return n_sm * 8;
+}
+
 int grid_x(long long n) {
   long long b = (n + 255) / 256;
-  if (b > 148 * 8) b = 148 * 8;
+  const int cap = max_blocks();
+  if (b > cap) b = cap;
   return (int)(b < 1 ? 1 : b);
 }
 
@@ -250,7 +259,7 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_boundaries; ++i) p.bnd[i] = boundaries[i];
   int gx = grid_x(B);
-  const int per = (148 * 8 + p.G + p.n_dense - 1) / (p.G + p.n_dense);
+  const int per = (max_blocks() + p.G + p.n_dense - 1) / (p.G + p.n_dense);
   if (gx > per) gx = per < 1 ? 1 : per;
   dim3 grid(gx, p.G + p.n_dense);
   k_feature_transform<<<grid, 256, 0, st>>>(p, numeric_dev, numeric_is_float, strings_dev, W, (long long)B, ids_out_dev,

@@ -2,9 +2,9 @@
 // RPCs per step (python/worker/ps_client.py:105-130 pull, :243-277 push), as NVLink traffic that is
 // contiguous in both directions and needs NO memory fences between GPUs.
 //
-// Measured on this box (tools/mgpu_probe.py): scattered 32 B accesses to a peer GPU -- reads AND
-// writes -- run at ~130-160 GB/s (a few G sectors/s, independent of request size), coalesced peer
-// traffic at the link rate.  So nothing scattered crosses NVLink:
+// Scattered 32 B accesses to a peer GPU -- reads AND writes -- run at a small fraction of the link
+// rate, bound by sectors per second whatever the request size (tools/mgpu_probe.py measures it);
+// coalesced peer traffic runs at the link rate.  So nothing scattered crosses NVLink:
 //   pull  k_x_post      requester buckets its unique ids BY OWNER (id % N) into its exchange buffer as
 //                       {id, slot} words: block-level histogram in shared memory, one cursor
 //                       reservation per (block, owner), the per-owner counts travel with the flag
@@ -26,7 +26,7 @@
 // written with one volatile vector store and polled with one volatile vector load, so a word is
 // either the stale epoch's or complete -- no ordering between different words is ever needed.
 // The first versions used st.release.sys / __threadfence_system(); a MEMBAR.SYS also waits on
-// the PCIe side, and with the next batch's H2D copy in flight the step went from 298 to 563 us
+// the PCIe side, and with the next batch's H2D copy in flight the step time nearly doubled
 // (tools/xchg_dma_probe.py).  All ranks launch the same kernels in the same order (bulk-synchronous
 // step); polls time out after ~2 s and raise instead of hanging the GPU.
 #pragma once

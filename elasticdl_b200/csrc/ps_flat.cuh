@@ -13,8 +13,8 @@
 //     block (up to 21 KB; sm_70+ takes 32 KB): the kernels read it through the constant cache with a
 //     warp-uniform index and never touch the device-side table directory.  The per-row dependent
 //     chain is id -> record -> store (it was count -> id -> TableView -> runtime scalars -> record ->
-//     store).  [The first flat version staged the directory into shared memory per block: with 1184
-//     blocks x 76 segments that prologue was half of the kernel -- ncu, profiles/r2_02.]
+//     store).  [The first flat version staged the directory into shared memory per block: with 8 blocks
+//     per SM x 76 segments that prologue dominated the kernel.]
 //   * each thread keeps U independent rows in flight: all id loads, then all record / gradient
 //     loads, then the arithmetic and the stores;
 //   * the update is "lane = (row, column)": the 8 lanes of a dim-8 row read 32 contiguous bytes of
@@ -22,8 +22,8 @@
 //     and every lane executes exactly one element update (the d8 kernel ran four on 2 of 8 lanes).
 // Measured and rejected (git history, commit "flat kernels: warp-uniform segment fast path"): specialising the
 // loop body for warp-iterations that lie inside one segment (segment constants loaded once, no per-item search)
-// cut instructions but cost 12-16 registers -- 4 M-row pull 35.5 % vs 36.2 % of the copy peak, dim-64 57-59 % vs
-// 58-60 %, step 191-192 vs 189-190 us: these kernels are bound by memory round trips, not by issue slots.
+// cut instructions but cost 12-16 registers and no time: these kernels are bound by memory round trips, not by
+// issue slots.
 // Arithmetic is opt_update<> of ps_kernels.cuh: results stay bit-identical to the oracle.
 // Replaces go/pkg/kernel/kernel.go:35-199 (Sparse* / Indexed* row loops) and
 // go/pkg/common/embedding_table.go:61-77 (Get / SetEmbeddingVectors).

@@ -1,4 +1,4 @@
-// sm_100a kernels of the PS hot path.  All of them are HBM-bound integer /
+// sm_90a kernels of the PS hot path.  All of them are HBM-bound integer /
 // fp32 elementwise work (no dense contraction -> no tensor cores): the rules
 // that matter are one 32-byte sector (two 128-bit accesses) per thread,
 // enough loads in flight to cover HBM / NVLink latency, and no wasted sectors.

@@ -1,5 +1,5 @@
 // unique (tf.unique, first-occurrence order + inverse index) over T equal-length id segments as ONE
-// persistent kernel (round 1: seven launches, 48 us at 38 x 32768 ids).
+// persistent kernel (round 1: seven launches).
 //
 //   phase 0  (only when something must be cleared) hash keys / position arrays
 //   phase A  insert: position array entry of every id <- min(position); all id loads, then all probes,
@@ -79,8 +79,8 @@ __device__ __forceinline__ long long u_id(const UArgs& a, const UIdLayout& L, in
 }
 // Branch-free id loads for unrolled loops: the element width is a property of the SEGMENT, so it is dispatched
 // once around the loop (U_KIND_SWITCH) and every load inside is one plain instruction.  With u_id() in the loop
-// each load sat behind its own width branch and the loads of a thread ran one after the other (ncu source view of
-// k_unique_small: 32 sequential round trips, 32 of its 39 us).
+// each load sat behind its own width branch and the loads of a thread ran one after the other (32 sequential
+// round trips in k_unique_small).
 template <int W, bool SGN>
 __device__ __forceinline__ long long u_ld(const unsigned char* b, long long i) {
   if (W == 1) return (long long)b[i];
@@ -150,8 +150,8 @@ __device__ __forceinline__ unsigned long long u_word(unsigned tag, unsigned flag
 // one segment (host-built map): segments whose ids are mostly distinct -- large tables: every position
 // costs an atomic and two uncached 32 B sector reads -- get one unit per block, segments with tiny id
 // ranges -- cache-resident position arrays, almost every position a duplicate -- several, so that all
-// blocks of a phase finish together (timeline, profiles/r2_04: with equal tiles the large-table blocks
-// took 2.4x the median and every other block waited at the grid barrier).
+// blocks of a phase finish together (with equal tiles the large-table blocks took much longer than the
+// median and every other block waited at the grid barrier; tools/unique_timeline.py shows it).
 constexpr int kUPPT = 4;
 constexpr int kUUnit = kUThreads * kUPPT;  // 1024
 
@@ -352,8 +352,8 @@ __global__ void __launch_bounds__(kUThreads, 4) k_unique(const __grid_constant__
   // The look-back works on whole runs: pass 1 counts the first occurrences of all the block's units and
   // publishes ONE aggregate, then looks back over the predecessor runs of the segment; pass 2 assigns the
   // ranks.  (Per-unit descriptors made a block's first unit wait for the previous block's LAST unit, which
-  // itself sat behind that block's earlier look-backs: the segment was processed serially -- timeline,
-  // profiles/r2_05.)
+  // itself sat behind that block's earlier look-backs: the segment was processed serially, as
+  // tools/unique_timeline.py showed.)
   for (int slot = blockIdx.x; slot < nslots; slot += gridDim.x) {
     int t, gcnt;
     long long j0;  // first unit of the run inside its segment
@@ -549,7 +549,7 @@ struct USmall {
 
 // IPT = ids per thread (k <= IPT * 1024): every id is loaded ONCE, with all of a thread's loads in flight together,
 // and stays in a register through the three passes (a one-block-per-SM kernel has nothing else to hide a load
-// behind: re-reading the ids per pass made it 40 us).  Thread tid owns positions j * 1024 + tid.
+// behind: re-reading the ids per pass made it slower).  Thread tid owns positions j * 1024 + tid.
 template <int IPT>
 __global__ void __launch_bounds__(kUSThreads, 1) k_unique_small(const __grid_constant__ UArgs a, const __grid_constant__ UIdLayout idl,
                                                                 const __grid_constant__ USmall us) {

@@ -1,7 +1,7 @@
 """DistributedOptimizer with fixed-global-batch gradient accumulation
 (elasticai_api/pytorch/optimizer.py:22-296) over torch.distributed.
 
-B200-first differences from the Horovod original:
+GPU-first differences from the Horovod original:
   * every gradient is a VIEW of one flat fp32 bucket, so `synchronize()` issues ONE
     all-reduce for the whole model (the reference fires one Horovod collective per
     parameter, optimizer.py:162-168; Keras ResNet-50 has 214 tensors) -- on NVSwitch the cost

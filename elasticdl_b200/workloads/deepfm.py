@@ -434,7 +434,7 @@ class DeepFMPSEngine:
         import ctypes as _ct
 
         # Branches: the step has six launch-bound kernels (pull_dense, tower prologue, push_begin, push_dense,
-        # push_end; 4-8 us each, ncu profiles/r2_*) that do not depend on the row kernels beside them.  With
+        # push_end) that do not depend on the row kernels beside them.  With
         # `branch` they run on a second stream -- inside a captured graph these become parallel branches --
         # while the main stream carries unique -> pull -> tower -> push rows:
         #   aux:  pull_dense -> push_begin -> tower prologue  | joined before the tower
@@ -596,7 +596,7 @@ class DeepFMPSEngine:
             # The dedup of the next batch runs beside the PUSH of this one: the push kernels are light
             # (48 registers, < 1 KB of shared memory) and share the SMs with the persistent dedup blocks,
             # whereas the tower's CTAs need the whole register file of an SM and would simply wait for
-            # the dedup to finish (measured: forking at the start of the step hid 11 of its 45 us).
+            # the dedup to finish (forking at the start of the step hid only a quarter of it).
             self.side.wait_stream(main)  # the other plan's buffers were last read by the previous step
             self._use(1 - p)
             with torch.cuda.stream(self.side):

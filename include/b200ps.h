@@ -1,5 +1,5 @@
 /*
- * b200ps.h -- C ABI of libb200ps.so: the B200-native replacement for the
+ * b200ps.h -- C ABI of libb200ps.so: the GPU-native replacement for the
  * ElasticDL parameter-server data path.
  *
  * What it replaces (paths relative to /root/reference/elasticdl/):

@@ -210,7 +210,7 @@ static void otable_insert_nolock(otable_t* t, int64_t key, float* row) {
   t->size++;
 }
 
-/* The B200 path's deterministic stand-in for the reference's lazy
+/* The GPU path's deterministic stand-in for the reference's lazy
  * RandomUniform(-0.05, 0.05, seed=len(map)) (embedding_table.go:51-54,
  * initializer.go:107-126).  The reference draws from Go's global math/rand
  * re-seeded with the current map size: insertion-order and race dependent, not

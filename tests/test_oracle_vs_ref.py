@@ -1,12 +1,14 @@
 """The oracle against the reference's OWN compiled kernels (oracle/_ref) and against the vectors they produced.
 
-* tests/golden/ref_kernel_vectors.npz was written by RUNNING /root/reference's kernel_api.cc (compiled unmodified,
+* tests/golden/ref_kernel_vectors.npz was written by RUNNING the reference's kernel_api.cc (compiled unmodified,
   oracle/Makefile `ref`) -- tests/golden/gen_kernel_vectors.py.  The C restatement (ps_oracle.c) and its numpy twin
   must reproduce every output bit for bit.  Runs anywhere (the fixture is committed).
-* where oracle/_ref itself is present (this container; the GPU box gets the prebuilt .so), the oracle is also
-  compared with it live on fresh random inputs, and kernel_test.go's own vectors are replayed through it.
+* tests/golden/ref_kernel_live.json (gen_kernel_vectors.py `live`) holds digests of what the reference kernels
+  returned on further seeded inputs, the outputs of kernel_test.go's own vectors and of the bench's CPU arm with the
+  reference's Adam as its row update; the oracle is held to those here, without the reference present.
 Bar: bit-exact (integer compare of the fp32 patterns).
 """
+import json
 import os
 import sys
 
@@ -16,10 +18,11 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
 import gen_kernel_vectors as G  # noqa: E402
 from oracle import ps_oracle as O  # noqa: E402
-from oracle import ref_kernels as R  # noqa: E402
 
 F = np.float32
 VEC = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_kernel_vectors.npz"))
+with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_kernel_live.json")) as _f:
+    LIVE = json.load(_f)
 
 
 def bits(a):
@@ -71,67 +74,43 @@ def test_oracle_reproduces_reference_kernel_vectors(name, runner):
         assert np.array_equal(bits(st[k]), bits(VEC[name + "/out_" + k])), (name, k)
 
 
-needs_ref = pytest.mark.skipif(R.lib() is None, reason="oracle/_ref not present (built only where /root/reference is)")
-
-
-@needs_ref
-@pytest.mark.parametrize("seed", range(6))
+@pytest.mark.parametrize("seed", G.LIVE_SEEDS)
 def test_oracle_equals_ref_live(seed):
     """Fresh random inputs each seed, sizes that exercise the SSE body and the scalar tail."""
-    rng = np.random.default_rng(seed)
-    n = int(rng.integers(1, 3000))
-    for name, kind, hp, _ in G.cases()[:13]:  # one of each kind / step
-        g3 = np.stack([G.inputs(rng, n)[0] for _ in range(3)])
-        base = [rng.standard_normal(n).astype(F)] + [np.abs(rng.standard_normal(n)).astype(F) for _ in range(3)]
-        a = [x.copy() for x in base]
+    want = LIVE["equals_ref_live"][str(seed)]
+    for name, kind, hp, g3, base in G.live_cases(seed):
         b = [x.copy() for x in base]
-        G.run_ref(kind, hp, g3, *a)
         run_oracle_c(kind, hp, g3, *b)
-        for x, y in zip(a, b):
-            assert np.array_equal(bits(x), bits(y)), (name, n)
+        assert G.digest(b) == want[name], (name, base[0].size)
 
 
-@needs_ref
 def test_ref_replays_kernel_test_go_vectors():
     """elasticdl/go/pkg/kernel/kernel_test.go:25-47 (SGD, exact) and :69-107 (Adam step 5, expected
-    values written with the Go-side formula, compared there with tolerance 1e-4... we keep 1e-6)."""
+    values written with the Go-side formula, compared there with tolerance 1e-4... we keep 1e-6), on what the
+    reference kernels returned for them; the oracle returns the same bits."""
+    ref = {k: np.array(v, dtype=np.uint32).view(F) for k, v in LIVE["kernel_test_go"].items()}
     g = np.arange(10, dtype=F) * F(0.5) + F(0.25)
     p = np.arange(10, dtype=F) * F(-0.3) + F(1.0)
     want = p - F(0.1) * g
-    R.sgd(g, p, 0.1)
-    assert np.array_equal(bits(p), bits(want))
+    assert np.array_equal(bits(ref["sgd_p"]), bits(want))
+    O.lib.oracle_sgd(O._f32(g), O._f32(p), 0.1, p.size)
+    assert np.array_equal(bits(p), bits(ref["sgd_p"]))
     rng = np.random.default_rng(3)
     g, p0, m0, v0 = [rng.random(10).astype(F) for _ in range(4)]
-    p, m, v = p0.copy(), m0.copy(), v0.copy()
-    R.adam(g, p, m, v, 0.1, 5, 0.9, 0.999, 1e-8)
+    p, m, v = ref["adam_p"], ref["adam_m"], ref["adam_v"]
     em = 0.9 * m0.astype(np.float64) + 0.1 * g
     ev = 0.999 * v0.astype(np.float64) + 0.001 * g.astype(np.float64) ** 2
     ep = p0 - 0.1 * np.sqrt(1 - 0.999 ** 5) / (1 - 0.9 ** 5) * em / (np.sqrt(ev) + 1e-8)
     assert np.allclose(m, em, rtol=1e-6) and np.allclose(v, ev, rtol=1e-6) and np.allclose(p, ep, rtol=1e-5, atol=1e-6)
+    po, mo, vo = p0.copy(), m0.copy(), v0.copy()
+    O.lib.oracle_adam(O._f32(g), O._f32(po), O._f32(mo), O._f32(vo), 0.1, po.size, 5, 0.9, 0.999, 1e-8, O._null_f32())
+    for x, y in ((po, p), (mo, m), (vo, v)):
+        assert np.array_equal(bits(x), bits(y))
 
 
-@needs_ref
 @pytest.mark.parametrize("dim", [1, 8])
 def test_sparse_adam_rows_through_the_reference_kernel(dim):
     """The CPU arm of bench.py updates table rows with the reference's own compiled Adam (one call per row, as
-    kernel.go:119-138 does through cgo): with and without the hook the tables end up bit-identical, duplicates
-    applied sequentially, AMSGrad slot included."""
-    import ctypes
-
-    rng = np.random.default_rng(dim)
-    ids = rng.integers(0, 50, 400).astype(np.int64)  # many duplicates: sequential application
-    grads = (rng.standard_normal((400, dim)) * 0.1).astype(F)
-
-    def run(hook):
-        O.lib.oracle_set_ref_adam(ctypes.cast(R.lib().Adam, ctypes.c_void_p) if hook else None)
-        try:
-            tabs = [O.OracleTable(dim, "uniform", seed=3)] + [O.OracleTable(dim, "zero") for _ in range(3)]
-            for step in (1, 2, 7):
-                O.lib.oracle_sparse_adam(tabs[0]._h, tabs[1]._h, tabs[2]._h, tabs[3]._h, O._i64(ids), O._f32(grads),
-                                         ids.size, 0.01, step, 0.9, 0.999, 1e-7)
-            return [t.get(np.arange(50)) for t in tabs]
-        finally:
-            O.lib.oracle_set_ref_adam(None)
-
-    for a, b in zip(run(True), run(False)):
-        assert np.array_equal(bits(a), bits(b))
+    kernel.go:119-138 does through cgo): the oracle's own row update leaves the tables bit-identical to what that
+    hook produced, duplicates applied sequentially, AMSGrad slot included."""
+    assert G.digest(G.sparse_adam_tables(dim, None)) == LIVE["sparse_adam"][str(dim)]

@@ -7,6 +7,9 @@ accumulator 0.1), PS shards striped over the GPUs (id % N), B = 262144 ids per p
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port 29551 \
         tools/bench_ftrl1b.py
 
+--rows defaults to 1e9 over two or more GPUs and to 5e8 on one: 1e9 records of 96 B (96 GB) exceed one H100's
+80 GB, 5e8 (48 GB) leave room for the id pool, workspaces and the CUDA context.
+
 One step per rank = unique (hashed: ids are unbounded for the dedup) -> pull rows -> synthetic gradient ->
 push (FTRL fused in the row kernel, params + accumulator + linear in one 96 B record).  At N > 1 every rank
 addresses all shards directly (flat kernels over peer-mapped slabs).  Rank 0 first checks one push of
@@ -42,7 +45,7 @@ def draw_ids(n, rows, dist_kind, gen, dev):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--rows", type=int, default=1_000_000_000)
+    ap.add_argument("--rows", type=int, default=0, help="table slots (0: 1e9, or 5e8 on a single GPU)")
     ap.add_argument("--dim", type=int, default=8)
     ap.add_argument("--batch", type=int, default=262144)
     ap.add_argument("--dist", default="uniform", choices=["uniform", "zipf"])
@@ -50,6 +53,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+    if args.rows <= 0:
+        args.rows = 1_000_000_000 if world > 1 else 500_000_000
     local = int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)

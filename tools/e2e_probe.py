@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Where does the e2e step lose its ~35 us against the device-resident step?  Same engine, same graphs, K steps each:
+"""Where does the e2e step lose time against the device-resident step?  Same engine, same graphs, K steps each:
   value      step_ahead_graph on device-resident packed batches (what bench.py's `value` times)
   feeder_dev the HostFeeder fed with DEVICE batches (same Python, D2D instead of H2D copies)
   feeder_h2d the HostFeeder fed with pinned HOST batches (what bench.py's `e2e` times)
@@ -61,7 +61,7 @@ def main():
                 scratch.copy_(host[j % pool], non_blocking=True)
 
     def value_dma(i):
-        bg_enqueue(2)  # ~2 x 92 us of DMA per ~190 us step: the link stays busy
+        bg_enqueue(2)  # two 4 MB copies per step keep the link busy
         eng.step_ahead_graph(devp[(i + 1) % pool])
 
     out["value_with_background_h2d_us"] = timed(value_dma)

@@ -1,7 +1,7 @@
 // Bare random-row gather / read-modify-write probes: what the HBM system of this GPU sustains for the ACCESS
 // PATTERN of the PS row kernels (one random 32..256 B record per id out of a table far larger than L2), with
 // none of the PS logic around it.  The roof the row kernels of csrc/ps_flat.cuh can be held against.
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/probes/gather_roof tools/probes/gather_roof.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/probes/gather_roof tools/probes/gather_roof.cu
 // Prints one JSON line per variant: algorithmic bytes use SURVEY 8d's formulas (id + row read + row write).
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -103,7 +103,7 @@ static float time_us(F launch, int reps = 20) {
 int main(int argc, char** argv) {
   const long long n = argc > 1 ? atoll(argv[1]) : 4000000;       // ids per launch
   const long long rows = argc > 2 ? atoll(argv[2]) : 16000000;   // table rows (ids are a random subset)
-  const double peak = argc > 3 ? atof(argv[3]) : 6567.4;
+  double peak = argc > 3 ? atof(argv[3]) : 0.0;  // GB/s; default: the stream copy measured below
   std::vector<int64_t> h(rows);
   std::iota(h.begin(), h.end(), 0);
   std::mt19937_64 rng(7);
@@ -113,12 +113,16 @@ int main(int argc, char** argv) {
   float *out, *grad, *sink;
   CK(cudaMalloc(&out, n * 256)); CK(cudaMalloc(&grad, n * 256)); CK(cudaMalloc(&sink, 4));
   CK(cudaMemset(grad, 0, n * 256));
-  // streaming copy roof on this box
+  // streaming copy roof of this GPU
   {
     const long long m = 1LL << 26;  // 1 GiB each way
+    int dev = 0, n_sm = 0;
+    CK(cudaGetDevice(&dev));
+    CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     float4 *a, *b; CK(cudaMalloc(&a, m * 16)); CK(cudaMalloc(&b, m * 16)); CK(cudaMemset(a, 0, m * 16));
-    const float us = time_us([&] { k_copy<<<148 * 16, 256>>>(a, b, m); }, 5);
+    const float us = time_us([&] { k_copy<<<n_sm * 16, 256>>>(a, b, m); }, 5);
     printf("{\"probe\": \"stream_copy\", \"bytes\": %lld, \"us\": %.1f, \"gbs\": %.0f}\n", 2 * m * 16, us, 2.0 * m * 16 / us / 1e3);
+    if (peak <= 0.0) peak = 2.0 * m * 16 / us / 1e3;
     CK(cudaFree(a)); CK(cudaFree(b));
   }
   struct Cfg { const char* name; int dim; int slots; };
