@@ -8,7 +8,8 @@
 //            odd, so a warp's 32 rows are bank-conflict free for 128-bit reads; wide values in WV[g][s])
 // and everything else -- H1 = X W1x, the FM sums, the per-sample middle, dX = dH1 W1x^T + FM term with the
 // per-unique-id reduction, dW1x += dH1^T X and the small gradients -- runs out of shared memory:
-//   G  gather             5 (group, sample) pairs per thread: rank load, 2 cp.async + 1 wide load
+//   G  gather             warp = the 5 id groups it reads in F (and the last warp the dense block), a lane pair
+//                         per 32 B row; F waits for the warp's own copies only (no CTA barrier between G and F)
 //   F  forward            warp = 40 tile columns (5 id groups), lane = sample: 16 accumulators + FM partials
 //   M  middle             partial records summed through shared memory; every warp redoes the tiny
 //                         per-sample MLP tail (it needs dh1 / dz / FM sums in registers for B1 anyway)
@@ -16,12 +17,14 @@
 //                         (warp-level id dedup), one vector red per distinct row
 //   B2 parameter grads    thread = tile column t x 16 hidden units + 4 hidden units of column 256 + t % 64
 //                         (all 8 warps busy), accumulated in registers across the CTA's tiles, one atomic
-//                         per output per CTA at the end
+//                         per output per CTA at the end; B1 writes no shared memory, so a warp goes from its
+//                         B1 straight into B2 (no barrier between them).  The 85 small gradients run on 255
+//                         threads, 3 per output over 11 samples each.
 // W1 is presented in TILE COLUMN ORDER (W1x[c][j]: deep columns first, then dense, then b1 as the weight
 // of the constant-1 column) by the prep kernel, so the bias needs no special case and every CTA loads it
-// with straight 16-byte copies.  fp32 SIMT: the step has 1 GFLOP of first-layer work -- the kernel is
-// bound by the row gather and shared-memory bandwidth, not by FMA throughput; tensor cores would need
-// 3xTF32 splitting to keep the fp32-grade parity with the torch reference the tests check.
+// with straight 16-byte copies.  fp32 SIMT: the step has 1 GFLOP of first-layer work, and the kernel waits on
+// the gather round trip and on its per-tile phases and barriers, not on FMA throughput (DESIGN.md section 10:
+// a 3xTF32 mma.sync version of F / B1 / B2 measured slower).
 #include <cuda_runtime.h>
 
 #include <cstdlib>
@@ -43,6 +46,10 @@ constexpr int RS = 39;        // rank row stride (odd): Rt[s][g]
 constexpr int RW = H1 + D + 2;  // partial record: h[16] | s[8] | q | lin
 constexpr int MS = 44;        // per-sample backward state: dh1 16 | a1 16 | dh2 4 | h2 4 | dz | pad 3
 constexpr int MAXG = 38;
+constexpr int NSMALL = H2 * H1 + 2 * H2 + ND;  // small gradients: dW2 64 | db2 4 | dw3 4 | dwd 13
+constexpr int SPART = 3;                       // threads per small gradient (255 threads, 11 samples each)
+constexpr int SPLEN = (TS + SPART - 1) / SPART;
+static_assert(NKP * KPC == NCOL && (NKP - 1) * KPC <= MAXG * D, "the last warp owns the dense block");
 
 struct Layout {
   int in, o_wd, o_w1, o_b1, o_w2, o_b2, o_w3, total;
@@ -150,7 +157,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   // B2 accumulators, persistent over the CTA's tiles, all 8 warps busy: thread t owns tile column t (16 hidden
   // units) and, of the remaining 64 columns, column 256 + t%64 x hidden units 4*(t/64) .. +3
   float2 acc0[H1 / 2], acc1[2];
-  float sacc = 0.f;  // threads t < 85: one small output each (dW2 64 | db2 4 | dw3 4 | dwd 13)
+  float sacc = 0.f;  // threads t < SPART * NSMALL: a third of one small output
 #pragma unroll
   for (int j = 0; j < H1 / 2; ++j) acc0[j] = make_float2(0.f, 0.f);
   acc1[0] = acc1[1] = make_float2(0.f, 0.f);
@@ -158,14 +165,16 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   __syncthreads();
 
   const long long ntile = ((long long)B + TS - 1) / TS;
-  // ranks of a tile: 4-byte cp.async, coalesced reads of inv (32 consecutive samples of one group per warp)
+  // Warp w owns id groups g0 .. g0 + 4 (tile columns 40 w .. 40 w + 39) in G, F and B1, and warp NKP - 1 also the
+  // dense | 1 | 0 0 block: each warp gathers exactly what it reads in F, so F waits for the warp's own copies
+  // only, not for the whole tile behind a CTA barrier.
+  const int g0 = warp * (KPC / D);
+  const int gl = max(0, min(G - g0, KPC / D));  // live groups of this warp
+  // ranks of a tile: 4-byte cp.async, lane = sample, coalesced reads of inv (32 consecutive samples of one group)
   auto fetch_ranks = [&](const long long tl, int* dst) {
-    const long long bb0 = tl * TS;
-    for (int i = t; i < G * TS; i += THREADS) {
-      long long b = bb0 + (i & 31);
-      if (b >= B) b = B - 1;  // dead samples replay the last one, their results are masked
-      cp_async4(dst + (i & 31) * RS + (i >> 5), a.inv + (long long)(i >> 5) * B + b);
-    }
+    long long b = tl * TS + lane;
+    if (b >= B) b = B - 1;  // dead samples replay the last one, their results are masked
+    for (int k = 0; k < gl; ++k) cp_async4(dst + lane * RS + g0 + k, a.inv + (long long)(g0 + k) * B + b);
   };
   // Tiles are handed out dynamically (one atomic per tile on a counter the prologue set to gridDim.x): with
   // 1024 tiles on 296 resident CTAs a static round-robin leaves SMs with 8 tiles next to SMs with 6.  A CTA
@@ -189,47 +198,34 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
     // ---------------- G: gather the tile once ----------------
     // The tile's ranks are already in Rt (prefetched while the previous tile was computed), so the gather is
     // ONE global round trip: the row copies of this tile and the rank prefetch of the next one fly together.
-    // Rows: lane = consecutive 16 B chunk of ONE sample's row (contiguous shared-memory destinations).
+    // Each warp copies its own groups' rows.
+    const bool live = b0 + lane < B;
     {
-      const int npair = G * TS;
-      constexpr int NFILL = (TS * 16 + THREADS - 1) / THREADS;  // dense | 1 | 0 0 columns: 2 per thread
-      float dv[NFILL];
+      float* xrow = X + lane * XS;
+      for (int k = 0; k < gl; ++k) {  // a lane pair copies one 32 B row: one request per row sector
+        const int g = g0 + k;
 #pragma unroll
-      for (int jj = 0; jj < NFILL; ++jj) {  // tile columns 304..319 of sample s: dense 13 | 1 | 0 | 0
-        const int i = t + THREADS * jj;
-        const int s = i >> 4, c = i & 15;
-        long long b = b0 + s;
-        if (b >= B) b = B - 1;
-        float v = c == ND ? 1.0f : 0.f;
-        if (i < TS * 16 && c < ND) v = a.dense[b * ND + c];
-        dv[jj] = v;
-      }
-      const int nchunk = G * 2;  // 16 B chunks per sample row
-      for (int i = t; i < TS * nchunk; i += THREADS) {
-        const int s = i / nchunk, ch = i - s * nchunk;
-        const int g = ch >> 1;
-        const int r = Rt[s * RS + g];
-        cp_async16(X + s * XS + ch * 4, a.bet_deep + ((long long)g * B + r) * D + (ch & 1) * 4);
-      }
-      for (int i = t; i < npair; i += THREADS) {  // wide values: lane = sample
-        const int g = i >> 5, s = i & 31;
-        cp_async4(WV + g * TS + s, a.bet_wide + (long long)g * B + Rt[s * RS + g]);
+        for (int q = 0; q < 2; ++q) {
+          const int s = 16 * q + (lane >> 1), h = lane & 1;
+          cp_async16(X + s * XS + g * D + 4 * h, a.bet_deep + ((long long)g * B + Rt[s * RS + g]) * D + 4 * h);
+        }
+        cp_async4(WV + g * TS + lane, a.bet_wide + (long long)g * B + Rt[lane * RS + g]);
       }
       if (tile_next < ntile) fetch_ranks(tile_next, Rt0 + (cur ^ 1) * (TS * RS));
-#pragma unroll
-      for (int jj = 0; jj < NFILL; ++jj) {
-        const int i = t + THREADS * jj;
-        if (i < TS * 16) X[(i >> 4) * XS + MAXG * D + (i & 15)] = dv[jj];
+      for (int g = g0 + gl; g < min(g0 + KPC / D, MAXG); ++g) {  // unused group columns (G < 38): zeros
+        *reinterpret_cast<float4*>(xrow + g * D) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(xrow + g * D + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
-      for (int i = t; i < TS * (MAXG - G) * D; i += THREADS) {  // unused group columns (G < 38): zeros
-        const int s = i / ((MAXG - G) * D), c = G * D + i % ((MAXG - G) * D);
-        X[s * XS + c] = 0.f;
+      if (warp == NKP - 1) {  // tile columns 304..319: dense 13 | 1 | 0 | 0
+        const float* dense = a.dense + (live ? b0 + lane : B - 1) * ND;
+        for (int c = 0; c < ND; ++c) cp_async4(xrow + MAXG * D + c, dense + c);
+        xrow[MAXG * D + ND] = 1.0f;
+        xrow[MAXG * D + ND + 1] = 0.f;
+        xrow[MAXG * D + ND + 2] = 0.f;
       }
       cp_async_wait_all();
+      __syncwarp();
     }
-    __syncthreads();
-    if (t == 0) s_tile[iter & 1] = atomicAdd(tile_counter, 1);  // tile of iteration iter + 2
-    const bool live = b0 + lane < B;
     // ---------------- F: partial H1 / FM sums over this warp's 40 columns ----------------
     {
       float2 h2[H1 / 2];
@@ -282,6 +278,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
       mine[(H1 + D + 1) * TS] = lin;
     }
     __syncthreads();
+    if (t == 0) s_tile[iter & 1] = atomicAdd(tile_counter, 1);  // tile of iteration iter + 2 (every thread has read the slot)
     // ---------------- M: sum the 8 partial records ----------------
     float tsum[4];
 #pragma unroll
@@ -353,6 +350,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         m4[9] = make_float4(h2[0], h2[1], h2[2], h2[3]);
         m4[10] = make_float4(dz, 0.f, 0.f, 0.f);
       }
+      __syncthreads();  // Mst complete; B1 writes no shared memory, so each warp runs B1 and B2 back to back
       // ---------------- B1: d loss / d embedding rows of this warp's groups, reduced per unique id ----------------
       const float* xrow = X + lane * XS;
 #pragma unroll 1
@@ -404,7 +402,6 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
           atomicAdd(a.gsum_wide + (long long)g * B + r, x[D]);
         }
       }
-      __syncthreads();  // Mst complete
       // ---------------- B2: parameter gradients, accumulated over the CTA's tiles ----------------
       {
         // second column: 256 + t % 64, hidden units 4*(t/64) .. +3 -- warp-uniform, so its dh1 quad is one of the
@@ -423,9 +420,9 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
           acc1[0] = ffma2(make_float2(dq.x, dq.y), xx1, acc1[0]);
           acc1[1] = ffma2(make_float2(dq.z, dq.w), xx1, acc1[1]);
         }
-        if (t < H2 * H1 + 2 * H2 + ND) {
-          const int o = t;
-          for (int s = 0; s < TS; ++s) {
+        if (t < SPART * NSMALL) {  // output t % NSMALL over a third of the samples
+          const int o = t % NSMALL, s0 = (t / NSMALL) * SPLEN, s1 = min(TS, s0 + SPLEN);
+          for (int s = s0; s < s1; ++s) {
             const float* m = Mst + s * MS;
             float v;
             if (o < H2 * H1) v = m[32 + o / H1] * m[16 + o % H1];                         // dh2[k] * a1[j]
@@ -450,14 +447,16 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
       const int dst = w1x_src(l, G, 256 + (t & 63), (t >> 6) * 4 + j);
       if (dst >= 0) atomicAdd(a.grads + dst, (j & 1) ? acc1[j >> 1].y : acc1[j >> 1].x);
     }
-    if (t < H2 * H1 + 2 * H2 + ND) {
+    if (t < SPART * NSMALL) P[t] = sacc;  // P is free: every thread has left the tile loop
+    __syncthreads();
+    if (t < NSMALL) {
       const int o = t;
       int off;
       if (o < H2 * H1) off = l.o_w2 + o;
       else if (o < H2 * H1 + H2) off = l.o_b2 + o - H2 * H1;
       else if (o < H2 * H1 + 2 * H2) off = l.o_w3 + o - H2 * H1 - H2;
       else off = l.o_wd + o - H2 * H1 - 2 * H2;
-      atomicAdd(a.grads + off, sacc);
+      atomicAdd(a.grads + off, P[o] + P[NSMALL + o] + P[2 * NSMALL + o]);
     }
     if (warp == 0) {
       for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_down_sync(0xffffffffu, loss_acc, o);
