@@ -25,6 +25,18 @@ class Seg(ctypes.Structure):
     ]
 
 
+DEEPFM_TILE_MAXG = 38
+
+
+class DeepFMRows(ctypes.Structure):  # b200_deepfm_rows_t (include/b200_deepfm.h)
+    _fields_ = [
+        ("uniq", ctypes.c_void_p),
+        ("deep_base", ctypes.c_void_p * DEEPFM_TILE_MAXG), ("wide_base", ctypes.c_void_p * DEEPFM_TILE_MAXG),
+        ("deep_stride", ctypes.c_int64), ("wide_stride", ctypes.c_int64),
+        ("deep_param_off", ctypes.c_int64), ("wide_param_off", ctypes.c_int64),
+    ]
+
+
 class DeepFMArgs(ctypes.Structure):  # b200_deepfm_args_t (include/b200_deepfm.h)
     _fields_ = [
         ("G", ctypes.c_int32), ("B", ctypes.c_int32),
@@ -34,6 +46,7 @@ class DeepFMArgs(ctypes.Structure):  # b200_deepfm_args_t (include/b200_deepfm.h
         ("params", ctypes.c_void_p), ("grads", ctypes.c_void_p),
         ("gsum_wide", ctypes.c_void_p), ("gsum_deep", ctypes.c_void_p),
         ("loss", ctypes.c_void_p), ("logits", ctypes.c_void_p), ("scratch", ctypes.c_void_p),
+        ("rows", ctypes.POINTER(DeepFMRows)),
     ]
 
 
@@ -91,6 +104,8 @@ SYMBOLS = {
     "b200ps_push_end_shard": (_i, [_vp, _i, _vp]),
     "b200ps_raw_register": (_i, [_vp, ctypes.c_char_p, _sz]),
     "b200ps_raw_ptr": (_i, [_vp, _i, _i, ctypes.POINTER(_vp), ctypes.POINTER(_sz)]),
+    "b200ps_table_rows_ptr": (_i, [_vp, _i, _i, ctypes.POINTER(ctypes.POINTER(_f)), ctypes.POINTER(_i64),
+                                   ctypes.POINTER(_i64), ctypes.POINTER(_i64)]),
     "b200ps_barrier": (_i, [_vp, _vp]),
     "b200ps_kernel_sgd": (_i, [_vp, _vp, _f, ctypes.c_longlong, _vp]),
     "b200ps_kernel_momentum": (_i, [_vp, _vp, _vp, _f, _i, _f, ctypes.c_longlong, _vp]),

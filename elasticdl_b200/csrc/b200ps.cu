@@ -1370,6 +1370,21 @@ int b200ps_raw_ptr(b200ps_t* ps, int table, int shard, void** ptr, size_t* bytes
   return B200PS_OK;
 }
 
+int b200ps_table_rows_ptr(b200ps_t* ps, int table, int shard, float** base, int64_t* row_stride, int64_t* param_off,
+                          int64_t* rows) {
+  if (!ps || table < 0 || table >= (int)ps->tables.size() || shard < 0 || shard >= ps->n_shards || !base ||
+      !row_stride || !param_off || !rows)
+    return fail(B200PS_EINVAL, "bad argument");
+  const Table& t = ps->tables[table];
+  if (t.raw || t.is_dense || t.hashed) return fail(B200PS_EINVAL, t.name + " is not a direct-indexed embedding table");
+  if (!t.alloc[shard].ptr) return fail(B200PS_ESTATE, "shard not attached (sync peers after registering)");
+  *base = (float*)((char*)t.alloc[shard].ptr + t.base_off);
+  *row_stride = t.row_stride;
+  *param_off = t.slot_off[0];
+  *rows = t.rows;
+  return B200PS_OK;
+}
+
 int b200ps_barrier(b200ps_t* ps, void* stream) {
   int rc = ready(ps);
   if (rc) return rc;

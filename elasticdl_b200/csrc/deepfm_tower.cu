@@ -545,6 +545,7 @@ int check_args(const b200_deepfm_args_t* a, bool backward) {
   if (!a || a->G < 1 || a->B < 1) { g_msg = "bad shape"; return -1; }
   if (ND + a->G * D + 1 > TB_COLW * TB_CPT) { g_msg = "too many id groups for the fused tower (max 46)"; return -1; }
   if (!a->inv || !a->bet_wide || !a->bet_deep || !a->dense || !a->params) { g_msg = "null input"; return -1; }
+  if (a->rows) { g_msg = "the fused tower reads pulled rows only"; return -1; }
   if (backward && (!a->labels || !a->grads || !a->gsum_wide || !a->gsum_deep || !a->loss || !a->scratch || !a->n_unique)) {
     g_msg = "null output";
     return -1;

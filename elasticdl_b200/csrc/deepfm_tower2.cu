@@ -78,6 +78,16 @@ constexpr int SM_R = 2 * TS * RS;          // 2496   ranks Rt[buffer][s][g]: thi
 constexpr int SM_WV = MAXG * TS;           // 1216   wide values WV[g][s]
 constexpr int SM_SMALL = 128;              // b... w2 64 | b2 4 | w3 4 | wd 16
 constexpr size_t SMEM_BYTES = (size_t)(SM_W1X + SM_X + SM_P + SM_R + SM_WV + SM_SMALL) * sizeof(float);
+constexpr int SM_U = TS * RS;              // 1248   table rows only: ids Ut[s][g] of the next tile, behind the rest
+static_assert(MAXG == B200_DEEPFM_TILE_MAXG, "include/b200_deepfm.h");
+
+// b200_deepfm_rows_t as the kernel reads it (parameter space): the param offsets folded into the bases.
+struct TileRows {
+  const int64_t* uniq;
+  const float* deep[MAXG];
+  const float* wide[MAXG];
+  long long deep_stride, wide_stride;
+};
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
@@ -127,8 +137,14 @@ __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_p
   }
 }
 
-template <bool BACKWARD>
-__global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a, const float* __restrict__ w1x_g) {
+// TABLE: the rows come straight from the tables' record slabs (TileRows) instead of bet_deep / bet_wide, which
+// saves the step a separate pull kernel.  The id of a (sample, group) is one more dependent read between the
+// rank and the row, so the ids of tile i + 1 are fetched right after the ranks of tile i + 1 land (end of G)
+// and fly during the compute of tile i: G stays one round trip, and only a CTA's first tile pays
+// rank -> id -> row back to back.
+template <bool BACKWARD, bool TABLE>
+__global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a, const float* __restrict__ w1x_g,
+                                                           const __grid_constant__ TileRows rows) {
   extern __shared__ __align__(16) float smem[];
   float* W1x = smem;                 // [NCOL][16]
   float* X = W1x + SM_W1X;           // [TS][XS]
@@ -140,6 +156,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   float* s_b2 = small + 64;   // [H2]
   float* s_w3 = small + 68;   // [H2]
   float* s_wd = small + 72;   // [ND]
+  int* Ut = reinterpret_cast<int*>(small + SM_SMALL);  // TABLE: [TS][RS] low words of the ids (< 2^31, direct-indexed)
   float* T = P;                          // [RW][TS] summed records (first RW*TS floats of P)
   float* Mst = P + RW * TS + 64;         // [TS][MS] per-sample backward state for B2 (after T, 16 B aligned)
 
@@ -176,6 +193,13 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
     if (b >= B) b = B - 1;  // dead samples replay the last one, their results are masked
     for (int k = 0; k < gl; ++k) cp_async4(dst + lane * RS + g0 + k, a.inv + (long long)(g0 + k) * B + b);
   };
+  // TABLE: the ids of a tile from its ranks, lane = sample; each lane reads the ranks its own copies wrote
+  auto fetch_ids = [&](const int* R) {
+    for (int k = 0; k < gl; ++k) {
+      const int g = g0 + k;
+      cp_async4(Ut + lane * RS + g, rows.uniq + (long long)g * B + R[lane * RS + g]);
+    }
+  };
   // Tiles are handed out dynamically (one atomic per tile on a counter the prologue set to gridDim.x): with
   // 1024 tiles on 296 resident CTAs a static round-robin leaves SMs with 8 tiles next to SMs with 6.  A CTA
   // needs the index of its NEXT tile while it gathers the current one (rank prefetch), so two slots rotate:
@@ -189,6 +213,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   int cur = 0;
   if ((long long)blockIdx.x < ntile) fetch_ranks(blockIdx.x, Rt0);
   cp_async_wait_all();
+  if (TABLE && (long long)blockIdx.x < ntile) {
+    fetch_ids(Rt0);
+    cp_async_wait_all();
+  }
   __syncthreads();
   for (int iter = 0;; ++iter, cur ^= 1) {
     const int tile = s_tile[iter & 1], tile_next = s_tile[(iter + 1) & 1];
@@ -201,15 +229,22 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
     // Each warp copies its own groups' rows.
     const bool live = b0 + lane < B;
     {
+      if (TABLE) {  // this tile's ids (fetched during the previous tile's compute) from every lane of the warp
+        cp_async_wait_all();
+        __syncwarp();
+      }
       float* xrow = X + lane * XS;
       for (int k = 0; k < gl; ++k) {  // a lane pair copies one 32 B row: one request per row sector
         const int g = g0 + k;
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const int s = 16 * q + (lane >> 1), h = lane & 1;
-          cp_async16(X + s * XS + g * D + 4 * h, a.bet_deep + ((long long)g * B + Rt[s * RS + g]) * D + 4 * h);
+          const float* src = TABLE ? rows.deep[g] + Ut[s * RS + g] * rows.deep_stride
+                                   : a.bet_deep + ((long long)g * B + Rt[s * RS + g]) * D;
+          cp_async16(X + s * XS + g * D + 4 * h, src + 4 * h);
         }
-        cp_async4(WV + g * TS + lane, a.bet_wide + (long long)g * B + Rt[lane * RS + g]);
+        cp_async4(WV + g * TS + lane, TABLE ? rows.wide[g] + Ut[lane * RS + g] * rows.wide_stride
+                                            : a.bet_wide + (long long)g * B + Rt[lane * RS + g]);
       }
       if (tile_next < ntile) fetch_ranks(tile_next, Rt0 + (cur ^ 1) * (TS * RS));
       for (int g = g0 + gl; g < min(g0 + KPC / D, MAXG); ++g) {  // unused group columns (G < 38): zeros
@@ -224,7 +259,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         xrow[MAXG * D + ND + 2] = 0.f;
       }
       cp_async_wait_all();
-      __syncwarp();
+      __syncwarp();  // (TABLE: also orders this tile's reads of Ut before the overwrite below)
+      if (TABLE && tile_next < ntile) fetch_ids(Rt0 + (cur ^ 1) * (TS * RS));
     }
     // ---------------- F: partial H1 / FM sums over this warp's 40 columns ----------------
     {
@@ -477,12 +513,40 @@ __global__ void k_publish_loss(const float* __restrict__ loss, float* ring, int 
 int check_args(const b200_deepfm_args_t* a, bool backward) {
   if (!a || a->G < 1 || a->B < 1) { g_msg = "bad shape"; return -1; }
   if (a->G > MAXG) { g_msg = "the tile tower holds at most 38 id groups"; return -1; }
-  if (!a->inv || !a->bet_wide || !a->bet_deep || !a->dense || !a->params || !a->scratch) { g_msg = "null input"; return -1; }
+  if (!a->inv || !a->dense || !a->params || !a->scratch || (!a->rows && (!a->bet_wide || !a->bet_deep))) {
+    g_msg = "null input";
+    return -1;
+  }
   if (backward && (!a->labels || !a->grads || !a->gsum_wide || !a->gsum_deep || !a->loss || !a->n_unique)) {
     g_msg = "null output";
     return -1;
   }
+  if (a->rows) {
+    const b200_deepfm_rows_t* r = a->rows;
+    if (!backward) { g_msg = "the forward-only tile tower reads pulled rows only"; return -1; }
+    if (!r->uniq || r->deep_stride < D || r->wide_stride < 1 || r->deep_param_off < 0 || r->wide_param_off < 0 ||
+        r->deep_stride % 4 || r->deep_param_off % 4) {
+      g_msg = "bad row source";
+      return -1;
+    }
+    for (int g = 0; g < a->G; ++g)
+      if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15)) {
+        g_msg = "bad row source";
+        return -1;
+      }
+  }
   return 0;
+}
+
+template <bool BACKWARD, bool TABLE>
+void launch_tile(int dev, unsigned grid, cudaStream_t st, const b200_deepfm_args_t& a, const float* w1x, const TileRows& rows) {
+  constexpr size_t smem = SMEM_BYTES + (TABLE ? SM_U * sizeof(int) : 0);
+  static bool attr_done[64] = {};
+  if (dev < 64 && !attr_done[dev]) {
+    cudaFuncSetAttribute(k_tower_tile<BACKWARD, TABLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr_done[dev] = true;
+  }
+  k_tower_tile<BACKWARD, TABLE><<<grid, THREADS, smem, st>>>(a, w1x, rows);
 }
 
 // what: 1 = prologue only (k_tile_prep), 2 = tile kernel only, 3 = both
@@ -492,11 +556,6 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
   int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  static bool attr_done[64][2] = {};
-  if (dev < 64 && !attr_done[dev][BACKWARD]) {
-    cudaFuncSetAttribute(k_tower_tile<BACKWARD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
-    attr_done[dev][BACKWARD] = true;
-  }
   b200_deepfm_args_t a = *args;
   if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
   float* w1x = a.scratch;  // NCOL*16 floats at the start of the scratch buffer, then the tile counter
@@ -513,7 +572,23 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
     if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
     return 0;
   }
-  k_tower_tile<BACKWARD><<<(unsigned)grid, THREADS, SMEM_BYTES, st>>>(*args, w1x);
+  TileRows rows{};
+  if constexpr (BACKWARD) {  // only the training entry points accept a row source (check_args)
+    if (const b200_deepfm_rows_t* r = args->rows) {
+      rows.uniq = r->uniq;
+      for (int g = 0; g < a.G; ++g) {
+        rows.deep[g] = r->deep_base[g] + r->deep_param_off;
+        rows.wide[g] = r->wide_base[g] + r->wide_param_off;
+      }
+      rows.deep_stride = r->deep_stride;
+      rows.wide_stride = r->wide_stride;
+      launch_tile<true, true>(dev, (unsigned)grid, st, *args, w1x, rows);
+    } else {
+      launch_tile<true, false>(dev, (unsigned)grid, st, *args, w1x, rows);
+    }
+  } else {
+    launch_tile<false, false>(dev, (unsigned)grid, st, *args, w1x, rows);
+  }
   g_launches += 1;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }

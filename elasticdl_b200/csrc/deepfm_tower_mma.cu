@@ -435,7 +435,7 @@ int64_t b200_deepfm_mma_launch_count(void) { return g_launches_mma; }
 int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
   if (!a || a->G < 1 || a->B < 1 || tile_of(a->G).kp / 8 > 4 * MAX_NT_W) return -1;
   if (!a->inv || !a->bet_wide || !a->bet_deep || !a->dense || !a->params || !a->labels || !a->grads || !a->gsum_wide ||
-      !a->gsum_deep || !a->loss || !a->n_unique)
+      !a->gsum_deep || !a->loss || !a->n_unique || a->rows)
     return -1;
   cudaStream_t st = (cudaStream_t)stream;
   int dev = 0, n_sm = 132;

@@ -9,10 +9,11 @@ tower DNN[16,4] over 13 + 38*8 inputs, FM over the 38x8 deep embeddings, linear
 part = sum of wide embeddings + Dense(1)(dense features); Adam lr 1e-3.
 
 `DeepFMPSEngine.step` is one pass of the hot path: pull dense -> unique ids
-(first-occurrence) -> pull rows (one launch per vector class for all 76 tables) ->
-gather -> tower fwd/bwd (torch, library GEMMs) -> segment-sum of per-occurrence
-gradients -> push (dense + 76 tables, fused Adam) -> version++.  No host sync
-inside the step; nothing but ids/features/labels comes from the host.
+(first-occurrence) -> pull rows (one launch for all 76 tables; with row_source="table" the
+tile tower reads the rows from the tables itself and there is no pull) -> gather -> tower
+fwd/bwd (torch, library GEMMs) -> segment-sum of per-occurrence gradients -> push (dense +
+76 tables, fused Adam) -> version++.  No host sync inside the step; nothing but
+ids/features/labels comes from the host.
 """
 import math
 
@@ -214,14 +215,30 @@ class HostFeeder:
         return loss
 
 
+def resolve_row_source(row_source, tower, n_shards, exchange, paired):
+    """DeepFMPSEngine's row_source: "table" (the tower reads the table records) needs the tile tower and every
+    record on this GPU in its own slab -- one shard, the direct exchange, unpaired tables."""
+    assert row_source in ("auto", "table", "pull")
+    table_ok = tower == "tile" and n_shards == 1 and exchange == "direct" and not paired
+    if row_source == "auto":
+        return "table" if table_ok else "pull"
+    if row_source == "table" and not table_ok:
+        raise ValueError('row_source="table" needs the tile tower, one shard, the direct exchange and unpaired tables')
+    return row_source
+
+
 class DeepFMPSEngine:
     def __init__(self, group, batch, lr=1e-3, init_std=0.01, seed=7, group_rows=GROUP_ROWS, deep_dim=DEEP_DIM,
-                 init_rows=True, tower="tile", paired=None, exchange=None, id_transport="int32"):
+                 init_rows=True, tower="tile", paired=None, exchange=None, id_transport="int32", row_source="auto"):
         """tower="tile": rows of 32 samples gathered once into shared memory, forward / backward / parameter
         gradients from the tile (csrc/deepfm_tower2.cu);
         tower="fused": round 1's hand-written CUDA tower (csrc/deepfm_tower.cu, three row gathers);
         tower="mma": its tensor-core variant (csrc/deepfm_tower_mma.cu, rows gathered once, 3xTF32 mma.sync);
-        tower="torch": torch autograd over library kernels (kept for A/B measurements and tests)."""
+        tower="torch": torch autograd over library kernels (kept for A/B measurements and tests).
+        row_source="table": the tile tower reads each sample's rows straight from the table records
+        (b200_deepfm_rows_t) and step() launches no row pull; "pull": the rows of the unique ids are first
+        pulled into bet_w / bet_d.  "auto" takes "table" where it applies: tile tower, one shard, direct
+        exchange, tables not paired."""
         assert tower in ("tile", "fused", "mma", "torch")
         if tower == "tile" and len(group_rows) > 38:
             tower = "fused"  # the tile tower holds at most 38 id groups in its shared-memory row
@@ -241,6 +258,7 @@ class DeepFMPSEngine:
         self.exchange = exchange
         if exchange == "owner":
             self.paired = False
+        self.row_source = resolve_row_source(row_source, tower, group.n_shards, exchange, self.paired)
         self.group = group
         self.B = int(batch)
         self.G = len(group_rows)
@@ -348,7 +366,7 @@ class DeepFMPSEngine:
         self.steps = 0
 
     _PLAN_ATTRS = ("uniq", "inv", "n_unique", "pull_segs", "push_segs", "pull_pair", "push_pair", "tower_args",
-                   "pull_names", "push_names")
+                   "tower_rows", "pull_names", "push_names")
 
     def _make_plan(self):
         dev, G, B = self.device, self.G, self.B
@@ -411,6 +429,32 @@ class DeepFMPSEngine:
         a.gsum_wide, a.gsum_deep = self.gsum_w.data_ptr(), self.gsum_d.data_ptr()
         a.loss, a.logits, a.scratch = self.loss_buf.data_ptr(), self.logits_buf.data_ptr(), self.scratch.data_ptr()
         self.tower_args = a
+        self.tower_rows = None
+        if self.row_source == "table":
+            self.tower_rows = self._table_rows()
+            a.rows = _ct.pointer(self.tower_rows)
+
+    def _table_rows(self):
+        """b200_deepfm_rows_t of the current plan: its unique ids and the record slabs of the G deep and G wide
+        tables (one shard)."""
+        import ctypes as _ct
+        from elasticdl_b200._lib import DeepFMRows
+
+        g, r = self.group, DeepFMRows()
+        r.uniq = self.uniq.data_ptr()
+        for fam, tids, bases in (("deep", self.deep_ids, r.deep_base), ("wide", self.wide_ids, r.wide_base)):
+            layout = set()
+            for k, tid in enumerate(tids):
+                base, stride, off, rows = _ct.POINTER(_ct.c_float)(), _ct.c_int64(), _ct.c_int64(), _ct.c_int64()
+                check(g.lib.b200ps_table_rows_ptr(g._h, tid, 0, _ct.byref(base), _ct.byref(stride), _ct.byref(off),
+                                                  _ct.byref(rows)))
+                bases[k] = _ct.cast(base, _ct.c_void_p).value
+                layout.add((stride.value, off.value))
+            assert len(layout) == 1, layout  # one record layout per family: same dim, same optimizer
+            (stride, off), = layout
+            setattr(r, fam + "_stride", stride)
+            setattr(r, fam + "_param_off", off)
+        return r
 
     def step(self, ids, dense, labels, ev=None, after_tower=None):
         """ids int64 [G, B] (group-major), dense fp32 [B, 13], labels fp32 [B] -- all on the device.
@@ -468,22 +512,23 @@ class DeepFMPSEngine:
         else:
             arr, n = self.pull_dense_segs
             check(lib.b200ps_pull_dense(h, arr, n, st))
-        # (3) pull the unique rows of all 76 tables
-        if self.exchange == "owner":
-            e = mark("pull_exchange")
-            check(lib.b200ps_xchg_pull(h, self.uniq.data_ptr(), self.n_unique.data_ptr(), self.bet_d.data_ptr(),
-                                       self.bet_w.data_ptr(), st))
-            done(e)
-        elif self.paired:
-            e = mark("pull_pair")
-            for arr, ptrs, n in self.pull_pair:
-                check(lib.b200ps_pull_rows_pair(h, arr, ptrs, n, st))
-            done(e)
-        else:
-            for name, (arr, n) in zip(self.pull_names, self.pull_segs):
-                e = mark(name)
-                check(lib.b200ps_pull_rows(h, arr, n, st))
+        # (3) pull the unique rows of all 76 tables (row_source "table": the tower reads them from the tables)
+        if self.row_source == "pull":
+            if self.exchange == "owner":
+                e = mark("pull_exchange")
+                check(lib.b200ps_xchg_pull(h, self.uniq.data_ptr(), self.n_unique.data_ptr(), self.bet_d.data_ptr(),
+                                           self.bet_w.data_ptr(), st))
                 done(e)
+            elif self.paired:
+                e = mark("pull_pair")
+                for arr, ptrs, n in self.pull_pair:
+                    check(lib.b200ps_pull_rows_pair(h, arr, ptrs, n, st))
+                done(e)
+            else:
+                for name, (arr, n) in zip(self.pull_names, self.pull_segs):
+                    e = mark(name)
+                    check(lib.b200ps_pull_rows(h, arr, n, st))
+                    done(e)
         if branch:
             main.wait_event(ev_prep)
             rc = lib.b200_deepfm_tile_main(_ct.byref(a), st)
@@ -725,6 +770,9 @@ class DeepFMPSEngine:
             cur = self.cur
             ws = torch.zeros(lib.b200ps_unique_workspace(self.G, self.B), dtype=torch.uint8, device=self.device)
             plan = self._make_plan()
+            # predict() pulls its rows: with no push after it, the pull is what marks rows as created on first
+            # read (embedding_table.go:41-58)
+            plan["tower_args"].rows = None
             self._use(cur)
             self._predict_state = (ws, plan)
         ws, plan = self._predict_state
@@ -764,7 +812,9 @@ class DeepFMPSEngine:
                 "push": U * (8 + 4 * 1 + (1 + opt_slots) * 8 * 1) + U * (8 + 4 * D + (1 + opt_slots) * 8 * D),
                 # tower: per (sample, group) one rank read + one deep row + one wide value gathered, the
                 # embedding gradient scattered back (reduced per unique id), + the dense inputs / labels
-                "tower_fwd_bwd": k * (4 + 4 * D + 4) + U * (4 * D + 4) + self.B * 4 * (N_DENSE + 1),
+                # (row_source "table": + the low word of the row's id)
+                "tower_fwd_bwd": k * (4 + 4 * D + 4 + (4 if self.row_source == "table" else 0)) + U * (4 * D + 4)
+                + self.B * 4 * (N_DENSE + 1),
                 "pull_pair": U * (8 + 8 * D + 8 * 1), "pull_exchange": U * (8 + 8 * D + 8 * 1),
                 "push_exchange": U * (8 + 4 * D + 4 * 1 + (1 + opt_slots) * 8 * (D + 1)),
                 "push_pair": U * (8 + 4 * D + 4 * 1 + (1 + opt_slots) * 8 * (D + 1)),

@@ -30,6 +30,19 @@ extern "C" {
 #define B200_DEEPFM_H1 16
 #define B200_DEEPFM_H2 4
 #define B200_DEEPFM_SCRATCH 44 /* floats of per-sample backward state */
+#define B200_DEEPFM_TILE_MAXG 38 /* id groups the tile tower holds */
+
+/* Where the tile tower reads its embedding rows when they are not pulled into bet_wide / bet_deep first:
+ * straight from the parameter server's direct-indexed record slabs (b200ps_table_rows_ptr).  The row of
+ * sample b in group g is the record of id uniq[g*B + inv[g*B + b]]; the ids are those the dedup wrote, so
+ * they are inside their table.  Deep records must be 16-byte aligned (base, stride and param offset). */
+typedef struct {
+  const int64_t* uniq;                           /* [G][B] unique ids of each group (device) */
+  const float* deep_base[B200_DEEPFM_TILE_MAXG]; /* record slab of group g's deep (dim 8) table */
+  const float* wide_base[B200_DEEPFM_TILE_MAXG]; /* record slab of group g's wide (dim 1) table */
+  int64_t deep_stride, wide_stride;              /* floats between consecutive records, same for every group */
+  int64_t deep_param_off, wide_param_off;        /* float offset of the parameter row inside a record */
+} b200_deepfm_rows_t;
 
 typedef struct {
   int32_t G;               /* id groups */
@@ -47,6 +60,9 @@ typedef struct {
   float* loss;             /* [1] mean binary cross entropy with logits */
   float* logits;           /* [B] or NULL */
   float* scratch;          /* B*B200_DEEPFM_SCRATCH + 16*(13+8G) floats: per-sample backward state, then W1^T */
+  const b200_deepfm_rows_t* rows; /* host struct or NULL.  Set: the tile tower's training entry points read the
+                                     rows from the tables and bet_wide / bet_deep are not used; the other
+                                     towers and the forward-only entry points refuse it (-1). */
 } b200_deepfm_args_t;
 
 size_t b200_deepfm_param_count(int G);

@@ -216,6 +216,13 @@ int b200ps_push_end_shard(b200ps_t* ps, int shard, void* stream);
  * id (shares the table id space).  raw_ptr: its address on `shard` as mapped on the client device. */
 int b200ps_raw_register(b200ps_t* ps, const char* name, size_t bytes);
 int b200ps_raw_ptr(b200ps_t* ps, int table, int shard, void** ptr, size_t* bytes);
+/* The record slab of a direct-indexed embedding table on `shard`, as mapped on the client device: slot s of
+ * the shard's records is at base + s * row_stride floats, its parameter row param_off floats further; rows =
+ * records on the shard.  For readers that gather rows themselves (b200_deepfm_rows_t).  Such a read does not
+ * mark a row as created; a push of the row does.  B200PS_EINVAL for hashed tables, dense parameters and raw
+ * buffers. */
+int b200ps_table_rows_ptr(b200ps_t* ps, int table, int shard, float** base, int64_t* row_stride, int64_t* param_off,
+                          int64_t* rows);
 int b200ps_barrier(b200ps_t* ps, void* stream);
 /* step++ only (a failed ApplyGradients still bumps it, quirk Q2). */
 int b200ps_bump_step(b200ps_t* ps, void* stream);
