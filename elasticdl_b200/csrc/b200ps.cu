@@ -440,34 +440,26 @@ int for_each_class(b200ps_t* ps, Split& sp, F&& launch) {
 // scan -> barrier) and the launch ramp again.  Sized for 8 blocks per SM the 48-register kernels (5 resident)
 // would run 1.6 waves, so the grid follows cudaOccupancyMaxActiveBlocksPerMultiprocessor of the kernel actually
 // launched.
-// U rows in flight per thread only once the work is several times what the resident threads cover.
-void flat_shape(b200ps_t* ps, long long items, int* U, int* grid, bool copy = false) {
-  static const int force_u = [] { const char* e = getenv("B200_FLAT_U"); return e ? atoi(e) : 0; }();      // tuning knobs
+// U rows in flight per thread only once the work is several times what the resident threads cover.  (U = 4
+// measured slower: its 80 registers cost more resident warps than the unroll adds.)
+int flat_u(b200ps_t* ps, long long items) {
   const long long resident1 = (long long)ps->n_sm * 6 * 256;  // about what the U = 1 kernels keep resident
-  *U = items >= resident1 * 8 ? 2 : 1;
-  // (U = 4 is reachable through B200_FLAT_U only: its 80 registers cost more resident warps than the unroll adds.)
-  if (force_u == 1 || force_u == 2 || (copy && force_u == 4)) *U = force_u;
-  *grid = 0;  // set by flat_grid() for the kernel instance that is launched
+  return items >= resident1 * 8 ? 2 : 1;
 }
 
 // blocks of `kern` (256 threads, no dynamic shared memory) resident on the whole device
 template <typename K>
 int flat_grid(b200ps_t* ps, K kern, long long items, int U) {
-  static const int per_sm = [] { const char* e = getenv("B200_FLAT_BLOCKS"); return e ? atoi(e) : 0; }();
   static std::mutex mu;
   static std::unordered_map<const void*, int> occ;
-  int o = per_sm;
-  if (o <= 0) {
-    std::lock_guard<std::mutex> lk(mu);
-    auto it = occ.find((const void*)kern);
-    if (it == occ.end()) {
-      int v = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 256, 0) != cudaSuccess || v < 1) v = 4;
-      it = occ.emplace((const void*)kern, v).first;
-    }
-    o = it->second;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = occ.find((const void*)kern);
+  if (it == occ.end()) {
+    int v = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 256, 0) != cudaSuccess || v < 1) v = 4;
+    it = occ.emplace((const void*)kern, v).first;
   }
-  const long long cap = (long long)ps->n_sm * o;
+  const long long cap = (long long)ps->n_sm * it->second;
   long long blocks = (items + 256LL * U - 1) / (256LL * U);
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
@@ -476,13 +468,6 @@ int flat_grid(b200ps_t* ps, K kern, long long items, int U) {
 
 #define DISPATCH_U(UVAL, ...)                          \
   switch (UVAL) {                                       \
-    case 2: { constexpr int U = 2; __VA_ARGS__; } break; \
-    default: { constexpr int U = 1; __VA_ARGS__; } break; \
-  }
-// the copy kernels also come with four rows in flight per thread (tuning knob B200_FLAT_U=4)
-#define DISPATCH_UC(UVAL, ...)                         \
-  switch (UVAL) {                                       \
-    case 4: { constexpr int U = 4; __VA_ARGS__; } break; \
     case 2: { constexpr int U = 2; __VA_ARGS__; } break; \
     default: { constexpr int U = 1; __VA_ARGS__; } break; \
   }
@@ -907,42 +892,20 @@ static int rows_copy(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
   if (rc) return rc;
   GroupView gv = group_view(ps);
   cudaStream_t st = (cudaStream_t)stream;
-  // The shared-memory staged gather (cp.async in, one bulk async copy out per warp: bytes in flight bounded by
-  // shared memory instead of registers) is OPT-IN (B200_STAGED_MIN = lane-items from which it is taken): random
-  // 32 B sectors are bound by the memory system's request rate, not by bytes in flight, so the extra
-  // shared-memory round trip only costs (compare with tools/probes/gather_roof.cu).
-  const char* staged_env = getenv("B200_STAGED_MIN");
-  const long long staged_min = staged_env ? atoll(staged_env) : (1LL << 62);
-  if (sp.flat_n && !write && sp.flat_items >= staged_min) {
-    constexpr int SU = 8;
-    long long blocks = (sp.flat_items + 256LL * SU - 1) / (256LL * SU);
-    const long long cap = (long long)ps->n_sm * 4;
-    if (blocks > cap) blocks = cap;
+  if (sp.flat_n) {
+    const int u_rt = flat_u(ps, sp.flat_items);
+    int grid;
     if (ps->n_shards == 1) {
       FlatArgs<1> fa;
       fill_flat(ps, sp, false, slot, &fa);
-      k_pull_staged<SU, 1><<<(unsigned)blocks, 256, 0, st>>>(fa);
-    } else {
-      FlatArgs<8> fa;
-      fill_flat(ps, sp, false, slot, &fa);
-      k_pull_staged<SU, 8><<<(unsigned)blocks, 256, 0, st>>>(fa);
-    }
-    ps->launches++;
-    CUDA_OK(cudaGetLastError());
-  } else if (sp.flat_n) {
-    int u_rt, grid;
-    flat_shape(ps, sp.flat_items, &u_rt, &grid, true);
-    if (ps->n_shards == 1) {
-      FlatArgs<1> fa;
-      fill_flat(ps, sp, false, slot, &fa);
-      DISPATCH_UC(u_rt, {
+      DISPATCH_U(u_rt, {
         if (write) { grid = flat_grid(ps, k_copy_flat<true, U, 1>, sp.flat_items, U); k_copy_flat<true, U, 1><<<grid, 256, 0, st>>>(fa); }
         else { grid = flat_grid(ps, k_copy_flat<false, U, 1>, sp.flat_items, U); k_copy_flat<false, U, 1><<<grid, 256, 0, st>>>(fa); }
       });
     } else {
       FlatArgs<8> fa;
       fill_flat(ps, sp, false, slot, &fa);
-      DISPATCH_UC(u_rt, {
+      DISPATCH_U(u_rt, {
         if (write) { grid = flat_grid(ps, k_copy_flat<true, U, 8>, sp.flat_items, U); k_copy_flat<true, U, 8><<<grid, 256, 0, st>>>(fa); }
         else { grid = flat_grid(ps, k_copy_flat<false, U, 8>, sp.flat_items, U); k_copy_flat<false, U, 8><<<grid, 256, 0, st>>>(fa); }
       });
@@ -1043,8 +1006,8 @@ int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
   cudaStream_t st = (cudaStream_t)stream;
   OptParams o = ps->opt;
   if (sp.flat_n) {
-    int u_rt, grid;
-    flat_shape(ps, sp.flat_items, &u_rt, &grid);
+    const int u_rt = flat_u(ps, sp.flat_items);
+    int grid;
     if (ps->n_shards == 1) {
       FlatArgs<1> fa;
       fill_flat(ps, sp, true, 0, &fa);
@@ -1207,8 +1170,7 @@ static int xview(b200ps_t* ps, XView* x) {
 // The owner-side constants of the exchanged table pairs on MY shard, for the fast exchange kernels.  false: some
 // table is hashed / owned by one shard / not allocated here -> the generic kernels run instead.
 static bool xtabs(b200ps_t* ps, XTabs* t) {
-  static const bool off = [] { const char* e = getenv("B200_XCHG_FAST"); return e && atoi(e) == 0; }();
-  if (off || ps->x_G > kXMaxG) return false;
+  if (ps->x_G > kXMaxG) return false;
   const int me = ps->x_me;
   t->shard_shift = -1;
   if ((ps->n_shards & (ps->n_shards - 1)) == 0) {
@@ -1237,14 +1199,9 @@ static bool xtabs(b200ps_t* ps, XTabs* t) {
   return true;
 }
 
-// grid.x per peer
+// grid.x per peer: 4 blocks per SM over all peers
 static int xchg_per_peer(b200ps_t* ps) {
-  static const int mult = [] {
-    const char* e = getenv("B200_XCHG_BLOCKS");  // blocks per SM over all peers (tuning knob)
-    const int m = e ? atoi(e) : 4;
-    return m < 1 ? 1 : m;
-  }();
-  const int v = ps->n_sm * mult / ps->n_shards;
+  const int v = ps->n_sm * 4 / ps->n_shards;
   return v < 2 ? 2 : v;
 }
 
@@ -1639,15 +1596,14 @@ static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int6
   URuns ur{};
   const long long ups = a.ntiles;
   long long blocks = 0;
-  // segments with a small id range go to k_unique_small: one block each, position array in shared memory
-  // (B200_UNIQUE_SMALL=<largest id range taken by k_unique_small>, 0 = off)
-  const int small_max = [] { const char* e = getenv("B200_UNIQUE_SMALL"); const int v = e ? atoi(e) : kUSmallMax; return v > kUSmallMax ? kUSmallMax : v; }();
+  // segments with an id range of at most kUSmallMax go to k_unique_small: one block each, position array in
+  // shared memory
   USmall us{};
   bool is_small[kMaxSegs] = {};
   int small_bound = 0;
   if (a.use_bounds && T <= kMaxSegs && k <= 32LL * kUSThreads) {
     for (int t = 0; t < T; ++t) {
-      if (a.ub.bound[t] > 0 && a.ub.bound[t] <= small_max) {
+      if (a.ub.bound[t] > 0 && a.ub.bound[t] <= kUSmallMax) {
         is_small[t] = true;
         us.seg[us.n++] = t;
         if (a.ub.bound[t] > small_bound) small_bound = a.ub.bound[t];

@@ -12,7 +12,6 @@
 // gather/scatter of embedding rows, not by math).
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <string>
 
 #include "../../include/b200_deepfm.h"
@@ -167,7 +166,7 @@ __device__ __forceinline__ void dot16x(float (&out)[NS], const float (&h)[NS][H1
   }
 }
 
-template <bool BACKWARD, int GC>  // GC = groups gathered per round per warp
+template <bool BACKWARD>
 __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a) {
   extern __shared__ __align__(16) float smem[];
   const Layout l = layout(a.G);
@@ -217,51 +216,37 @@ __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a)
 #pragma unroll
       for (int d = 0; d < D; ++d) s[n][d] = 0.f;
     }
-    // pass 1 over this warp's groups: GC*NS rank loads, then 3*GC*NS independent row loads in flight
-    for (int g0 = part; g0 < G; g0 += NPART * GC) {
-      int r[GC][NS];
+    // pass 1 over this warp's groups: NS rank loads, then 3*NS independent row loads in flight
+    for (int g = part; g < G; g += NPART) {
+      int r[NS];
 #pragma unroll
-      for (int u = 0; u < GC; ++u) {
-        const int g = g0 + u * NPART;
+      for (int n = 0; n < NS; ++n) r[n] = a.inv[(long long)g * B + bb[n]];
+      float4 e0[NS], e1[NS];
+      float wv[NS];
 #pragma unroll
-        for (int n = 0; n < NS; ++n) r[u][n] = g < G ? a.inv[(long long)g * B + bb[n]] : 0;
+      for (int n = 0; n < NS; ++n) {
+        const float4* row = reinterpret_cast<const float4*>(a.bet_deep + ((long long)g * B + r[n]) * D);
+        e0[n] = row[0];
+        e1[n] = row[1];
+        wv[n] = a.bet_wide[(long long)g * B + r[n]];
       }
-      float4 e0[GC][NS], e1[GC][NS];
-      float wv[GC][NS];
+      const float* w = sp.w1t + (ND + g * D) * H1;
+      float ev[D][NS];
 #pragma unroll
-      for (int u = 0; u < GC; ++u) {
-        const int g = g0 + u * NPART < G ? g0 + u * NPART : part;
+      for (int n = 0; n < NS; ++n) {
+        sinv[g * SPB + sl0 + 32 * n] = r[n];
+        lin[n] += wv[n];
+        ev[0][n] = e0[n].x; ev[1][n] = e0[n].y; ev[2][n] = e0[n].z; ev[3][n] = e0[n].w;
+        ev[4][n] = e1[n].x; ev[5][n] = e1[n].y; ev[6][n] = e1[n].z; ev[7][n] = e1[n].w;
+      }
+#pragma unroll
+      for (int d = 0; d < D; ++d) {
 #pragma unroll
         for (int n = 0; n < NS; ++n) {
-          const float4* row = reinterpret_cast<const float4*>(a.bet_deep + ((long long)g * B + r[u][n]) * D);
-          e0[u][n] = row[0];
-          e1[u][n] = row[1];
-          wv[u][n] = a.bet_wide[(long long)g * B + r[u][n]];
+          s[n][d] += ev[d][n];
+          q[n] = fmaf(ev[d][n], ev[d][n], q[n]);
         }
-      }
-#pragma unroll
-      for (int u = 0; u < GC; ++u) {
-        const int g = g0 + u * NPART;
-        if (g < G) {
-          const float* w = sp.w1t + (ND + g * D) * H1;
-          float ev[D][NS];
-#pragma unroll
-          for (int n = 0; n < NS; ++n) {
-            sinv[g * SPB + sl0 + 32 * n] = r[u][n];
-            lin[n] += wv[u][n];
-            ev[0][n] = e0[u][n].x; ev[1][n] = e0[u][n].y; ev[2][n] = e0[u][n].z; ev[3][n] = e0[u][n].w;
-            ev[4][n] = e1[u][n].x; ev[5][n] = e1[u][n].y; ev[6][n] = e1[u][n].z; ev[7][n] = e1[u][n].w;
-          }
-#pragma unroll
-          for (int d = 0; d < D; ++d) {
-#pragma unroll
-            for (int n = 0; n < NS; ++n) {
-              s[n][d] += ev[d][n];
-              q[n] = fmaf(ev[d][n], ev[d][n], q[n]);
-            }
-            axpy16x(h, w + d * H1, ev[d]);
-          }
-        }
+        axpy16x(h, w + d * H1, ev[d]);
       }
     }
     // combine the NPART partial sums of each sample through shared memory
@@ -343,69 +328,60 @@ __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a)
     if (BACKWARD) {
       // pass 2: d loss / d embedding rows of this warp's groups, reduced per unique id
       // (deduplicate_indexed_slices' sum)
-      for (int g0 = part; g0 < G; g0 += NPART * GC) {
-        int r[GC][NS];
-        float4 e0[GC][NS], e1[GC][NS];
+      for (int g = part; g < G; g += NPART) {
+        int r[NS];
+        float4 e0[NS], e1[NS];
 #pragma unroll
-        for (int u = 0; u < GC; ++u) {
-          const int g = g0 + u * NPART < G ? g0 + u * NPART : part;
+        for (int n = 0; n < NS; ++n) {
+          r[n] = sinv[g * SPB + sl0 + 32 * n];
+          const float4* row = reinterpret_cast<const float4*>(a.bet_deep + ((long long)g * B + r[n]) * D);
+          e0[n] = row[0];
+          e1[n] = row[1];
+        }
+        const float* w = sp.w1t + (ND + g * D) * H1;
+        float x[NS][D + 1];
+        float ev[D][NS];
 #pragma unroll
-          for (int n = 0; n < NS; ++n) {
-            r[u][n] = sinv[g * SPB + sl0 + 32 * n];
-            const float4* row = reinterpret_cast<const float4*>(a.bet_deep + ((long long)g * B + r[u][n]) * D);
-            e0[u][n] = row[0];
-            e1[u][n] = row[1];
-          }
+        for (int n = 0; n < NS; ++n) {
+          ev[0][n] = e0[n].x; ev[1][n] = e0[n].y; ev[2][n] = e0[n].z; ev[3][n] = e0[n].w;
+          ev[4][n] = e1[n].x; ev[5][n] = e1[n].y; ev[6][n] = e1[n].z; ev[7][n] = e1[n].w;
         }
 #pragma unroll
-        for (int u = 0; u < GC; ++u) {
-          const int g = g0 + u * NPART;
-          if (g >= G) break;  // warp-uniform
-          const float* w = sp.w1t + (ND + g * D) * H1;
-          float x[NS][D + 1];
-          float ev[D][NS];
+        for (int d = 0; d < D; ++d) {
+          float dt[NS];
+          dot16x(dt, dh1, w + d * H1);
 #pragma unroll
-          for (int n = 0; n < NS; ++n) {
-            ev[0][n] = e0[u][n].x; ev[1][n] = e0[u][n].y; ev[2][n] = e0[u][n].z; ev[3][n] = e0[u][n].w;
-            ev[4][n] = e1[u][n].x; ev[5][n] = e1[u][n].y; ev[6][n] = e1[u][n].z; ev[7][n] = e1[u][n].w;
-          }
+          for (int n = 0; n < NS; ++n) x[n][d] = fmaf(dz[n], s[n][d] - ev[d][n], dt[n]);
+        }
 #pragma unroll
-          for (int d = 0; d < D; ++d) {
-            float dt[NS];
-            dot16x(dt, dh1, w + d * H1);
+        for (int n = 0; n < NS; ++n) {
+          x[n][D] = dz[n];  // wide row gradient
+          // warp-level id dedup: lanes hitting the same row combine pairwise up a tree threaded
+          // through the peer mask (pointer doubling), ceil(log2(max multiplicity)) rounds for the
+          // whole warp -- the small tables of this model put ~10 equal ids in every warp
+          const int key = live[n] ? r[n] : -1 - lane;
+          const unsigned peers = __match_any_sync(0xffffffffu, key);
+          const int rank = __popc(peers & ((1u << lane) - 1));
+          const bool leader = rank == 0;
+          const int maxn = __reduce_max_sync(0xffffffffu, (unsigned)__popc(peers));
+          const unsigned above = peers & ~((2u << lane) - 1);
+          int nxt = above ? __ffs(above) - 1 : -1;  // peer `step` ranks above me
+          for (int step = 1; step < maxn; step <<= 1) {
+            const int src = nxt >= 0 ? nxt : lane;
+            const bool take = nxt >= 0 && (rank & (2 * step - 1)) == 0;
 #pragma unroll
-            for (int n = 0; n < NS; ++n) x[n][d] = fmaf(dz[n], s[n][d] - ev[d][n], dt[n]);
-          }
-#pragma unroll
-          for (int n = 0; n < NS; ++n) {
-            x[n][D] = dz[n];  // wide row gradient
-            // warp-level id dedup: lanes hitting the same row combine pairwise up a tree threaded
-            // through the peer mask (pointer doubling), ceil(log2(max multiplicity)) rounds for the
-            // whole warp -- the small tables of this model put ~10 equal ids in every warp
-            const int key = live[n] ? r[u][n] : -1 - lane;
-            const unsigned peers = __match_any_sync(0xffffffffu, key);
-            const int rank = __popc(peers & ((1u << lane) - 1));
-            const bool leader = rank == 0;
-            const int maxn = __reduce_max_sync(0xffffffffu, (unsigned)__popc(peers));
-            const unsigned above = peers & ~((2u << lane) - 1);
-            int nxt = above ? __ffs(above) - 1 : -1;  // peer `step` ranks above me
-            for (int step = 1; step < maxn; step <<= 1) {
-              const int src = nxt >= 0 ? nxt : lane;
-              const bool take = nxt >= 0 && (rank & (2 * step - 1)) == 0;
-#pragma unroll
-              for (int e = 0; e <= D; ++e) {
-                const float yv = __shfl_sync(0xffffffffu, x[n][e], src);
-                if (take) x[n][e] += yv;
-              }
-              const int nn = __shfl_sync(0xffffffffu, nxt, src);
-              nxt = nxt >= 0 ? nn : -1;
+            for (int e = 0; e <= D; ++e) {
+              const float yv = __shfl_sync(0xffffffffu, x[n][e], src);
+              if (take) x[n][e] += yv;
             }
-            if (live[n] && leader) {
-              float* od = a.gsum_deep + ((long long)g * B + r[u][n]) * D;
-              atomicAdd(reinterpret_cast<float4*>(od), make_float4(x[n][0], x[n][1], x[n][2], x[n][3]));
-              atomicAdd(reinterpret_cast<float4*>(od + 4), make_float4(x[n][4], x[n][5], x[n][6], x[n][7]));
-              atomicAdd(a.gsum_wide + (long long)g * B + r[u][n], x[n][D]);
-            }
+            const int nn = __shfl_sync(0xffffffffu, nxt, src);
+            nxt = nxt >= 0 ? nn : -1;
+          }
+          if (live[n] && leader) {
+            float* od = a.gsum_deep + ((long long)g * B + r[n]) * D;
+            atomicAdd(reinterpret_cast<float4*>(od), make_float4(x[n][0], x[n][1], x[n][2], x[n][3]));
+            atomicAdd(reinterpret_cast<float4*>(od + 4), make_float4(x[n][4], x[n][5], x[n][6], x[n][7]));
+            atomicAdd(a.gsum_wide + (long long)g * B + r[n], x[n][D]);
           }
         }
       }
@@ -569,23 +545,16 @@ int b200_deepfm_fwd_bwd(const b200_deepfm_args_t* args, void* stream) {
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const size_t smem = tower_a_smem(args->G);
   static bool attr_done[64] = {false};
-  static int gc = 0;
-  if (gc == 0) {
-    const char* e = getenv("B200_TOWER_GC");  // tuning knob: row gathers in flight per lane
-    gc = (e && atoi(e) == 2) ? 2 : 1;
-  }
   if (dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(k_tower_a<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    cudaFuncSetAttribute(k_tower_a<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    cudaFuncSetAttribute(k_tower_a<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
+    cudaFuncSetAttribute(k_tower_a<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
+    cudaFuncSetAttribute(k_tower_a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
     attr_done[dev] = true;
   }
   dim3 gp(8, args->G);
   k_tower_prep<<<gp, 256, 0, st>>>(*args, l.total);
   long long blocks = ((long long)args->B + SPB - 1) / SPB;
   long long cap = (long long)n_sm * 8;
-  if (gc == 2) k_tower_a<true, 2><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
-  else k_tower_a<true, 1><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
+  k_tower_a<true><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
   long long chunks = ((long long)args->B + S_CHUNK - 1) / S_CHUNK;
   cap = (long long)n_sm * 4;  // 4 blocks per SM by shared memory / registers
   static bool attr_b[64] = {false};
@@ -608,10 +577,10 @@ int b200_deepfm_forward(const b200_deepfm_args_t* args, void* stream) {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const size_t smem = tower_a_smem(args->G);
-  cudaFuncSetAttribute(k_tower_a<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
+  cudaFuncSetAttribute(k_tower_a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
   long long blocks = ((long long)args->B + SPB - 1) / SPB;
   long long cap = (long long)n_sm * 8;
-  k_tower_a<false, 1><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
+  k_tower_a<false><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
   g_launches += 1;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }

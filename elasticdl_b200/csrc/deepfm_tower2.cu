@@ -27,7 +27,6 @@
 // a 3xTF32 mma.sync version of F / B1 / B2 measured slower).
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <string>
 
 #include "../../include/b200_deepfm.h"
@@ -560,8 +559,7 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
   if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
   float* w1x = a.scratch;  // NCOL*16 floats at the start of the scratch buffer, then the tile counter
   const long long ntile = ((long long)a.B + TS - 1) / TS;
-  static const int per_sm = [] { const char* e = getenv("B200_TILE_CTAS"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
-  long long grid = (long long)n_sm * per_sm;
+  long long grid = (long long)n_sm * 2;  // the 2 CTAs per SM of k_tower_tile's __launch_bounds__
   if (grid > ntile) grid = ntile;
   if (what & 1) {
     k_tile_prep<<<dim3(4, BACKWARD ? a.G : 1), 256, 0, st>>>(a, layout(a.G).total, w1x, (int)grid);

@@ -17,7 +17,6 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <cstdlib>
 #include <string>
 
 #include "../../include/b200_deepfm.h"
@@ -101,8 +100,8 @@ long long g_launches_mma = 0;
 //   A (16x8, row): a0 (gid, tig)  a1 (gid+8, tig)  a2 (gid, tig+4)  a3 (gid+8, tig+4)
 //   B ( 8x8, col): b0 (k = tig, n = gid)  b1 (k = tig+4, n = gid)
 //   C (16x8):      c0 (gid, 2 tig)  c1 (gid, 2 tig+1)  c2 (gid+8, 2 tig)  c3 (gid+8, 2 tig+1)
-template <bool BACKWARD, int MIN_CTAS>  // MIN_CTAS resident CTAs per SM bound the register allocation
-__global__ void __launch_bounds__(THREADS, MIN_CTAS) k_tower_mma(b200_deepfm_args_t a) {
+template <bool BACKWARD>  // 2 resident CTAs per SM: up to 255 registers (3 would cap them at 168)
+__global__ void __launch_bounds__(THREADS, 2) k_tower_mma(b200_deepfm_args_t a) {
   extern __shared__ __align__(16) float smem[];
   const int G = a.G, B = a.B;
   const Layout l = layout(G);
@@ -444,18 +443,11 @@ int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
   const size_t smem = mma_smem_bytes(a->G);
   static bool attr_done[64] = {false};
   static int per_sm[64] = {0};
-  static int min_ctas = 0;
-  if (min_ctas == 0) {
-    const char* e = getenv("B200_MMA_MIN_CTAS");  // tuning knob: 2 (up to 255 registers) or 3 (<= 168)
-    min_ctas = (e && atoi(e) == 3) ? 3 : 2;
-  }
   if (smem > 100 * 1024) return -1;
   if (dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(k_tower_mma<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(k_tower_mma<true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    cudaFuncSetAttribute(k_tower_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     int nb = 0;
-    cudaError_t e = min_ctas == 3 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tower_mma<true, 3>, THREADS, smem)
-                                  : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tower_mma<true, 2>, THREADS, smem);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tower_mma<true>, THREADS, smem);
     if (e != cudaSuccess || nb < 1) nb = 1;
     per_sm[dev] = nb;
     attr_done[dev] = true;
@@ -465,8 +457,7 @@ int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
   const long long nchunk = ((long long)a->B + MT - 1) / MT;
   const long long cap = (long long)n_sm * (dev < 64 ? per_sm[dev] : 1);
   const unsigned grid = (unsigned)(nchunk < cap ? nchunk : cap);
-  if (min_ctas == 3) k_tower_mma<true, 3><<<grid, THREADS, smem, st>>>(*a);
-  else k_tower_mma<true, 2><<<grid, THREADS, smem, st>>>(*a);
+  k_tower_mma<true><<<grid, THREADS, smem, st>>>(*a);
   g_launches_mma += 2;
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }

@@ -248,108 +248,6 @@ __global__ void __launch_bounds__(256) k_copy_flat(const __grid_constant__ FlatA
 }
 
 // ---------------------------------------------------------------------------
-// pull, staged through shared memory (the gather of PullEmbeddingVectors at scale): every lane issues U
-// 16 B cp.async copies (LDGSTS: HBM -> shared memory, no register holds the data while it is in flight)
-// into its warp's staging slice, laid out in item order -- which is also the order of the user's output
-// rows -- and one elected lane then writes the whole slice back with ONE 1-D bulk async copy per
-// contiguous run (cp.async.bulk.global.shared::cta: the TMA engine streams shared memory to HBM, SASS
-// UBLKCP).  Bytes in flight per SM are bounded by shared memory (U * 512 B per warp), not by registers:
-// U = 8 keeps 4 KB per warp in flight where the register path held 1 KB.
-// Segments that are not vectorisable (dim % 4 != 0, unaligned rows) take the direct 4-byte path in the same
-// launch; a warp that meets an out-of-range id falls back to per-lane stores from the staging slice.
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ void cp_async16_flat(void* smem, const void* gmem) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void bulk_store(void* gmem, const void* smem, unsigned bytes) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem), "r"(s), "r"(bytes) : "memory");
-}
-
-template <int U, int NSMAX>
-__global__ void __launch_bounds__(256) k_pull_staged(const __grid_constant__ FlatArgs<NSMAX> p) {
-  __shared__ long long prefix[kMaxSegs + 1];
-  __shared__ __align__(128) float4 stage[8][32 * U];  // per warp: U * 512 B, item order
-  flat_prefix(p, prefix);
-  const int nseg = p.nseg;
-  const long long total = prefix[nseg];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  float4* mine = stage[wid];
-  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long long nwarp = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long wb = warp * (32 * U); wb < total; wb += nwarp * (32 * U)) {
-    const long long w0 = wb + lane;
-    int seg = flat_seg_of(prefix, nseg, w0 < total ? w0 : total - 1);
-    FlatItem it[U];
-    long long id[U];
-#pragma unroll
-    for (int k = 0; k < U; ++k) {
-      it[k] = flat_item(p, prefix, wb + k * 32 + lane, total, seg);
-      id[k] = it[k].live ? p.seg[it[k].seg].ids[it[k].row] : 0;
-    }
-    uint32_t* pres[U];
-    uint32_t bit[U];
-    bool bad = false;
-#pragma unroll
-    for (int k = 0; k < U; ++k) {
-      pres[k] = nullptr;
-      bit[k] = 0;
-      if (!it[k].live) continue;
-      const FlatSegP& sp = p.seg[it[k].seg];
-      const FlatLoc loc = flat_locate(p, it[k].seg, id[k]);
-      if (!loc.ok) {
-        if (it[k].col == 0) atomicOr(p.err, kErrRange);
-        bad = true;
-        it[k].live = false;
-        continue;
-      }
-      if (sp.vec) {
-        cp_async16_flat(&mine[k * 32 + lane], loc.rec + sp.soff[p.slot] + 4 * it[k].col);
-      } else {  // scalar segment: straight through
-        st_f1(sp.rows + it[k].row * sp.dim + it[k].col, ld_f1(loc.rec + sp.soff[p.slot] + it[k].col));
-      }
-      if (it[k].col == 0) { pres[k] = loc.pres; bit[k] = loc.bit; }
-    }
-    // created-row bitmap: all reads first, then the (rare) sets
-    uint32_t word[U];
-#pragma unroll
-    for (int k = 0; k < U; ++k) word[k] = pres[k] ? *(volatile uint32_t*)pres[k] : 0xffffffffu;
-#pragma unroll
-    for (int k = 0; k < U; ++k)
-      if (pres[k] && !(word[k] & bit[k])) atomicOr_system(pres[k], bit[k]);
-    asm volatile("cp.async.wait_all;" ::: "memory");
-    const bool any_bad = __any_sync(0xffffffffu, bad);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // my generic-proxy view of the staged data -> async proxy
-    __syncwarp();
-    if (!any_bad) {
-      if (lane == 0) {  // one bulk copy per run of consecutive items of a vectorisable segment
-        long long w = wb;
-        const long long wend = wb + 32 * U < total ? wb + 32 * U : total;
-        int sg = flat_seg_of(prefix, nseg, w);
-        while (w < wend) {
-          while (w >= prefix[sg + 1]) ++sg;
-          const long long rend = prefix[sg + 1] < wend ? prefix[sg + 1] : wend;
-          const FlatSegP& sp = p.seg[sg];
-          if (sp.vec) bulk_store(sp.rows + (w - prefix[sg]) * 4, &mine[w - wb], (unsigned)((rend - w) * 16));
-          w = rend;
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the slice is reused by the next iteration
-      }
-    } else {  // some id of this warp was out of range: per-lane stores of the rows that did arrive
-#pragma unroll
-      for (int k = 0; k < U; ++k) {
-        if (!it[k].live) continue;
-        const FlatSegP& sp = p.seg[it[k].seg];
-        if (sp.vec) st_f4(sp.rows + it[k].row * sp.dim + 4 * it[k].col, mine[k * 32 + lane]);
-      }
-    }
-    __syncwarp();
-  }
-}
-
-// ---------------------------------------------------------------------------
 // push: lane = (row, column).  dim-1 tables whose record is one float4 [p, s0, s1, s2] keep the
 // single 16 B access.
 // ---------------------------------------------------------------------------

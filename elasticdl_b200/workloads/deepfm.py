@@ -298,8 +298,6 @@ class DeepFMPSEngine:
             gen = torch.Generator(device=dev).manual_seed(seed)
             for names, dim in ((self.wide_names, 1), (self.deep_names, D)):
                 for n, r in zip(names, group_rows):
-                    if r % group.n_shards and group.n_shards > 1:
-                        pass
                     ids = torch.arange(r, device=dev)
                     if len(group.local_shards) != group.n_shards:
                         # multi-process: every rank initialises the rows it owns
@@ -331,10 +329,6 @@ class DeepFMPSEngine:
         self.id_transport = id_transport
         self.widths = id_widths(group_rows) if id_transport == "narrow" else [4] * G
         self._c_widths = (_ctb.c_int32 * G)(*self.widths)
-        import os as _os
-
-        self.lookahead_blocks_per_sm = int(_os.environ.get("B200_LOOKAHEAD_UNIQUE_BLOCKS", "0"))
-        self.lookahead_fork = _os.environ.get("B200_LOOKAHEAD_FORK", "push")  # "push" | "start" (tuning knob)
         self.bet_w = torch.zeros((G * B, 1), **f32)
         self.bet_d = torch.zeros((G * B, D), **f32)
         self.act_w = torch.empty((G * B, 1), **f32)
@@ -358,7 +352,6 @@ class DeepFMPSEngine:
         self.cur = 0
         self.side = None
         self.aux = None  # second stream of the branched step (see step())
-        self.branch = _os.environ.get("B200_STEP_BRANCHES", "1") != "0"
         self.graph = None
         self.graphs_ahead = None
         if self.exchange == "owner":
@@ -483,7 +476,7 @@ class DeepFMPSEngine:
         # while the main stream carries unique -> pull -> tower -> push rows:
         #   aux:  pull_dense -> push_begin -> tower prologue  | joined before the tower
         #   aux:  push_dense                                   | beside the row push, joined before push_end
-        branch = self.branch and self.tower_kind == "tile" and ev is None
+        branch = self.tower_kind == "tile" and ev is None
         main = torch.cuda.current_stream(self.device)
         if branch:
             if self.aux is None:
@@ -599,19 +592,19 @@ class DeepFMPSEngine:
         the device has finished that step (synchronize / event) and for the last LOSS_RING steps."""
         return float(self.loss_ring[step_index % self.LOSS_RING])
 
-    def _unique_into(self, ids, blocks_per_sm=0):
-        """tf.unique per id group into the current plan, on the current stream.  blocks_per_sm > 0: a thin
-        persistent grid (the lookahead pipeline runs the dedup beside the training kernels)."""
+    def _unique_into(self, ids):
+        """tf.unique per id group into the current plan, on the current stream (the library's default grid:
+        blocks_per_sm = 0)."""
         g = self.group
         if ids.dtype == torch.uint8:  # the id region of a packed batch with per-group widths
             check(g.lib.b200ps_unique_packed(g._h, ids.data_ptr(), self._c_widths, self.G, self.B, self.bounds,
                                              self.uniq.data_ptr(), self.inv.data_ptr(), self.n_unique.data_ptr(),
-                                             self.ws.data_ptr(), self.ws.numel(), int(blocks_per_sm), g._stream()))
+                                             self.ws.data_ptr(), self.ws.numel(), 0, g._stream()))
             return
         check(g.lib.b200ps_unique_bounded_ex(g._h, ids.data_ptr(), 1 if ids.dtype == torch.int32 else 0, self.G, self.B,
                                              self.bounds, self.uniq.data_ptr(), self.inv.data_ptr(),
-                                             self.n_unique.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                                             int(blocks_per_sm), g._stream()))
+                                             self.n_unique.data_ptr(), self.ws.data_ptr(), self.ws.numel(), 0,
+                                             g._stream()))
 
     # ------------------------------------------------------------------ lookahead pipeline
     def _ensure_plans(self):
@@ -645,12 +638,10 @@ class DeepFMPSEngine:
             self.side.wait_stream(main)  # the other plan's buffers were last read by the previous step
             self._use(1 - p)
             with torch.cuda.stream(self.side):
-                self._unique_into(next_ids, blocks_per_sm=self.lookahead_blocks_per_sm)
+                self._unique_into(next_ids)
             self._use(p)
 
-        if self.lookahead_fork != "push":
-            fork()  # "start": beside the whole step
-        loss = self.step(None, dense, labels, ev=ev, after_tower=fork if self.lookahead_fork == "push" else None)
+        loss = self.step(None, dense, labels, ev=ev, after_tower=fork)
         main.wait_stream(self.side)  # join
         self._use(1 - p)
         return loss

@@ -992,13 +992,12 @@ def test_unique_packed_per_segment_id_widths():
 
 
 @pytest.mark.parametrize("n_shards", [1, 2])
-def test_staged_pull_large_gather_bit_exact(n_shards, monkeypatch):
-    """The shared-memory staged gather (cp.async in, bulk async copy out; opt-in through B200_STAGED_MIN) returns
-    exactly the table rows: mixed dims (8, 64 staged; 1, 10 direct) in one launch, ragged warp tails, device-side
-    counts, and an out-of-range id (that warp falls back to per-lane stores, the error is raised)."""
+def test_large_mixed_dim_pull_bit_exact(n_shards):
+    """A large flat pull (k_copy_flat) returns exactly the table rows: mixed dims (8, 64 in 16 B chunks; 1, 10 in
+    floats) in one launch, ragged warp tails, device-side counts, and an out-of-range id (every other row still
+    arrives, the error is raised)."""
     from elasticdl_b200 import _lib
 
-    monkeypatch.setenv("B200_STAGED_MIN", "100000")
     group, client, _ = make_pair(n_shards, "adam")
     rng = np.random.RandomState(9)
     dims, caps = [8, 64, 1, 10], [300_000, 200_000, 50_000, 5_000]
@@ -1021,7 +1020,7 @@ def test_staged_pull_large_gather_bit_exact(n_shards, monkeypatch):
         keep.append((ids, nl, rows, t_ids, n_dev))
         items.append((group.lookup(n_)[0], m, t_ids, n_dev, rows))
     arr, nseg = group.make_segs(items)
-    _lib.check(lib.b200ps_pull_rows(h, arr, nseg, group._stream()))  # 0.6 M + 3.2 M + ... lane-items: the staged kernel
+    _lib.check(lib.b200ps_pull_rows(h, arr, nseg, group._stream()))  # 0.6 M + 3.2 M + ... lane-items
     group.check()
     for (ids, nl, rows, _, _), n_ in zip(keep, names):
         got = rows.cpu().numpy()
@@ -1068,8 +1067,8 @@ def test_wide_rows_big_gather(n_shards):
 
 
 @pytest.mark.parametrize("k", [700, 9000, 32768])
-def test_unique_small_segments_in_shared_memory(k, monkeypatch):
-    """B200_UNIQUE_SMALL: segments whose id range fits a shared-memory position array are deduplicated by one
+def test_unique_small_segments_in_shared_memory(k):
+    """Segments whose id range fits a shared-memory position array (kUSmallMax = 16384) are deduplicated by one
     block each (k_unique_small, ids in registers: 8 / 16 / 32 per thread), the others by the grid-wide kernel --
     same first-occurrence order, inverse index and counts as tf.unique, over several calls (epochs of the
     grid-wide kernel) and with out-of-range ids (counted as id 0 AND reported through the group's error word)."""
@@ -1077,7 +1076,6 @@ def test_unique_small_segments_in_shared_memory(k, monkeypatch):
 
     from elasticdl_b200 import _lib
 
-    monkeypatch.setenv("B200_UNIQUE_SMALL", "16384")
     group, _, _ = make_pair(1)
     lib = _lib.lib()
     rng = np.random.RandomState(33)
