@@ -9,6 +9,7 @@ import os
 
 from elasticdl_b200 import build as _build
 
+ABI_VERSION = 2  # B200PS_ABI_VERSION of include/b200ps.h
 MAX_SHARDS = 16
 MAX_SEGS = 96
 
@@ -97,7 +98,7 @@ SYMBOLS = {
     "b200ps_push_begin": (_i, [_vp, _f, ctypes.POINTER(ctypes.c_int32), _vp]),
     "b200ps_push_rows": (_i, [_vp, _segp, _i, _vp]),
     "b200ps_push_dense": (_i, [_vp, _segp, _i, _vp]),
-    "b200ps_push_dense_reduce": (_i, [_vp, _i, ctypes.POINTER(_vp), _i, _f, _vp]),
+    "b200ps_push_dense_reduce": (_i, [_vp, _i, ctypes.POINTER(_vp), _i, _f, _i, _vp]),
     "b200ps_push_end": (_i, [_vp, _vp, _vp]),
     "b200ps_bump_step": (_i, [_vp, _vp]),
     "b200ps_push_begin_shard": (_i, [_vp, _i, _f, ctypes.POINTER(ctypes.c_int32), _vp]),
@@ -171,8 +172,9 @@ def lib():
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args
-        if handle.b200ps_abi_version() != 1:
-            raise ImportError("libb200ps.so ABI version mismatch")
+        if handle.b200ps_abi_version() != ABI_VERSION:
+            raise ImportError("libb200ps.so ABI version %d, this package needs %d: rebuild it"
+                              % (handle.b200ps_abi_version(), ABI_VERSION))
         _lib = handle
     return _lib
 

@@ -295,10 +295,15 @@ int alloc_table_on_shard(b200ps_t* ps, Table& t, int s, int table_id) {
     a.is_dense = 1;
     a.seed = t.seed ^ (0x9E3779B97F4A7C15ULL * (uint64_t)(s + 1));
   }
+  // a pair's record section is [A(8) | B(1) | pad(3)]: A's and B's columns are initialised together as 9
+  // columns, the pads are zeroed with the rest of the slab
+  const bool pair = t.pair_b >= 0;
+  if (pair) a.dim = 9;
   bool need_kernel = !t.raw && (t.uniform || (ps->opt.kind == kFTRL && ps->opt.init_accum != 0.0f));
   if (need_kernel) {
-    if (t.bytes > t.present_off && t.present_off) CUDA_OK(cudaMemsetAsync((char*)p + t.present_off, 0, t.bytes - t.present_off, 0));
-    long long work = t.rows * (long long)t.dim * (t.n_slots + 1);
+    if (pair) CUDA_OK(cudaMemsetAsync(p, 0, t.bytes, 0));
+    else if (t.bytes > t.present_off && t.present_off) CUDA_OK(cudaMemsetAsync((char*)p + t.present_off, 0, t.bytes - t.present_off, 0));
+    long long work = t.rows * (long long)a.dim * (t.n_slots + 1);
     k_init_rows<<<grid_for(ps, work), 256>>>(a);
     ps->launches++;
     CUDA_OK(cudaGetLastError());
@@ -1377,11 +1382,12 @@ int b200ps_push_dense(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* st
 }
 
 int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* grads_dev, int n_replicas, float scale,
-                             void* stream) {
+                             int divide, void* stream) {
   int rc = ready(ps);
   if (rc) return rc;
   if (dense_id < 0 || dense_id >= (int)ps->tables.size() || !ps->tables[dense_id].is_dense) return fail(B200PS_ENOTFOUND, "not a dense parameter");
   if (n_replicas < 1 || n_replicas > kMaxShards || !grads_dev) return fail(B200PS_EINVAL, "n_replicas out of range");
+  if (divide && scale == 0.0f) return fail(B200PS_EINVAL, "divisor is zero");
   DeviceGuard g(ps->client_device);
   const Table& t = ps->tables[dense_id];
   ReplicaGrads rg{};
@@ -1392,6 +1398,7 @@ int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* gra
   }
   rg.n = n_replicas;
   rg.scale = scale;
+  rg.divide = divide ? 1 : 0;
   long long numel = t.rows * t.dim;
   GroupView gv = group_view(ps);
   cudaStream_t st = (cudaStream_t)stream;

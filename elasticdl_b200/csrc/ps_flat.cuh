@@ -1,7 +1,8 @@
 // Flat-scheduled row kernels (round 2): pull / set / push for every direct-indexed table and
 // dense-parameter row view, any dim, up to kMaxSegs (table, ids) segments in ONE launch.
 //
-// Why they replace the per-segment grids of ps_kernels.cuh (k_rows_copy_d8 / k_push_rows_d8 / _d1):
+// Why one flat launch rather than one grid row per segment (blockIdx.y = segment, as the hashed-table kernels
+// k_rows_copy / k_push_rows of ps_kernels.cuh still run):
 //   * a DeepFM step addresses 76 tables whose live sizes (device-side unique counts) range from 3 to
 //     25 000 rows.  blockIdx.y = segment gave the big segments 3+ grid-stride passes of dependent
 //     latencies while the blocks of the small ones exited at once.  Here the lane-items of all
@@ -19,7 +20,7 @@
 //     loads, then the arithmetic and the stores;
 //   * the update is "lane = (row, column)": the 8 lanes of a dim-8 row read 32 contiguous bytes of
 //     param, of each slot and of the gradient -- one full sector per array per row, no shuffles --
-//     and every lane executes exactly one element update (the d8 kernel ran four on 2 of 8 lanes).
+//     and every lane executes exactly one element update.
 // Measured and rejected (git history, commit "flat kernels: warp-uniform segment fast path"): specialising the
 // loop body for warp-iterations that lie inside one segment (segment constants loaded once, no per-item search)
 // cut instructions but cost 12-16 registers and no time: these kernels are bound by memory round trips, not by

@@ -267,15 +267,7 @@ __global__ void __launch_bounds__(256) k_push_rows(GroupView gv, SegBatch sb, Op
   }
 }
 
-// ---------------------------------------------------------------------------
-// Small-row specialisations.  A dim-8 fp32 row is one 32 B sector and its Adam record
-// ([p | m | v], 96 B) is three; issuing it as per-thread 16 B accesses costs one L1 tag /
-// L2 request / NVLink packet per 16 B.  Here consecutive lanes cover consecutive 16 B chunks
-// of the SAME record, so one warp instruction touches whole records: 2 lanes per row for the
-// gather (one 32 B request per row), 8 lanes per row for the update (one <= 128 B request per
-// record for the load and one for the store); the slot chunks meet in lanes 0/1 of the octet
-// through shuffles.  dim-1 rows keep their whole record [p, s0, s1, s2] in one float4.
-// ---------------------------------------------------------------------------
+// float4 shuffle within groups of `width` lanes (the paired-record kernels below)
 __device__ __forceinline__ float4 shfl4(float4 v, int src, int width) {
   float4 r;
   r.x = __shfl_sync(0xffffffffu, v.x, src, width);
@@ -283,84 +275,6 @@ __device__ __forceinline__ float4 shfl4(float4 v, int src, int width) {
   r.z = __shfl_sync(0xffffffffu, v.z, src, width);
   r.w = __shfl_sync(0xffffffffu, v.w, src, width);
   return r;
-}
-
-template <bool WRITE>
-__global__ void __launch_bounds__(256) k_rows_copy_d8(GroupView gv, SegBatch sb, int slot) {
-  const b200ps_seg_t& sg = sb.seg[blockIdx.y];
-  const TableView& tv = gv.tables[sg.table];
-  const int n = seg_count(sg);
-  const int lane = threadIdx.x & 31, c = lane & 1;
-  const long long rows_pad = ((long long)n + 15) / 16 * 16;  // keep warps converged for the shuffles
-  const long long stride = (long long)gridDim.x * blockDim.x / 2;
-  for (long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 2; row < rows_pad; row += stride) {
-    const bool live = row < n;
-    long long id = (live && c == 0) ? sg.ids_dev[row] : 0;
-    id = __shfl_sync(0xffffffffu, id, 0, 2);
-    if (!live) continue;
-    RowLoc loc = locate(gv, tv, id);
-    if (!loc.ok) {
-      if (c == 0) atomicOr(gv.err, kErrRange);
-      continue;
-    }
-    float* rec = loc.rec + tv.slot_off[slot] + 4 * c;
-    float* user = sg.rows_dev + row * 8 + 4 * c;
-    const float4 x = ld_f4(WRITE ? user : rec);
-    if (c == 0) mark_present(tv, loc);
-    st_f4(WRITE ? rec : user, x);
-  }
-}
-
-__host__ __device__ constexpr int d8_lanes(int opt) {  // lanes per record: power of two >= 2*(1+S)
-  return opt_slots(opt) == 0 ? 2 : opt_slots(opt) == 1 ? 4 : 8;
-}
-
-template <int OPT>
-__global__ void __launch_bounds__(256) k_push_rows_d8(GroupView gv, SegBatch sb, OptParams o) {
-  constexpr int S = opt_slots(OPT);
-  constexpr int R4 = 2 * (1 + S);  // 16 B chunks per record
-  constexpr int LPR = d8_lanes(OPT);
-  const b200ps_seg_t& sg = sb.seg[blockIdx.y];
-  const TableView& tv = gv.tables[sg.table];
-  const int n = seg_count(sg);
-  const int lane = threadIdx.x & 31, c = lane & (LPR - 1);
-  constexpr int RPW = 32 / LPR;  // rows per warp
-  const long long rows_pad = ((long long)n + RPW - 1) / RPW * RPW;
-  const long long stride = (long long)gridDim.x * blockDim.x / LPR;
-  for (long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / LPR; row < rows_pad; row += stride) {
-    const bool live = row < n;
-    long long id = (live && c == 0) ? sg.ids_dev[row] : 0;
-    id = __shfl_sync(0xffffffffu, id, 0, LPR);
-    RowLoc loc = live ? locate(gv, tv, id) : RowLoc{nullptr, 0, 0, false};  // dead lanes must not claim a hashed slot
-    const bool ok = live && loc.ok;
-    if (live && !loc.ok && c == 0) atomicOr(gv.err, kErrRange);
-    float* rec = loc.rec + 4 * c;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f), g = v;
-    if (ok && c < R4) v = ld_f4(rec);
-    if (ok && c < 2) g = ld_f4(sg.rows_dev + row * 8 + 4 * c);
-    if (ok && c == 0) mark_present(tv, loc);
-    // slot chunks of half h = c & 1 live in lanes h, h+2, h+4, h+6 of the octet
-    float4 p = v, s0 = v, s1 = v, s2 = v;
-    if (S > 0) s0 = shfl4(v, (c & 1) + 2, LPR);
-    if (S > 1) s1 = shfl4(v, (c & 1) + 4, LPR);
-    if (S > 2) s2 = shfl4(v, (c & 1) + 6, LPR);
-    if (c < 2) {
-      const float lr = gv.rt->lr[loc.shard], alpha = gv.rt->alpha[loc.shard], l2adj = gv.rt->l2adj[loc.shard];
-      float* gf = reinterpret_cast<float*>(&g);
-      float* pf = reinterpret_cast<float*>(&p);
-      float* af = reinterpret_cast<float*>(&s0);
-      float* bf = reinterpret_cast<float*>(&s1);
-      float* cf = reinterpret_cast<float*>(&s2);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) opt_update<OPT>(gf[e], pf[e], af[e], bf[e], cf[e], lr, alpha, l2adj, o);
-    }
-    // hand the updated slot chunks back to the lanes that own their 16 B of the record
-    float4 out = p;
-    if (S > 0) { const float4 t = shfl4(s0, c & 1, LPR); if ((c >> 1) == 1) out = t; }
-    if (S > 1) { const float4 t = shfl4(s1, c & 1, LPR); if ((c >> 1) == 2) out = t; }
-    if (S > 2) { const float4 t = shfl4(s2, c & 1, LPR); if ((c >> 1) == 3) out = t; }
-    if (ok && c < R4) st_f4(rec, out);
-  }
 }
 
 // ---------------------------------------------------------------------------
@@ -466,29 +380,6 @@ __global__ void __launch_bounds__(256) k_pair_push(GroupView gv, PairBatch pb, O
   }
 }
 
-// dim-1 tables: the record [p, s0, s1, s2] (16 B) is one float4 per row.
-template <int OPT>
-__global__ void __launch_bounds__(256) k_push_rows_d1(GroupView gv, SegBatch sb, OptParams o) {
-  constexpr int S = opt_slots(OPT);
-  const b200ps_seg_t& sg = sb.seg[blockIdx.y];
-  const TableView& tv = gv.tables[sg.table];
-  const int n = seg_count(sg);
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += stride) {
-    RowLoc loc = locate(gv, tv, sg.ids_dev[row]);
-    if (!loc.ok) {
-      atomicOr(gv.err, kErrRange);
-      continue;
-    }
-    float4 r = ld_f4(loc.rec);
-    const float g = sg.rows_dev[row];
-    mark_present(tv, loc);
-    opt_update<OPT>(g, r.x, r.y, r.z, r.w, gv.rt->lr[loc.shard], gv.rt->alpha[loc.shard], gv.rt->l2adj[loc.shard], o);
-    if (S == 0) *loc.rec = r.x;  // keep the padding untouched: one 4 B store
-    else st_f4(loc.rec, r);
-  }
-}
-
 // ---------------------------------------------------------------------------
 // Dense kernels (kernel.go:27-32,58-66,99-116,163-169): whole-tensor update,
 // optionally reducing R replica gradients first (sync-SGD averaging fused with
@@ -498,6 +389,7 @@ struct ReplicaGrads {
   const float* g[kMaxShards];
   int n;
   float scale;
+  int divide;  // 1: g = sum / scale (sync-SGD average, servicer.py:207); 0: g = sum * scale (allreduce postscale)
 };
 
 template <int OPT, int VEC, bool TWICE>
@@ -534,7 +426,8 @@ __device__ __forceinline__ void dense_update_range(const GroupView& gv, const Ta
     }
 #pragma unroll
     for (int e = 0; e < VEC; ++e) {
-      if (rg.scale != 1.0f) g[e] = mul(g[e], rg.scale);
+      if (rg.divide) g[e] = fdiv(g[e], rg.scale);
+      else if (rg.scale != 1.0f) g[e] = mul(g[e], rg.scale);
       opt_update<OPT>(g[e], p[e], s0[e], s1[e], s2[e], lr, alpha, l2adj, o);
       if (TWICE) {  // quirk Q1: dense AMSGrad falls through into plain Adam (optimizer.go:186-192)
         opt_update<kAdam>(g[e], p[e], s0[e], s1[e], s2[e], lr, alpha, l2adj, o);
@@ -564,6 +457,7 @@ __global__ void __launch_bounds__(256) k_push_dense(GroupView gv, SegBatch sb, O
   rg.g[0] = sg.rows_dev;
   rg.n = 1;
   rg.scale = 1.0f;
+  rg.divide = 0;
   const bool vec = ((tv.rows * tv.dim) & 3) == 0 && ((uintptr_t)sg.rows_dev & 15u) == 0;
   if (vec) dense_update_range<OPT, 4, TWICE>(gv, tv, rg, o);
   else dense_update_range<OPT, 1, TWICE>(gv, tv, rg, o);

@@ -149,7 +149,7 @@ class _FusedPSBackend(object):
         self._check(lib.b200ps_barrier(h, st))                      # every rank's gradients are complete
         self._check(lib.b200ps_push_begin_shard(h, self.rank, float(lr), None, st))
         self._check(lib.b200ps_push_dense_reduce(h, self.slice_ids[self.rank], self._reduce_ptrs, self.world,
-                                                 float(scale), st))   # reduce + scale + update, one kernel
+                                                 float(scale), 0, st))  # reduce + scale + update, one kernel
         self._check(lib.b200ps_push_end_shard(h, self.rank, st))
         self._check(lib.b200ps_barrier(h, st))                      # every slice is updated
         arr, n = self._pull

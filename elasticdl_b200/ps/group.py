@@ -345,10 +345,13 @@ class PSGroup:
     def push_dense(self, items):
         self._run_segs(self.lib.b200ps_push_dense, items)
 
-    def push_dense_reduce(self, name, grads, scale=1.0):
+    def push_dense_reduce(self, name, grads, scale=1.0, divide=False):
+        """Sum the replica gradients `grads` left to right, then divide the sum by `scale` (divide=True, the
+        sync-SGD average) or multiply it by `scale`, and apply the optimizer update -- one kernel."""
         tid, _, is_dense, _ = self.lookup(name)
         ptrs = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
-        check(self.lib.b200ps_push_dense_reduce(self._h, tid, ptrs, len(grads), float(scale), self._stream()))
+        check(self.lib.b200ps_push_dense_reduce(self._h, tid, ptrs, len(grads), float(scale), 1 if divide else 0,
+                                                self._stream()))
 
     def push_end(self, sync=True):
         """Version++ on every shard; returns the new versions (list) when sync."""

@@ -287,7 +287,7 @@ class PSClient(object):
             w = owner.grads_to_wait
             g.push_begin(learning_rate, [version] * self.ps_num)
             for name, parts in buf["dense"].items():
-                g.push_dense_reduce(name, parts, scale=1.0 / w)
+                g.push_dense_reduce(name, parts, scale=w, divide=True)  # grad / grads_to_wait in fp32
             row_items = []
             for name, (vals, ids) in buf["sparse"].items():
                 tid, dim, _, _ = g.lookup(name)

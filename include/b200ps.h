@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define B200PS_ABI_VERSION 1
+#define B200PS_ABI_VERSION 2
 #define B200PS_MAX_SHARDS 16
 #define B200PS_MAX_SEGS 96 /* segments per batched launch (DeepFM: 76 tables in one) */
 
@@ -191,12 +191,14 @@ int b200ps_push_begin(b200ps_t* ps, float learning_rate, const int32_t* model_ve
 int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream);
 /* Dense gradients: rows_dev = gradient [numel]. */
 int b200ps_push_dense(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream);
-/* Dense gradient REDUCE fused with the update: g = scale * sum_r grads_dev[r]
- * (r = 0..n_replicas-1, pointers may be peer memory), then the optimizer update
- * in place (sync-SGD averaging, python/ps/servicer.py:205-212, fused with
- * kernel_api.cc:6-96). */
+/* Dense gradient REDUCE fused with the update: s = sum_r grads_dev[r] in fp32, left to right
+ * (r = 0..n_replicas-1, pointers may be peer memory), then g = s / scale when divide != 0 (sync-SGD
+ * averaging, python/ps/servicer.py:205-212: grad / grads_to_wait) or g = s * scale when divide == 0
+ * (Horovod's postscale_factor, elasticai_api/pytorch/optimizer.py:141-157), then the optimizer update
+ * in place (kernel_api.cc:6-96).  s / w and s * fl(1/w) differ in the last bit for most w that are not
+ * powers of two.  divide with scale 0 is B200PS_EINVAL. */
 int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* grads_dev,
-                             int n_replicas, float scale, void* stream);
+                             int n_replicas, float scale, int divide, void* stream);
 int b200ps_push_end(b200ps_t* ps, int32_t* versions_out_host, void* stream);
 /* begin / end that reach ONE shard only: the owner-side ApplyGradients of the allreduce controller's fused
  * reduce + update (every rank updates the slice it owns exactly once per step), and of the per-shard gRPC

@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_python_vectors.json")
 
 
-def test_abi_exports_every_declared_symbol():
+def test_abi_v2_exports_every_declared_symbol():
     from elasticdl_b200 import _lib
 
     header = "".join(open(os.path.join(ROOT, "include", h)).read() for h in ("b200ps.h", "b200_deepfm.h", "b200_features.h"))
@@ -27,7 +27,7 @@ def test_abi_exports_every_declared_symbol():
     lib = _lib.lib()
     for name in declared:
         assert getattr(lib, name) is not None
-    assert lib.b200ps_abi_version() == 1
+    assert lib.b200ps_abi_version() == _lib.ABI_VERSION == 2
     out = subprocess.check_output(["nm", "-D", "--defined-only", os.path.join(ROOT, "elasticdl_b200", "csrc", "libb200ps.so")], text=True)
     exported = set(re.findall(r"\b(b200(?:ps|_deepfm|feat)_[a-z_0-9]+)$", out, flags=re.M))
     assert declared <= exported

@@ -149,8 +149,8 @@ class HostGroup(PSGroup):
             self.calls.append(["push_rows", self._name_of(tid),
                                {int(i): row.tolist() for i, row in zip(ids[:live].tolist(), g)}])
 
-    def push_dense_reduce(self, name, grads, scale=1.0):
-        self.calls.append(["push_dense_reduce", name, [g.reshape(-1).tolist() for g in grads], float(scale)])
+    def push_dense_reduce(self, name, grads, scale=1.0, divide=False):
+        self.calls.append(["push_dense_reduce", name, [g.reshape(-1).tolist() for g in grads], float(scale), divide])
 
     def push_end(self, sync=True):
         self.versions = [v + 1 for v in self.versions]  # every shard, every push (quirk Q7)
@@ -264,10 +264,10 @@ def test_product_ps_client_errors_before_any_update():
         client.pull_embedding_vectors("e", [])
 
 
-def test_product_sync_sgd_host_logic_pserver_servicer_test_py_366():
+def test_product_sync_sgd_host_logic_divides_pserver_servicer_test_py_366():
     """Sync-SGD as the Python PS does it (python/ps/servicer.py:168-238; vector of pserver_servicer_test.py:366-432):
     grads_to_wait = 2 -> the first push is buffered (accepted, version unchanged), the second applies ONE update with
-    the dense gradients averaged (the fused reduce kernel gets both parts and scale 1/2) and the sparse gradients
+    the dense gradients averaged (the fused reduce kernel gets both parts and divides their sum by 2) and the sparse gradients
     concatenated then summed per id, version 0 -> 1; a third push that still carries version 0 is rejected."""
     import threading
 
@@ -291,8 +291,8 @@ def test_product_sync_sgd_host_logic_pserver_servicer_test_py_366():
     assert kinds == ["push_begin", "push_dense_reduce", "push_dense_reduce", "push_rows", "push_end"]
     assert group.calls[0][1:] == [0.1, [0]]
     for c in group.calls[1:3]:
-        name, parts, scale = c[1], c[2], c[3]
-        assert scale == 0.5 and parts == [g0[name].reshape(-1).tolist(), g1[name].reshape(-1).tolist()]
+        name, parts, scale, divide = c[1], c[2], c[3], c[4]
+        assert scale == 2 and divide is True and parts == [g0[name].reshape(-1).tolist(), g1[name].reshape(-1).tolist()]
     rows = group.calls[3][2]
     assert group.calls[3][1] == "emb" and list(rows) == [3, 1, 9]  # first-occurrence order over e0 ++ e1
     assert np.array_equal(np.asarray(rows[3], F), e0[0][0] + e0[0][2])
