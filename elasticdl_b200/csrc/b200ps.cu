@@ -124,9 +124,7 @@ struct b200ps {
   int x_table = -1, x_G = 0, x_B = 0, x_me = -1;
   long long x_cap = 0, x_off_ids = 0, x_off_resp = 0, x_off_upd = 0, x_off_served = 0;
   bool x_pulled = false;
-  int* d_x_deep = nullptr;
-  int* d_x_wide = nullptr;
-  std::vector<int> x_deep_host, x_wide_host;
+  XTabs x_tabs{};
   // the dedup's two kernels (small segments / large segments) run side by side: a second stream + fork / join events
   cudaStream_t u_side = nullptr;
   cudaEvent_t u_fork = nullptr, u_join = nullptr;
@@ -544,8 +542,6 @@ int b200ps_destroy(b200ps_t* ps) {
   cudaFree(ps->d_versions);
   cudaFree(ps->d_count);
   cudaFree(ps->d_state);
-  cudaFree(ps->d_x_deep);
-  cudaFree(ps->d_x_wide);
   if (ps->u_side) cudaStreamDestroy(ps->u_side);
   if (ps->u_fork) cudaEventDestroy(ps->u_fork);
   if (ps->u_join) cudaEventDestroy(ps->u_join);
@@ -1101,18 +1097,43 @@ int b200ps_push_rows_pair(b200ps_t* ps, const b200ps_seg_t* segs_a, float* const
 
 // ---- owner-computes exchange (ps_exchange.cuh) ----------------------------------
 int b200ps_xchg_create(b200ps_t* ps, int G, int B, const int32_t* deep_tables, const int32_t* wide_tables) {
-  if (!ps || G < 1 || B < 1 || !deep_tables || !wide_tables) return fail(B200PS_EINVAL, "bad exchange definition");
+  if (!ps || B < 1 || !deep_tables || !wide_tables) return fail(B200PS_EINVAL, "bad exchange definition");
+  if (G < 1 || G > kXMaxG) return fail(B200PS_EINVAL, "the exchange moves 1 to " + std::to_string(kXMaxG) + " table pairs");
   if (ps->x_table >= 0) return fail(B200PS_ESTATE, "exchange already created");
   int me = -1, n_local = 0;
   for (int s = 0; s < ps->n_shards; ++s)
     if (ps->shard[s].local) { me = s; ++n_local; }
   if (n_local != 1) return fail(B200PS_ESTATE, "the exchange needs exactly one local shard per process (rank-per-GPU)");
+  // the owner-side constants of every pair on my shard: the exchange kernels take them instead of the table directory
+  XTabs xt{};
+  xt.shard_shift = group_view(ps).shard_shift;
   for (int g = 0; g < G; ++g) {
     if (deep_tables[g] < 0 || deep_tables[g] >= (int)ps->tables.size() || wide_tables[g] < 0 ||
         wide_tables[g] >= (int)ps->tables.size())
       return fail(B200PS_ENOTFOUND, "unknown table id in exchange definition");
-    if (ps->tables[deep_tables[g]].dim != 8 || ps->tables[wide_tables[g]].dim != 1)
-      return fail(B200PS_EWIDTH, "the exchange moves dim-8 / dim-1 table pairs");
+    const Table& d = ps->tables[deep_tables[g]];
+    const Table& w = ps->tables[wide_tables[g]];
+    if (d.dim != 8 || w.dim != 1) return fail(B200PS_EWIDTH, "the exchange moves dim-8 / dim-1 table pairs");
+    if (d.hashed || w.hashed || d.is_dense || w.is_dense || d.owner >= 0 || w.owner >= 0 || d.raw || w.raw)
+      return fail(B200PS_EINVAL, "the exchange moves direct-indexed tables striped over every shard "
+                                 "(not hashed, dense, pinned to one shard or raw)");
+    for (int j = 0; j <= kMaxSlots; ++j) {
+      if (g == 0) {
+        xt.deep_soff[j] = (int)d.slot_off[j];
+        xt.wide_soff[j] = (int)w.slot_off[j];
+      } else if (xt.deep_soff[j] != (int)d.slot_off[j] || xt.wide_soff[j] != (int)w.slot_off[j]) {
+        return fail(B200PS_EINVAL, "the exchanged deep tables, and the wide tables, need one slot layout each");
+      }
+    }
+    if (!d.alloc[me].ptr || !w.alloc[me].ptr) return fail(B200PS_ESTATE, "an exchanged table is not allocated on the local shard");
+    xt.deep[g] = (float*)((char*)d.alloc[me].ptr + d.base_off);
+    xt.wide[g] = (float*)((char*)w.alloc[me].ptr + w.base_off);
+    xt.deep_pres[g] = d.present_off ? (uint32_t*)((char*)d.alloc[me].ptr + d.present_off) : nullptr;
+    xt.wide_pres[g] = w.present_off ? (uint32_t*)((char*)w.alloc[me].ptr + w.present_off) : nullptr;
+    xt.deep_rows[g] = d.rows;
+    xt.wide_rows[g] = w.rows;
+    xt.deep_stride[g] = (int)d.row_stride;
+    xt.wide_stride[g] = (int)w.row_stride;
   }
   ps->x_G = G;
   ps->x_B = B;
@@ -1139,13 +1160,7 @@ int b200ps_xchg_create(b200ps_t* ps, int G, int B, const int32_t* deep_tables, c
     if (id < 0) return id;
     ps->x_table = id;
   }
-  DeviceGuard g(ps->client_device);
-  CUDA_OK(cudaMalloc(&ps->d_x_deep, sizeof(int) * G));
-  CUDA_OK(cudaMalloc(&ps->d_x_wide, sizeof(int) * G));
-  CUDA_OK(cudaMemcpy(ps->d_x_deep, deep_tables, sizeof(int) * G, cudaMemcpyHostToDevice));
-  CUDA_OK(cudaMemcpy(ps->d_x_wide, wide_tables, sizeof(int) * G, cudaMemcpyHostToDevice));
-  ps->x_deep_host.assign(deep_tables, deep_tables + G);
-  ps->x_wide_host.assign(wide_tables, wide_tables + G);
+  ps->x_tabs = xt;  // stays valid: a table's allocation on its shard lives as long as the group
   return B200PS_OK;
 }
 
@@ -1163,45 +1178,11 @@ static int xview(b200ps_t* ps, XView* x) {
   x->off_upd = ps->x_off_upd;
   x->off_served = ps->x_off_served;
   x->cap = ps->x_cap;
-  x->deep_tab = ps->d_x_deep;
-  x->wide_tab = ps->d_x_wide;
   x->n = ps->n_shards;
   x->me = ps->x_me;
   x->G = ps->x_G;
   x->B = ps->x_B;
   return B200PS_OK;
-}
-
-// The owner-side constants of the exchanged table pairs on MY shard, for the fast exchange kernels.  false: some
-// table is hashed / owned by one shard / not allocated here -> the generic kernels run instead.
-static bool xtabs(b200ps_t* ps, XTabs* t) {
-  if (ps->x_G > kXMaxG) return false;
-  const int me = ps->x_me;
-  t->shard_shift = -1;
-  if ((ps->n_shards & (ps->n_shards - 1)) == 0) {
-    int sh = 0;
-    while ((1 << sh) < ps->n_shards) ++sh;
-    t->shard_shift = sh;
-  }
-  for (int g = 0; g < ps->x_G; ++g) {
-    const Table& d = ps->tables[ps->x_deep_host[g]];
-    const Table& w = ps->tables[ps->x_wide_host[g]];
-    if (d.hashed || w.hashed || d.owner >= 0 || w.owner >= 0 || d.is_dense || w.is_dense) return false;
-    if (!d.alloc[me].ptr || !w.alloc[me].ptr) return false;
-    t->deep[g] = (float*)((char*)d.alloc[me].ptr + d.base_off);
-    t->wide[g] = (float*)((char*)w.alloc[me].ptr + w.base_off);
-    t->deep_pres[g] = d.present_off ? (uint32_t*)((char*)d.alloc[me].ptr + d.present_off) : nullptr;
-    t->wide_pres[g] = w.present_off ? (uint32_t*)((char*)w.alloc[me].ptr + w.present_off) : nullptr;
-    t->deep_rows[g] = d.rows;
-    t->wide_rows[g] = w.rows;
-    t->deep_stride[g] = (int)d.row_stride;
-    t->wide_stride[g] = (int)w.row_stride;
-    for (int j = 0; j <= kMaxSlots; ++j) {
-      if (g == 0) { t->deep_soff[j] = (int)d.slot_off[j]; t->wide_soff[j] = (int)w.slot_off[j]; }
-      else if (t->deep_soff[j] != (int)d.slot_off[j] || t->wide_soff[j] != (int)w.slot_off[j]) return false;
-    }
-  }
-  return true;
 }
 
 // grid.x per peer: 4 blocks per SM over all peers
@@ -1210,25 +1191,42 @@ static int xchg_per_peer(b200ps_t* ps) {
   return v < 2 ? 2 : v;
 }
 
+// The pull's three kernels (post, serve, unscatter) and the push's three (send_upd, apply, wait_applied) on `st`;
+// with `ev`, ev[i] is recorded after the i-th kernel.
+static void xchg_pull_kernels(b200ps_t* ps, const XView& x, const int64_t* uniq_dev, const int32_t* n_unique_dev,
+                              float* bet_deep_dev, float* bet_wide_dev, cudaStream_t st, cudaEvent_t* ev = nullptr) {
+  dim3 grid(xchg_per_peer(ps), ps->n_shards);
+  k_x_post<<<ps->n_sm, 256, 0, st>>>(x, uniq_dev, n_unique_dev);
+  if (ev) cudaEventRecord(ev[0], st);
+  k_x_serve<4><<<grid, 256, 0, st>>>(x, ps->x_tabs, ps->d_err);
+  if (ev) cudaEventRecord(ev[1], st);
+  k_x_unscatter<4><<<grid, 256, 0, st>>>(x, ps->d_err, bet_deep_dev, bet_wide_dev);
+  if (ev) cudaEventRecord(ev[2], st);
+  ps->launches += 3;
+}
+
+static void xchg_push_kernels(b200ps_t* ps, const XView& x, const float* gsum_deep_dev, const float* gsum_wide_dev,
+                              cudaStream_t st, cudaEvent_t* ev = nullptr) {
+  const OptParams o = ps->opt;
+  dim3 grid(xchg_per_peer(ps), ps->n_shards);
+  k_x_send_upd<4><<<grid, 256, 0, st>>>(x, ps->d_rt, gsum_deep_dev, gsum_wide_dev);
+  if (ev) cudaEventRecord(ev[0], st);
+  // the apply kernel holds 80 registers: 3 blocks per SM are resident, a 4th would wait for a second wave
+  dim3 grid_apply((unsigned)std::max(2, ps->n_sm * 3 / ps->n_shards), ps->n_shards);
+  DISPATCH_OPT(o.kind, k_x_apply<OPT, 2><<<grid_apply, 256, 0, st>>>(x, ps->x_tabs, ps->d_err, o));
+  if (ev) cudaEventRecord(ev[1], st);
+  k_x_wait_applied<<<1, 32, 0, st>>>(x, ps->d_err);
+  if (ev) cudaEventRecord(ev[2], st);
+  ps->launches += 3;
+}
+
 int b200ps_xchg_pull(b200ps_t* ps, const int64_t* uniq_dev, const int32_t* n_unique_dev, float* bet_deep_dev,
                      float* bet_wide_dev, void* stream) {
   XView x;
   int rc = xview(ps, &x);
   if (rc) return rc;
   DeviceGuard g(ps->client_device);
-  cudaStream_t st = (cudaStream_t)stream;
-  GroupView gv = group_view(ps);
-  dim3 grid(xchg_per_peer(ps), ps->n_shards);
-  k_x_post<<<ps->n_sm, 256, 0, st>>>(x, uniq_dev, n_unique_dev);
-  XTabs xt;
-  if (xtabs(ps, &xt)) {
-    k_x_serve2<4><<<grid, 256, 0, st>>>(x, xt, gv.err);
-    k_x_unscatter2<4><<<grid, 256, 0, st>>>(x, gv.err, bet_deep_dev, bet_wide_dev);
-  } else {
-    k_x_serve<<<grid, 256, 0, st>>>(x, gv);
-    k_x_unscatter<<<grid, 256, 0, st>>>(x, gv, bet_deep_dev, bet_wide_dev);
-  }
-  ps->launches += 3;
+  xchg_pull_kernels(ps, x, uniq_dev, n_unique_dev, bet_deep_dev, bet_wide_dev, (cudaStream_t)stream);
   ps->x_pulled = true;
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
@@ -1241,22 +1239,7 @@ int b200ps_xchg_push(b200ps_t* ps, const float* gsum_deep_dev, const float* gsum
   if (!ps->x_pulled) return fail(B200PS_ESTATE, "b200ps_xchg_push follows the b200ps_xchg_pull of the same id lists");
   ps->x_pulled = false;
   DeviceGuard g(ps->client_device);
-  cudaStream_t st = (cudaStream_t)stream;
-  GroupView gv = group_view(ps);
-  OptParams o = ps->opt;
-  dim3 grid(xchg_per_peer(ps), ps->n_shards);
-  XTabs xt;
-  if (xtabs(ps, &xt)) {
-    k_x_send_upd2<4><<<grid, 256, 0, st>>>(x, gv.rt, gsum_deep_dev, gsum_wide_dev);
-    // the apply kernel holds 80 registers: 3 blocks per SM are resident, a 4th would wait for a second wave
-    dim3 grid_apply((unsigned)std::max(2, ps->n_sm * 3 / ps->n_shards), ps->n_shards);
-    DISPATCH_OPT(o.kind, k_x_apply2<OPT, 2><<<grid_apply, 256, 0, st>>>(x, xt, gv.err, o));
-  } else {
-    k_x_send_upd<<<grid, 256, 0, st>>>(x, gv, gsum_deep_dev, gsum_wide_dev);
-    DISPATCH_OPT(o.kind, k_x_apply<OPT><<<grid, 256, 0, st>>>(x, gv, o));
-  }
-  k_x_wait_applied<<<1, 32, 0, st>>>(x, gv);
-  ps->launches += 3;
+  xchg_push_kernels(ps, x, gsum_deep_dev, gsum_wide_dev, (cudaStream_t)stream);
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
 }
@@ -1271,32 +1254,11 @@ int b200ps_xchg_profile(b200ps_t* ps, const int64_t* uniq_dev, const int32_t* n_
   if (rc) return rc;
   DeviceGuard g(ps->client_device);
   cudaStream_t st = (cudaStream_t)stream;
-  GroupView gv = group_view(ps);
-  OptParams o = ps->opt;
-  dim3 grid(xchg_per_peer(ps), ps->n_shards);
   cudaEvent_t ev[7];
   for (auto& e : ev) CUDA_OK(cudaEventCreate(&e));
   cudaEventRecord(ev[0], st);
-  XTabs xt;
-  const bool fast = xtabs(ps, &xt);
-  k_x_post<<<ps->n_sm, 256, 0, st>>>(x, uniq_dev, n_unique_dev);
-  cudaEventRecord(ev[1], st);
-  if (fast) k_x_serve2<4><<<grid, 256, 0, st>>>(x, xt, gv.err);
-  else k_x_serve<<<grid, 256, 0, st>>>(x, gv);
-  cudaEventRecord(ev[2], st);
-  if (fast) k_x_unscatter2<4><<<grid, 256, 0, st>>>(x, gv.err, bet_deep_dev, bet_wide_dev);
-  else k_x_unscatter<<<grid, 256, 0, st>>>(x, gv, bet_deep_dev, bet_wide_dev);
-  cudaEventRecord(ev[3], st);
-  if (fast) k_x_send_upd2<4><<<grid, 256, 0, st>>>(x, gv.rt, gsum_deep_dev, gsum_wide_dev);
-  else k_x_send_upd<<<grid, 256, 0, st>>>(x, gv, gsum_deep_dev, gsum_wide_dev);
-  cudaEventRecord(ev[4], st);
-  dim3 grid_apply((unsigned)std::max(2, ps->n_sm * 3 / ps->n_shards), ps->n_shards);
-  if (fast) { DISPATCH_OPT(o.kind, k_x_apply2<OPT, 2><<<grid_apply, 256, 0, st>>>(x, xt, gv.err, o)); }
-  else { DISPATCH_OPT(o.kind, k_x_apply<OPT><<<grid, 256, 0, st>>>(x, gv, o)); }
-  cudaEventRecord(ev[5], st);
-  k_x_wait_applied<<<1, 32, 0, st>>>(x, gv);
-  cudaEventRecord(ev[6], st);
-  ps->launches += 6;
+  xchg_pull_kernels(ps, x, uniq_dev, n_unique_dev, bet_deep_dev, bet_wide_dev, st, ev + 1);
+  xchg_push_kernels(ps, x, gsum_deep_dev, gsum_wide_dev, st, ev + 4);
   CUDA_OK(cudaStreamSynchronize(st));
   for (int i = 0; i < 6; ++i) cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]);
   for (auto& e : ev) cudaEventDestroy(e);

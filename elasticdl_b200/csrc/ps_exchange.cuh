@@ -49,7 +49,6 @@ struct XHeader {  // first page of every rank's exchange buffer
   // local
   int epoch;
   int post_cursor[kMaxShards]; // requester: ids bucketed so far for each owner (this epoch)
-  int cursor[kMaxShards];      // (unused since the ids arrive bucketed)
   int served_cnt[kMaxShards];  // owner: rows served to each source by the last pull
   unsigned done_blocks;
   unsigned done_src[kMaxShards];
@@ -59,8 +58,6 @@ struct XView {
   char* buf[kMaxShards];  // every rank's exchange buffer (peer-mapped); buf[me] is local
   long long off_ids, off_resp, off_upd, off_served;  // byte offsets of the regions
   long long cap;                                     // entries per (owner, source) lane = G * B
-  const int* deep_tab;                               // [G] table ids (device)
-  const int* wide_tab;                               // [G]
   int n, me, G, B;
 };
 
@@ -240,225 +237,12 @@ __device__ __forceinline__ long long id_of(int lo, int hi) {
   return (long long)(((unsigned long long)(unsigned)hi << 32) | (unsigned)lo);
 }
 
-// Owner: stream MY bucket of source blockIdx.y's id list, gather the rows, return them at the same index.
-__global__ void __launch_bounds__(256) k_x_serve(XView x, GroupView gv) {
-  const int src = blockIdx.y;
-  XHeader* h = xhdr(x, x.me);
-  __shared__ int s_epoch, s_total;
-  if (threadIdx.x == 0) {
-    s_epoch = h->epoch;
-    s_total = poll8(&h->req[src], s_epoch, gv.err).x;
-  }
-  __syncthreads();
-  const int epoch = s_epoch, total = s_total;
-  const char* ids = xids(x, src, x.me);  // the ids source `src` wants from me (remote unless src == me), read coalesced
-  char* resp = xresp(x, src, x.me);      // remote, written contiguously: entry i answers id i
-  char* served = xserved(x, x.me, src);
-  const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;
-  const unsigned gm = 0xfu << (lane & 28);
-  const long long stride = (long long)gridDim.x * blockDim.x / 4;
-  // four lanes per id -- they load {deep lo, deep hi, wide, -} and store one tagged word each
-  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 4; i < total; i += stride) {
-    int4 e = make_int4(0, 0, 0, 0);
-    if (lane4 == 0) e = poll16(ids + i * kXIdEntry, epoch, gv.err);  // one remote 16 B read per id
-    e.x = __shfl_sync(gm, e.x, 0, 4);
-    e.y = __shfl_sync(gm, e.y, 0, 4);
-    e.z = __shfl_sync(gm, e.z, 0, 4);
-    const long long id = id_of(e.x, e.y);
-    const int slot = e.z;
-    const int g = slot / x.B;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (lane4 < 2) {
-      const TableView& td = gv.tables[x.deep_tab[g]];
-      RowLoc loc = locate(gv, td, id);
-      if (loc.ok) {
-        v = ld_f4(loc.rec + 4 * lane4);
-        if (lane4 == 0) mark_present(td, loc);
-      } else if (lane4 == 0) {
-        atomicOr(gv.err, kErrRange);
-      }
-    } else if (lane4 == 2) {
-      const TableView& tw = gv.tables[x.wide_tab[g]];
-      RowLoc lw = locate(gv, tw, id);
-      if (lw.ok) {
-        v.x = *lw.rec;
-        mark_present(tw, lw);
-      }
-    }
-    const float d3 = __shfl_sync(gm, v.w, 0, 4), d6 = __shfl_sync(gm, v.z, 1, 4), d7 = __shfl_sync(gm, v.w, 1, 4);
-    char* out = resp + i * kXResp + 16 * lane4;
-    if (lane4 == 0) st_word16(out, __float_as_int(v.x), __float_as_int(v.y), __float_as_int(v.z), epoch);
-    else if (lane4 == 1) st_word16(out, __float_as_int(d3), __float_as_int(v.x), __float_as_int(v.y), epoch);
-    else if (lane4 == 2) st_word16(out, __float_as_int(d6), __float_as_int(d7), __float_as_int(v.x), epoch);
-    else {
-      st_word16(out, slot, 0, 0, epoch);
-      int4 rec = make_int4((int)(id & 0xffffffffLL), (int)(id >> 32), g, 0);
-      *reinterpret_cast<int4*>(served + i * kXServed) = rec;
-    }
-  }
-  __shared__ bool last;
-  __threadfence();  // served records: local, read by this GPU's later kernels
-  __syncthreads();
-  if (threadIdx.x == 0) last = atomicAdd(&h->done_src[src], 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last && threadIdx.x == 0) {
-    h->served_cnt[src] = total;
-    st_word8(&xhdr(x, src)->resp[x.me], total, epoch);
-    h->done_src[src] = 0;
-  }
-}
-
-// Requester: rows of owner blockIdx.y land in my response region -> bet_d / bet_w.
-__global__ void __launch_bounds__(256) k_x_unscatter(XView x, GroupView gv, float* bet_d, float* bet_w) {
-  const int owner = blockIdx.y;
-  XHeader* h = xhdr(x, x.me);
-  __shared__ int s_cnt, s_epoch;
-  if (threadIdx.x == 0) {
-    s_epoch = h->epoch;
-    s_cnt = poll8(&h->resp[owner], s_epoch, gv.err).x;
-  }
-  __syncthreads();
-  const int cnt = s_cnt, epoch = s_epoch;
-  const char* resp = xresp(x, x.me, owner);
-  const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;
-  const unsigned gm = 0xfu << (lane & 28);
-  const long long stride = (long long)gridDim.x * blockDim.x / 4;
-  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 4; i < cnt; i += stride) {
-    const int4 p = poll16(resp + i * kXResp + 16 * lane4, epoch, gv.err);
-    const int slot = __shfl_sync(gm, p.x, 3, 4);
-    float* row = bet_d + (long long)slot * 8;
-    if (lane4 == 0) {
-      row[0] = __int_as_float(p.x); row[1] = __int_as_float(p.y); row[2] = __int_as_float(p.z);
-    } else if (lane4 == 1) {
-      row[3] = __int_as_float(p.x); row[4] = __int_as_float(p.y); row[5] = __int_as_float(p.z);
-    } else if (lane4 == 2) {
-      row[6] = __int_as_float(p.x); row[7] = __int_as_float(p.y);
-      bet_w[slot] = __int_as_float(p.z);
-    }
-  }
-}
-
-// Requester: gradient rows to owner blockIdx.y, in the order that owner served my rows.
-__global__ void __launch_bounds__(256) k_x_send_upd(XView x, GroupView gv, const float* __restrict__ gsum_d,
-                                                    const float* __restrict__ gsum_w) {
-  const int owner = blockIdx.y;
-  XHeader* h = xhdr(x, x.me);
-  const int epoch = h->epoch;
-  const int cnt = ld_word8(&h->resp[owner]).x;  // validated by this step's k_x_unscatter
-  const char* resp = xresp(x, x.me, owner);
-  char* upd = xupd(x, owner, x.me);  // remote, contiguous
-  const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;
-  const unsigned gm = 0xfu << (lane & 28);
-  if (blockIdx.x == 0 && threadIdx.x == 0)  // this push's lr / Adam alpha / l2 for that shard (k_push_begin)
-    st_word16(&xhdr(x, owner)->updh[x.me], __float_as_int(gv.rt->lr[owner]), __float_as_int(gv.rt->alpha[owner]),
-              __float_as_int(gv.rt->l2adj[owner]), epoch);
-  const long long stride = (long long)gridDim.x * blockDim.x / 4;
-  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 4; i < cnt; i += stride) {
-    const int slot = ld_word16(resp + i * kXResp + 48).x;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (lane4 < 2) v = *reinterpret_cast<const float4*>(gsum_d + (long long)slot * 8 + 4 * lane4);
-    else if (lane4 == 2) v.x = gsum_w[slot];
-    const float g3 = __shfl_sync(gm, v.w, 0, 4), g6 = __shfl_sync(gm, v.z, 1, 4), g7 = __shfl_sync(gm, v.w, 1, 4);
-    char* out = upd + i * kXUpd + 16 * lane4;
-    if (lane4 == 0) st_word16(out, __float_as_int(v.x), __float_as_int(v.y), __float_as_int(v.z), epoch);
-    else if (lane4 == 1) st_word16(out, __float_as_int(g3), __float_as_int(v.x), __float_as_int(v.y), epoch);
-    else if (lane4 == 2) st_word16(out, __float_as_int(g6), __float_as_int(g7), __float_as_int(v.x), epoch);
-  }
-}
-
-// Owner: apply the updates of source blockIdx.y to the rows served to it (its own ApplyGradients:
-// lr / Adam alpha were fixed by the source's push_begin on this shard).
-template <int OPT>
-__global__ void __launch_bounds__(256) k_x_apply(XView x, GroupView gv, OptParams o) {
-  constexpr int S = opt_slots(OPT);
-  const int src = blockIdx.y;
-  XHeader* h = xhdr(x, x.me);
-  __shared__ int s_epoch, s_cnt;
-  __shared__ float s_lr, s_alpha, s_l2;
-  if (threadIdx.x == 0) {
-    s_epoch = h->epoch;
-    const int4 hd = poll16(&h->updh[src], s_epoch, gv.err);
-    s_cnt = h->served_cnt[src];
-    s_lr = __int_as_float(hd.x);
-    s_alpha = __int_as_float(hd.y);
-    s_l2 = __int_as_float(hd.z);
-  }
-  __syncthreads();
-  const int cnt = s_cnt, epoch = s_epoch;
-  const float lr = s_lr, alpha = s_alpha, l2adj = s_l2;
-  const char* upd = xupd(x, x.me, src);
-  const char* served = xserved(x, x.me, src);
-  const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;  // deep lo, deep hi, wide, idle
-  const unsigned gm = 0xfu << (lane & 28);
-  const long long stride = (long long)gridDim.x * blockDim.x / 4;
-  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 4; i < cnt; i += stride) {
-    const int4 e = *reinterpret_cast<const int4*>(served + i * kXServed);
-    const long long id = id_of(e.x, e.y);
-    int4 p = make_int4(0, 0, 0, 0);
-    if (lane4 < 3) p = poll16(upd + i * kXUpd + 16 * lane4, epoch, gv.err);
-    // words {g0 g1 g2}{g3 g4 g5}{g6 g7 gw} -> lane 0: g0..g3, lane 1: g4..g7, lane 2: gw
-    const int q1x = __shfl_sync(gm, p.x, 1, 4), q2x = __shfl_sync(gm, p.x, 2, 4), q2y = __shfl_sync(gm, p.y, 2, 4);
-    if (lane4 < 2) {
-      const TableView& td = gv.tables[x.deep_tab[e.z]];
-      RowLoc loc = locate(gv, td, id);
-      if (!loc.ok) continue;  // already reported by the serving pass
-      float4 g = lane4 == 0 ? make_float4(__int_as_float(p.x), __int_as_float(p.y), __int_as_float(p.z), __int_as_float(q1x))
-                            : make_float4(__int_as_float(p.y), __int_as_float(p.z), __int_as_float(q2x), __int_as_float(q2y));
-      float* rec = loc.rec + 4 * lane4;
-      float4 pr = ld_f4(rec), s0 = pr, s1 = pr, s2 = pr;
-      if (S > 0) s0 = ld_f4(rec + td.slot_off[1]);
-      if (S > 1) s1 = ld_f4(rec + td.slot_off[2]);
-      if (S > 2) s2 = ld_f4(rec + td.slot_off[3]);
-      float* gf = reinterpret_cast<float*>(&g);
-      float* pf = reinterpret_cast<float*>(&pr);
-      float* af = reinterpret_cast<float*>(&s0);
-      float* bf = reinterpret_cast<float*>(&s1);
-      float* cf = reinterpret_cast<float*>(&s2);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) opt_update<OPT>(gf[k], pf[k], af[k], bf[k], cf[k], lr, alpha, l2adj, o);
-      st_f4(rec, pr);
-      if (S > 0) st_f4(rec + td.slot_off[1], s0);
-      if (S > 1) st_f4(rec + td.slot_off[2], s1);
-      if (S > 2) st_f4(rec + td.slot_off[3], s2);
-    } else if (lane4 == 2) {
-      const TableView& tw = gv.tables[x.wide_tab[e.z]];
-      RowLoc lw = locate(gv, tw, id);
-      if (!lw.ok) continue;
-      float* rec = lw.rec;
-      float g = __int_as_float(p.z), pr = *rec, s0 = 0.f, s1 = 0.f, s2 = 0.f;
-      if (S > 0) s0 = rec[tw.slot_off[1]];
-      if (S > 1) s1 = rec[tw.slot_off[2]];
-      if (S > 2) s2 = rec[tw.slot_off[3]];
-      opt_update<OPT>(g, pr, s0, s1, s2, lr, alpha, l2adj, o);
-      *rec = pr;
-      if (S > 0) rec[tw.slot_off[1]] = s0;
-      if (S > 1) rec[tw.slot_off[2]] = s1;
-      if (S > 2) rec[tw.slot_off[3]] = s2;
-    }
-  }
-  __shared__ bool last;
-  __threadfence();  // rows are local: this GPU's later kernels (its next serve) read them in stream order
-  __syncthreads();
-  if (threadIdx.x == 0) last = atomicAdd(&h->done_src[src], 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last && threadIdx.x == 0) {
-    asm volatile("st.volatile.global.s32 [%0], %1;" ::"l"(&xhdr(x, src)->applied[x.me]), "r"(epoch) : "memory");
-    h->done_src[src] = 0;
-  }
-}
-
-// =============================================================================
-// Fast variants (round 2): the same protocol and the same words on the wire as the four kernels above, with
-//   * the owner's table constants resolved on the HOST (XTabs, a __grid_constant__ parameter): base pointer,
-//     bitmap, stride and row count of each of the G (deep, wide) pairs on MY shard -- no dependent loads of a
-//     table directory between an id and its record;
-//   * XU entries in flight per 4-lane group: all remote / inbox words of an iteration are loaded before the
-//     first one is used, then all records, then the stores.  Every pass of these kernels is a chain of two to
-//     four dependent round trips (NVLink word -> HBM record -> NVLink store); round 1 ran 3-4 passes of one
-//     entry per lane group, now one pass covers the list.
-// Used when every exchanged table is direct-indexed and striped (the hashed / dense-owner cases keep the generic
-// kernels above).
-// =============================================================================
+// The owner's table constants, resolved once on the host by b200ps_xchg_create and passed as a
+// __grid_constant__: base pointer, created-row bitmap, stride and row count of each of the G (deep, wide)
+// pairs on MY shard, so no table directory is read between an id and its record.  Every pass of a data
+// kernel is a chain of two to four dependent round trips (NVLink word -> HBM record -> NVLink store), so
+// each 4-lane group keeps XU entries in flight: all words of an iteration are loaded before the first
+// one is used, then all records, then the stores.
 constexpr int kXMaxG = kMaxSegs / 2;
 struct XTabs {
   float* deep[kXMaxG];
@@ -475,8 +259,9 @@ __device__ __forceinline__ long long xslot_of(const XView& x, const XTabs& t, lo
   return t.shard_shift >= 0 ? id >> t.shard_shift : id / x.n;
 }
 
+// Owner: stream MY bucket of source blockIdx.y's id list, gather the rows, return them at the same index.
 template <int XU>
-__global__ void __launch_bounds__(256) k_x_serve2(const __grid_constant__ XView x, const __grid_constant__ XTabs t, unsigned* err) {
+__global__ void __launch_bounds__(256) k_x_serve(const __grid_constant__ XView x, const __grid_constant__ XTabs t, unsigned* err) {
   const int src = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
   __shared__ int s_epoch, s_total;
@@ -568,8 +353,9 @@ __global__ void __launch_bounds__(256) k_x_serve2(const __grid_constant__ XView 
   }
 }
 
+// Requester: rows of owner blockIdx.y land in my response region -> bet_d / bet_w.
 template <int XU>
-__global__ void __launch_bounds__(256) k_x_unscatter2(const __grid_constant__ XView x, unsigned* err, float* bet_d, float* bet_w) {
+__global__ void __launch_bounds__(256) k_x_unscatter(const __grid_constant__ XView x, unsigned* err, float* bet_d, float* bet_w) {
   const int owner = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
   __shared__ int s_cnt, s_epoch;
@@ -610,9 +396,10 @@ __global__ void __launch_bounds__(256) k_x_unscatter2(const __grid_constant__ XV
   }
 }
 
+// Requester: gradient rows to owner blockIdx.y, in the order that owner served my rows.
 template <int XU>
-__global__ void __launch_bounds__(256) k_x_send_upd2(const __grid_constant__ XView x, const PushRt* rt, const float* __restrict__ gsum_d,
-                                                     const float* __restrict__ gsum_w) {
+__global__ void __launch_bounds__(256) k_x_send_upd(const __grid_constant__ XView x, const PushRt* rt, const float* __restrict__ gsum_d,
+                                                    const float* __restrict__ gsum_w) {
   const int owner = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
   const int epoch = h->epoch;
@@ -655,9 +442,11 @@ __global__ void __launch_bounds__(256) k_x_send_upd2(const __grid_constant__ XVi
   }
 }
 
+// Owner: apply the updates of source blockIdx.y to the rows served to it (its own ApplyGradients:
+// lr / Adam alpha were fixed by the source's push_begin on this shard).
 template <int OPT, int XU>
-__global__ void __launch_bounds__(256) k_x_apply2(const __grid_constant__ XView x, const __grid_constant__ XTabs t, unsigned* err,
-                                                  const OptParams o) {
+__global__ void __launch_bounds__(256) k_x_apply(const __grid_constant__ XView x, const __grid_constant__ XTabs t, unsigned* err,
+                                                 const OptParams o) {
   constexpr int S = opt_slots(OPT);
   const int src = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
@@ -758,7 +547,7 @@ __global__ void __launch_bounds__(256) k_x_apply2(const __grid_constant__ XView 
 }
 
 // Requester: all owners have applied my updates (push_end bumps the versions after this).
-__global__ void k_x_wait_applied(XView x, GroupView gv) {
+__global__ void k_x_wait_applied(XView x, unsigned* err) {
   XHeader* h = xhdr(x, x.me);
   if (threadIdx.x >= x.n) return;
   const int epoch = h->epoch;
@@ -766,7 +555,7 @@ __global__ void k_x_wait_applied(XView x, GroupView gv) {
     if (ld_word4(&h->applied[threadIdx.x]) >= epoch) return;
     __nanosleep(64);
   }
-  atomicOr(gv.err, kErrTimeout);
+  atomicOr(err, kErrTimeout);
 }
 
 }  // namespace b200ps_impl

@@ -19,7 +19,7 @@ import math
 
 import torch
 
-from elasticdl_b200._lib import check
+from elasticdl_b200._lib import MAX_SEGS, check
 
 # model_zoo/dac_ctr/feature_config.py:61-75 (len(boundaries)+1 buckets; I4 is not in FEATURE_GROUPS)
 INT_BUCKETS = [5, 10, 9, 10, 9, 9, 10, 10, 3, 6, 2, 9]
@@ -251,9 +251,11 @@ class DeepFMPSEngine:
         self.paired = bool(paired) and deep_dim == 8
         # exchange="owner": rank-per-GPU groups bucket ids by owner and move everything over NVLink in
         # contiguous runs, the owner serves / updates its own shard (csrc/ps_exchange.cuh);
-        # exchange="direct": kernels dereference the peer shard row by row.
+        # exchange="direct": kernels dereference the peer shard row by row.  The exchange moves at most
+        # MAX_SEGS / 2 id groups (b200ps_xchg_create).
         if exchange is None:
-            exchange = "owner" if (group.n_shards > 1 and len(group.local_shards) == 1 and deep_dim == 8) else "direct"
+            exchange = "owner" if (group.n_shards > 1 and len(group.local_shards) == 1 and deep_dim == 8
+                                   and len(group_rows) <= MAX_SEGS // 2) else "direct"
         assert exchange in ("owner", "direct")
         self.exchange = exchange
         if exchange == "owner":

@@ -152,7 +152,14 @@ int b200ps_push_rows_pair(b200ps_t* ps, const b200ps_seg_t* segs_a, float* const
  * buffers of b200ps_unique.  create: collective, then re-export / import the shards (the exchange
  * buffer is a peer-mapped allocation).  push belongs between b200ps_push_begin and b200ps_push_end
  * and updates the rows of the b200ps_xchg_pull that precedes it (gsum indexed like that pull's
- * bet rows); a push without its pull returns B200PS_ESTATE. */
+ * bet rows); a push without its pull returns B200PS_ESTATE.
+ * create accepts 1 <= G <= B200PS_MAX_SEGS / 2 pairs of direct-indexed tables striped over every
+ * shard (b200ps_table_register or b200ps_table_register_pair), with one slot layout among the
+ * deep tables and one among the wide tables, and a process that owns exactly one shard.  It
+ * returns B200PS_EINVAL for G out of range, a hashed table, a dense parameter, a table pinned to
+ * one shard, a raw buffer or differing slot layouts; B200PS_EWIDTH for dims other than 8 / 1;
+ * B200PS_ENOTFOUND for an unknown table id; B200PS_ESTATE for a second create, a process without
+ * exactly one local shard or a table not allocated on it.  A refused create changes nothing. */
 int b200ps_xchg_create(b200ps_t* ps, int G, int B, const int32_t* deep_tables, const int32_t* wide_tables);
 int b200ps_xchg_pull(b200ps_t* ps, const int64_t* uniq_dev, const int32_t* n_unique_dev, float* bet_deep_dev,
                      float* bet_wide_dev, void* stream);

@@ -1,7 +1,9 @@
 """Owner-computes exchange (csrc/ps_exchange.cuh) vs the direct peer path and the oracle
-(torchrun, one rank per GPU).  Checks: xchg_pull == pull_rows bit for bit; xchg_push (Adam) ==
-oracle applying every rank's push on disjoint rows; created-row counts; a DeepFM engine in
-exchange mode trains; no wait timed out."""
+(torchrun, one rank per GPU).  Checks: xchg_create refuses hashed, dense and raw tables and too many
+groups; xchg_pull == pull_rows bit for bit; xchg_push (Adam) == oracle applying every rank's push on
+disjoint rows; created-row counts; a DeepFM engine in exchange mode trains, one with too many groups
+takes the direct path; no wait timed out."""
+import ctypes
 import os
 import sys
 
@@ -12,6 +14,7 @@ import torch.distributed as dist
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from elasticdl_b200 import _lib  # noqa: E402
 from elasticdl_b200._lib import check  # noqa: E402
 from elasticdl_b200.ps import PSGroup  # noqa: E402
 from oracle import ps_oracle as O  # noqa: E402
@@ -38,7 +41,21 @@ def main():
     G, B, D = len(rows), 4096, 8
     deep = [group.register_table("d%d" % g, D, "zero", r) for g, r in enumerate(rows)]
     wide = [group.register_table("w%d" % g, 1, "zero", r) for g, r in enumerate(rows)]
+    hashed_id = group.register_table("hashed", D, "zero", expected_rows=64)
+    dense_id = group.register_dense("dense", (16, D), 0)
+    raw_id = check(group.lib.b200ps_raw_register(group._h, b"raw", 64))
     group.commit()
+
+    def create(dt, wt):
+        return group.lib.b200ps_xchg_create(group._h, len(dt), B, (ctypes.c_int32 * len(dt))(*dt),
+                                            (ctypes.c_int32 * len(wt))(*wt))
+
+    # the exchange serves direct-indexed striped tables only, and at most MAX_SEGS / 2 pairs; a refused
+    # create leaves no exchange behind, so the valid one below still succeeds
+    kx = _lib.MAX_SEGS // 2 + 1
+    for dt, wt in (([hashed_id] + deep[1:], wide), ([dense_id] + deep[1:], wide), (deep, [raw_id] + wide[1:]),
+                   ((deep * kx)[:kx], (wide * kx)[:kx])):
+        assert create(dt, wt) == _lib.EINVAL, (dt, wt, group.lib.b200ps_last_error())
     group.xchg_create(G, B, deep, wide)
     servers = [O.OracleServer(i, *ADAM, num_ps=world) for i in range(world)]
     oc = O.OraclePSClient(servers)
@@ -149,10 +166,14 @@ def main():
         l2 = float(eng.step_graph(ids, dense, labels))
     g2.check()
     assert l2 <= l1 + 1e-3
+    # ---- more id groups than the exchange moves: the engine takes the direct path ------------------
+    g3 = PSGroup(world, *ADAM, device=local, local_shards=[rank])
+    assert DeepFMPSEngine(g3, 64, group_rows=[16] * kx).exchange == "direct"
     dist.barrier()
     if rank == 0:
         print("mgpu_xchg_check ok: world=%d exchange pull bit-exact vs direct, push bit-exact vs oracle, "
               "engine loss %.4f -> %.4f -> %.4f" % (world, l0, l1, l2))
+    g3.close()
     g2.close()
     group.close()
     dist.destroy_process_group()
