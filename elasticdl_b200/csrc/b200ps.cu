@@ -1211,13 +1211,17 @@ static void xchg_push_kernels(b200ps_t* ps, const XView& x, const float* gsum_de
   dim3 grid(xchg_per_peer(ps), ps->n_shards);
   k_x_send_upd<4><<<grid, 256, 0, st>>>(x, ps->d_rt, gsum_deep_dev, gsum_wide_dev);
   if (ev) cudaEventRecord(ev[0], st);
-  // the apply kernel holds 80 registers: 3 blocks per SM are resident, a 4th would wait for a second wave
-  dim3 grid_apply((unsigned)std::max(2, ps->n_sm * 3 / ps->n_shards), ps->n_shards);
-  DISPATCH_OPT(o.kind, k_x_apply<OPT, 2><<<grid_apply, 256, 0, st>>>(x, ps->x_tabs, ps->d_err, o));
+  // one apply launch per source, in rank order: a row that several ranks pushed this step gets every rank's
+  // update, as if the ranks had pushed one after the other (concurrent sources would race on the record's
+  // read-modify-write and lose updates or tear the record).
+  // The apply kernel holds 80 registers: 3 blocks per SM are resident, a 4th would wait for a second wave
+  const unsigned grid_apply = (unsigned)ps->n_sm * 3;
+  for (int src = 0; src < ps->n_shards; ++src)
+    DISPATCH_OPT(o.kind, k_x_apply<OPT, 2><<<grid_apply, 256, 0, st>>>(x, ps->x_tabs, ps->d_err, o, src));
   if (ev) cudaEventRecord(ev[1], st);
   k_x_wait_applied<<<1, 32, 0, st>>>(x, ps->d_err);
   if (ev) cudaEventRecord(ev[2], st);
-  ps->launches += 3;
+  ps->launches += 2 + ps->n_shards;
 }
 
 int b200ps_xchg_pull(b200ps_t* ps, const int64_t* uniq_dev, const int32_t* n_unique_dev, float* bet_deep_dev,

@@ -18,8 +18,11 @@
 //                       serve order) and writes the matching gradient rows CONTIGUOUSLY into the
 //                       owner's inbox: no bucketing, no atomics
 //         k_x_apply     the owner applies the fused optimizer to its own shard: entry i of source s
-//                       updates the row it served as entry i (with the source's lr / Adam alpha)
+//                       updates the row it served as entry i (with the source's lr / Adam alpha); one
+//                       launch per source in rank order, so a row several ranks pushed gets every update
 // A push therefore rides on the routing of the pull that precedes it (the training step's order).
+// An id outside the owner's table is served as a zero row and flagged in the response header word; the
+// REQUESTER's k_x_unscatter raises the range error, as the direct pull reports it to its caller.
 //
 // Cross-GPU synchronisation is flag-in-data (the idea of NCCL's LL protocol): everything a peer
 // reads is made of naturally aligned 16-byte (or 8-byte) words whose last lane is the epoch TAG,
@@ -44,7 +47,7 @@ struct XHeader {  // first page of every rank's exchange buffer
   int2 req[kMaxShards];   // [src] {ids published, tag}
   int4 updh[kMaxShards];  // [src] {lr, alpha, l2adj (float bits), tag}
   // written by owner ranks into the REQUESTER's header
-  int2 resp[kMaxShards];    // [owner] {rows returned, tag}
+  int4 resp[kMaxShards];    // [owner] {rows returned, 1 if an id was outside the table, 0, tag}
   int applied[kMaxShards];  // [owner] tag: that owner has applied my updates
   // local
   int epoch;
@@ -52,6 +55,7 @@ struct XHeader {  // first page of every rank's exchange buffer
   int served_cnt[kMaxShards];  // owner: rows served to each source by the last pull
   unsigned done_blocks;
   unsigned done_src[kMaxShards];
+  unsigned range_src[kMaxShards];  // owner: an id of that source's bucket was outside the table (this pull)
 };
 
 struct XView {
@@ -313,7 +317,7 @@ __global__ void __launch_bounds__(256) k_x_serve(const __grid_constant__ XView x
           v[k] = ld_f4(t.deep[g] + sl * t.deep_stride[g] + 4 * lane4);
           if (lane4 == 0 && t.deep_pres[g]) { pres[k] = t.deep_pres[g] + (sl >> 5); bit[k] = 1u << (sl & 31); }
         } else if (lane4 == 0) {
-          atomicOr(err, kErrRange);
+          atomicOr(&h->range_src[src], 1u);  // the requester reports it (k_x_unscatter), not this shard
         }
       } else if (lane4 == 2) {
         if (id >= 0 && sl < t.wide_rows[g]) {
@@ -348,7 +352,8 @@ __global__ void __launch_bounds__(256) k_x_serve(const __grid_constant__ XView x
   __syncthreads();
   if (last && threadIdx.x == 0) {
     h->served_cnt[src] = total;
-    st_word8(&xhdr(x, src)->resp[x.me], total, epoch);
+    const unsigned bad = atomicExch(&h->range_src[src], 0u);  // every block's flag: they fenced before done_src
+    st_word16(&xhdr(x, src)->resp[x.me], total, (int)bad, 0, epoch);
     h->done_src[src] = 0;
   }
 }
@@ -361,7 +366,9 @@ __global__ void __launch_bounds__(256) k_x_unscatter(const __grid_constant__ XVi
   __shared__ int s_cnt, s_epoch;
   if (threadIdx.x == 0) {
     s_epoch = h->epoch;
-    s_cnt = poll8(&h->resp[owner], s_epoch, err).x;
+    const int4 r = poll16(&h->resp[owner], s_epoch, err);
+    s_cnt = r.x;
+    if (r.y && blockIdx.x == 0) atomicOr(err, kErrRange);  // an id I asked that owner for is outside the table
   }
   __syncthreads();
   const int cnt = s_cnt, epoch = s_epoch;
@@ -403,7 +410,7 @@ __global__ void __launch_bounds__(256) k_x_send_upd(const __grid_constant__ XVie
   const int owner = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
   const int epoch = h->epoch;
-  const int cnt = ld_word8(&h->resp[owner]).x;  // validated by this step's unscatter
+  const int cnt = ld_word16(&h->resp[owner]).x;  // validated by this step's unscatter
   const char* resp = xresp(x, x.me, owner);
   char* upd = xupd(x, owner, x.me);  // remote, contiguous
   const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;
@@ -442,13 +449,14 @@ __global__ void __launch_bounds__(256) k_x_send_upd(const __grid_constant__ XVie
   }
 }
 
-// Owner: apply the updates of source blockIdx.y to the rows served to it (its own ApplyGradients:
-// lr / Adam alpha were fixed by the source's push_begin on this shard).
+// Owner: apply the updates of source `src` to the rows served to it (its own ApplyGradients:
+// lr / Adam alpha were fixed by the source's push_begin on this shard).  One launch per source, in rank
+// order: two sources may update the same row in one step, and each launch reads what the one before it wrote,
+// so every source's update lands, as if the ranks had pushed one after the other.
 template <int OPT, int XU>
 __global__ void __launch_bounds__(256) k_x_apply(const __grid_constant__ XView x, const __grid_constant__ XTabs t, unsigned* err,
-                                                 const OptParams o) {
+                                                 const OptParams o, const int src) {
   constexpr int S = opt_slots(OPT);
-  const int src = blockIdx.y;
   XHeader* h = xhdr(x, x.me);
   __shared__ int s_epoch, s_cnt;
   __shared__ float s_lr, s_alpha, s_l2;

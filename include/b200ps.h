@@ -152,7 +152,11 @@ int b200ps_push_rows_pair(b200ps_t* ps, const b200ps_seg_t* segs_a, float* const
  * buffers of b200ps_unique.  create: collective, then re-export / import the shards (the exchange
  * buffer is a peer-mapped allocation).  push belongs between b200ps_push_begin and b200ps_push_end
  * and updates the rows of the b200ps_xchg_pull that precedes it (gsum indexed like that pull's
- * bet rows); a push without its pull returns B200PS_ESTATE.
+ * bet rows); a push without its pull returns B200PS_ESTATE.  A row that several ranks push in one
+ * step receives every rank's update, applied in rank order (rank 0's first), as if the ranks had
+ * pushed one after the other.  An id outside the table (negative, or >= the table's rows per shard
+ * x N) comes back as a zero row and makes the requesting rank's next b200ps_check fail with
+ * B200PS_ERANGE; a push leaves such a row alone.
  * create accepts 1 <= G <= B200PS_MAX_SEGS / 2 pairs of direct-indexed tables striped over every
  * shard (b200ps_table_register or b200ps_table_register_pair), with one slot layout among the
  * deep tables and one among the wide tables, and a process that owns exactly one shard.  It

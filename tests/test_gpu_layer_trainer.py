@@ -447,8 +447,9 @@ def test_multi_gpu_peer_shards_via_torchrun():
 @pytest.mark.parametrize("script,token", [("mgpu_xchg_check.py", "mgpu_xchg_check ok"),
                                           ("mgpu_allreduce_check.py", "mgpu_allreduce ok")])
 def test_multi_gpu_exchange_and_allreduce_via_torchrun(script, token):
-    """Owner-computes exchange (pull bit-exact vs direct peer access, push bit-exact vs the oracle) and the
-    allreduce controller incl. its fused reduce+update (NCCL with two GPUs; on one GPU the two ranks share it)."""
+    """Owner-computes exchange set-up (create refusals, a DeepFM engine training on it; its data paths are
+    tests/test_gpu_exchange_paths.py) and the allreduce controller incl. its fused reduce+update (NCCL with two
+    GPUs; on one GPU the two ranks share it)."""
     out = _torchrun_two_ranks(script, 29534)
     assert out.returncode == 0 and token in out.stdout, out.stdout[-3000:] + out.stderr[-3000:]
 
