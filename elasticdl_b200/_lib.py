@@ -146,7 +146,7 @@ SYMBOLS = {
     "b200_deepfm_tile_prologue": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
     "b200_deepfm_tile_main": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
     "b200_deepfm_tile_launch_count": (_i64, []),
-    "b200_deepfm_tile_last_error": (ctypes.c_char_p, []),
+    "b200_deepfm_last_error": (ctypes.c_char_p, []),
     # include/b200_features.h
     "b200feat_last_error": (ctypes.c_char_p, []),
     "b200feat_transform": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i64, _vp, _i, _vp, _vp]),

@@ -10,61 +10,28 @@
 //
 // fp32 throughout; no tensor cores (0.3 GFLOP per batch -- the kernel is bound by the
 // gather/scatter of embedding rows, not by math).
-#include <cuda_runtime.h>
-
-#include <string>
-
-#include "../../include/b200_deepfm.h"
+#include "deepfm_common.cuh"
 
 namespace {
 
-constexpr int ND = B200_DEEPFM_NDENSE, D = B200_DEEPFM_DIM, H1 = B200_DEEPFM_H1, H2 = B200_DEEPFM_H2;
-constexpr int SCR = B200_DEEPFM_SCRATCH;
-constexpr int WD_PAD = 16;  // w_dense padded to 16 floats
-
-struct Layout {
-  int in;  // ND + G*D
-  int o_wd, o_w1, o_b1, o_w2, o_b2, o_w3, total;
-};
-__host__ __device__ inline Layout layout(int G) {
-  Layout l;
-  l.in = ND + G * D;
-  l.o_wd = 0;
-  l.o_w1 = WD_PAD;
-  l.o_b1 = l.o_w1 + H1 * l.in;
-  l.o_w2 = l.o_b1 + H1;
-  l.o_b2 = l.o_w2 + H2 * H1;
-  l.o_w3 = l.o_b2 + H2;
-  l.total = l.o_w3 + H2;
-  return l;
-}
+using namespace deepfm;
 
 long long g_launches = 0;
-thread_local std::string g_msg;
 
 __global__ void __launch_bounds__(256) k_tower_prep(b200_deepfm_args_t a, int n_params) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (tid == 0) *a.loss = 0.f;
   if (blockIdx.y == 0) {
-    for (long long i = tid; i < n_params; i += stride) a.grads[i] = 0.f;
     // W1 transposed to [IN][16] once per step (behind the per-sample scratch): every k_tower_a block
     // then fills its shared memory with straight 16-byte copies instead of 5072 scattered stores
     const Layout l = layout(a.G);
-    float* w1t = a.scratch + (long long)a.B * SCR;
+    float* w1t = a.scratch + (long long)a.B * STATE;
     for (long long i = tid; i < (long long)H1 * l.in; i += stride) {
       const int j = (int)(i / l.in), e = (int)(i - (long long)j * l.in);
       w1t[e * H1 + j] = a.params[l.o_w1 + i];
     }
   }
-  // live rows only: rows >= n_unique[g] are never read by the push
-  for (int g = blockIdx.y; g < a.G; g += gridDim.y) {
-    const int u = a.n_unique[g];
-    float* gw = a.gsum_wide + (long long)g * a.B;
-    float4* gd = reinterpret_cast<float4*>(a.gsum_deep + (long long)g * a.B * D);
-    for (long long i = tid; i < u; i += stride) gw[i] = 0.f;
-    for (long long i = tid; i < 2LL * u; i += stride) gd[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+  zero_step_outputs(a, n_params);
 }
 
 // shared-memory copy of the parameters: W1 transposed to [IN][16] so that the 16 outputs of
@@ -173,7 +140,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a)
   SmemParams sp = carve(smem, l.in);
   float* red = smem + smem_floats(l.in);                       // [NPART][RW][SPB]
   int* sinv = reinterpret_cast<int*>(red + NPART * RW * SPB);  // [G][SPB]
-  load_params(a.params, BACKWARD ? a.scratch + (long long)a.B * SCR : nullptr, l, sp);
+  load_params(a.params, BACKWARD ? a.scratch + (long long)a.B * STATE : nullptr, l, sp);
   const int B = a.B, G = a.G;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int part = warp % NPART;
@@ -297,31 +264,11 @@ __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a)
       if (part == 0 && live[n] && a.logits != nullptr) a.logits[b] = z;
       dz[n] = 0.f;
       if (BACKWARD) {
-        const float y = a.labels[bb[n]];
-        const float lb = fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));  // BCE with logits
-        if (part == 0 && live[n]) loss_acc += lb;
-        const float p = 1.f / (1.f + expf(-z));
-        dz[n] = live[n] ? (p - y) / (float)B : 0.f;
         float dh2[H2];
-#pragma unroll
-        for (int k = 0; k < H2; ++k) dh2[k] = h2[k] > 0.f ? dz[n] * sp.w3[k] : 0.f;
-#pragma unroll
-        for (int j = 0; j < H1; ++j) {
-          float acc = 0.f;
-#pragma unroll
-          for (int k = 0; k < H2; ++k) acc = fmaf(sp.w2[k * H1 + j], dh2[k], acc);
-          dh1[n][j] = h[n][j] > 0.f ? acc : 0.f;
-        }
-        if (part == 0 && live[n]) {  // backward state for k_tower_b: [dh1 16 | a1 16 | dh2 4 | h2 4 | dz | pad 3]
-          float4* sc = reinterpret_cast<float4*>(a.scratch + b * SCR);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd)
-            sc[qd] = make_float4(dh1[n][4 * qd], dh1[n][4 * qd + 1], dh1[n][4 * qd + 2], dh1[n][4 * qd + 3]);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) sc[4 + qd] = make_float4(a1[4 * qd], a1[4 * qd + 1], a1[4 * qd + 2], a1[4 * qd + 3]);
-          sc[8] = make_float4(dh2[0], dh2[1], dh2[2], dh2[3]);
-          sc[9] = make_float4(h2[0], h2[1], h2[2], h2[3]);
-          sc[10] = make_float4(dz[n], 0.f, 0.f, 0.f);
+        const float lb = backward_tail(z, a.labels[bb[n]], live[n], B, h[n], h2, sp.w2, sp.w3, dz[n], dh2, dh1[n]);
+        if (part == 0 && live[n]) {
+          loss_acc += lb;
+          store_state(a.scratch + b * STATE, dh1[n], a1, dh2, h2, dz[n]);  // backward state for k_tower_b
         }
       }
     }
@@ -356,42 +303,14 @@ __global__ void __launch_bounds__(TA_THREADS, 2) k_tower_a(b200_deepfm_args_t a)
 #pragma unroll
         for (int n = 0; n < NS; ++n) {
           x[n][D] = dz[n];  // wide row gradient
-          // warp-level id dedup: lanes hitting the same row combine pairwise up a tree threaded
-          // through the peer mask (pointer doubling), ceil(log2(max multiplicity)) rounds for the
-          // whole warp -- the small tables of this model put ~10 equal ids in every warp
-          const int key = live[n] ? r[n] : -1 - lane;
-          const unsigned peers = __match_any_sync(0xffffffffu, key);
-          const int rank = __popc(peers & ((1u << lane) - 1));
-          const bool leader = rank == 0;
-          const int maxn = __reduce_max_sync(0xffffffffu, (unsigned)__popc(peers));
-          const unsigned above = peers & ~((2u << lane) - 1);
-          int nxt = above ? __ffs(above) - 1 : -1;  // peer `step` ranks above me
-          for (int step = 1; step < maxn; step <<= 1) {
-            const int src = nxt >= 0 ? nxt : lane;
-            const bool take = nxt >= 0 && (rank & (2 * step - 1)) == 0;
-#pragma unroll
-            for (int e = 0; e <= D; ++e) {
-              const float yv = __shfl_sync(0xffffffffu, x[n][e], src);
-              if (take) x[n][e] += yv;
-            }
-            const int nn = __shfl_sync(0xffffffffu, nxt, src);
-            nxt = nxt >= 0 ? nn : -1;
-          }
-          if (live[n] && leader) {
-            float* od = a.gsum_deep + ((long long)g * B + r[n]) * D;
-            atomicAdd(reinterpret_cast<float4*>(od), make_float4(x[n][0], x[n][1], x[n][2], x[n][3]));
-            atomicAdd(reinterpret_cast<float4*>(od + 4), make_float4(x[n][4], x[n][5], x[n][6], x[n][7]));
-            atomicAdd(a.gsum_wide + (long long)g * B + r[n], x[n][D]);
-          }
+          // the small tables of this model put ~10 equal ids in every warp
+          dedup_red(x[n], r[n], live[n], lane, a, g);
         }
       }
     }
     __syncthreads();  // red / sinv are reused by the next block of samples
   }
-  if (BACKWARD) {
-    for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_down_sync(0xffffffffu, loss_acc, o);
-    if (lane == 0 && part == 0) atomicAdd(a.loss, loss_acc / (float)B);
-  }
+  if (BACKWARD) add_warp_loss(loss_acc, a.loss, B, lane == 0 && part == 0);
 }
 
 __host__ inline size_t tower_a_smem(int G) {
@@ -407,12 +326,11 @@ constexpr int S_CHUNK = 32;  // 52 KB of shared memory per block -> 4 blocks (16
 constexpr int TB_COLW = 96;                    // threads owning dW1/db1 columns (3 warps)
 constexpr int TB_CPT = 4;                      // columns per thread: each staged dh1 row feeds 64 FMAs
 constexpr int TB_THREADS = TB_COLW + 32;       // + one warp for the small gradients
-constexpr int N_SMALL = H2 * H1 + H2 + H2 + ND;  // dW2 64 | db2 4 | dw3 4 | dw_dense 13
 
 // tile row: [deep G*8 | dense 13 | 1.0 (bias column) | pad]
 __host__ __device__ inline int tb_xpad(int G) { return (G * D + ND + 1 + 3) / 4 * 4; }
 __host__ inline size_t tower_b_smem(int G) {
-  return ((size_t)S_CHUNK * SCR + (size_t)S_CHUNK * tb_xpad(G)) * sizeof(float) + (size_t)G * S_CHUNK * sizeof(int);
+  return ((size_t)S_CHUNK * STATE + (size_t)S_CHUNK * tb_xpad(G)) * sizeof(float) + (size_t)G * S_CHUNK * sizeof(int);
 }
 
 __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a) {
@@ -420,8 +338,8 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
   const Layout l = layout(a.G);
   const int B = a.B, G = a.G, t = threadIdx.x;
   const int IN = l.in, XP = tb_xpad(G), NDEEP = G * D, NCOL = IN + 1;
-  float* sc = smem_b;                                     // [S][SCR]
-  float* xt = sc + S_CHUNK * SCR;                         // [S][XP]
+  float* sc = smem_b;                                     // [S][STATE]
+  float* xt = sc + S_CHUNK * STATE;                         // [S][XP]
   int* sinv = reinterpret_cast<int*>(xt + S_CHUNK * XP);  // [G][S]
   const bool is_col = t < TB_COLW;
   float acc[TB_CPT][H1];
@@ -436,9 +354,9 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
     const int n = (int)min((long long)S_CHUNK, B - b0);
     __syncthreads();
     {
-      const float4* src = reinterpret_cast<const float4*>(a.scratch + b0 * SCR);
+      const float4* src = reinterpret_cast<const float4*>(a.scratch + b0 * STATE);
       float4* dst = reinterpret_cast<float4*>(sc);
-      for (int i = t; i < n * (SCR / 4); i += TB_THREADS) dst[i] = src[i];
+      for (int i = t; i < n * (STATE / 4); i += TB_THREADS) dst[i] = src[i];
       for (int i = t; i < n * (ND + 1); i += TB_THREADS) {
         const int s_ = i / (ND + 1), e = i - s_ * (ND + 1);
         xt[s_ * XP + NDEEP + e] = e < ND ? a.dense[(b0 + s_) * ND + e] : 1.0f;
@@ -462,7 +380,7 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
     if (is_col) {
 #pragma unroll 2
       for (int s_ = 0; s_ < n; ++s_) {
-        const float4* d4 = reinterpret_cast<const float4*>(sc + s_ * SCR);
+        const float4* d4 = reinterpret_cast<const float4*>(sc + s_ * STATE);
         const float4 q0 = d4[0], q1 = d4[1], q2 = d4[2], q3 = d4[3];
         const float dh[H1] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
 #pragma unroll
@@ -475,16 +393,11 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
       }
     } else {
       for (int s_ = 0; s_ < n; ++s_) {
-        const float* r = sc + s_ * SCR;
+        const float* r = sc + s_ * STATE;
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
           const int small = (t - TB_COLW) + 32 * i;
-          float v = 0.f;
-          if (small < H2 * H1) v = r[32 + small / H1] * r[16 + small % H1];             // dh2[k] * a1[j]
-          else if (small < H2 * H1 + H2) v = r[32 + small - H2 * H1];                    // dh2[k]
-          else if (small < H2 * H1 + 2 * H2) v = r[40] * r[36 + small - H2 * H1 - H2];   // dz * h2[k]
-          else if (small < N_SMALL) v = r[40] * xt[s_ * XP + NDEEP + small - H2 * H1 - 2 * H2];  // dz * dense[e]
-          sacc[i] += v;
+          if (small < NSMALL) sacc[i] += small_grad(small, r, xt + s_ * XP + NDEEP);
         }
       }
     }
@@ -506,27 +419,22 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       const int small = (t - TB_COLW) + 32 * i;
-      if (small >= N_SMALL) continue;
-      int off;
-      if (small < H2 * H1) off = l.o_w2 + small;
-      else if (small < H2 * H1 + H2) off = l.o_b2 + small - H2 * H1;
-      else if (small < H2 * H1 + 2 * H2) off = l.o_w3 + small - H2 * H1 - H2;
-      else off = l.o_wd + small - H2 * H1 - 2 * H2;
-      atomicAdd(a.grads + off, sacc[i]);
+      if (small < NSMALL) atomicAdd(a.grads + small_grad_offset(l, small), sacc[i]);
     }
   }
 }
 
 int check_args(const b200_deepfm_args_t* a, bool backward) {
-  if (!a || a->G < 1 || a->B < 1) { g_msg = "bad shape"; return -1; }
-  if (ND + a->G * D + 1 > TB_COLW * TB_CPT) { g_msg = "too many id groups for the fused tower (max 46)"; return -1; }
-  if (!a->inv || !a->bet_wide || !a->bet_deep || !a->dense || !a->params) { g_msg = "null input"; return -1; }
-  if (a->rows) { g_msg = "the fused tower reads pulled rows only"; return -1; }
-  if (backward && (!a->labels || !a->grads || !a->gsum_wide || !a->gsum_deep || !a->loss || !a->scratch || !a->n_unique)) {
-    g_msg = "null output";
-    return -1;
-  }
+  if (check_common(a, backward)) return -1;
+  if (ND + a->G * D + 1 > TB_COLW * TB_CPT) return fail(-1, "too many id groups for the fused tower (max 46)");
+  if (a->rows) return fail(-1, "the fused tower reads pulled rows only");
+  if (backward && !a->scratch) return fail(-1, "null output");
   return 0;
+}
+
+unsigned tower_a_grid(int B, int n_sm) {
+  const long long blocks = ((long long)B + SPB - 1) / SPB, cap = (long long)n_sm * 8;
+  return (unsigned)(blocks < cap ? blocks : cap);
 }
 
 }  // namespace
@@ -535,56 +443,33 @@ extern "C" {
 
 size_t b200_deepfm_param_count(int G) { return (size_t)layout(G).total; }
 int64_t b200_deepfm_launch_count(void) { return g_launches; }
+const char* b200_deepfm_last_error(void) { return last_error().c_str(); }
 
 int b200_deepfm_fwd_bwd(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, true)) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = layout(args->G);
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  const size_t smem = tower_a_smem(args->G);
-  static bool attr_done[64] = {false};
-  if (dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(k_tower_a<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    cudaFuncSetAttribute(k_tower_a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    attr_done[dev] = true;
-  }
-  dim3 gp(8, args->G);
-  k_tower_prep<<<gp, 256, 0, st>>>(*args, l.total);
-  long long blocks = ((long long)args->B + SPB - 1) / SPB;
-  long long cap = (long long)n_sm * 8;
-  k_tower_a<true><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
-  long long chunks = ((long long)args->B + S_CHUNK - 1) / S_CHUNK;
-  cap = (long long)n_sm * 4;  // 4 blocks per SM by shared memory / registers
-  static bool attr_b[64] = {false};
-  if (dev < 64 && !attr_b[dev]) {
-    cudaFuncSetAttribute(k_tower_b, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    attr_b[dev] = true;
-  }
+  int n_sm;
+  const int dev = current_device(&n_sm);
+  max_dynamic_smem_once<k_tower_a<true>>(dev, 110 * 1024);
+  max_dynamic_smem_once<k_tower_b>(dev, 110 * 1024);
+  k_tower_prep<<<dim3(8, args->G), 256, 0, st>>>(*args, l.total);
+  k_tower_a<true><<<tower_a_grid(args->B, n_sm), TA_THREADS, tower_a_smem(args->G), st>>>(*args);
+  const long long chunks = ((long long)args->B + S_CHUNK - 1) / S_CHUNK;
+  const long long cap = (long long)n_sm * 4;  // 4 blocks per SM by shared memory / registers
   k_tower_b<<<(unsigned)(chunks < cap ? chunks : cap), TB_THREADS, tower_b_smem(args->G), st>>>(*args);
   g_launches += 3;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
-  return 0;
+  return launch_status();
 }
 
 int b200_deepfm_forward(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, false) || !args->logits) return -1;
-  cudaStream_t st = (cudaStream_t)stream;
-  const Layout l = layout(args->G);
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  const size_t smem = tower_a_smem(args->G);
-  cudaFuncSetAttribute(k_tower_a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-  long long blocks = ((long long)args->B + SPB - 1) / SPB;
-  long long cap = (long long)n_sm * 8;
-  k_tower_a<false><<<(unsigned)(blocks < cap ? blocks : cap), TA_THREADS, smem, st>>>(*args);
+  if (check_args(args, false)) return -1;
+  int n_sm;
+  const int dev = current_device(&n_sm);
+  max_dynamic_smem_once<k_tower_a<false>>(dev, 110 * 1024);
+  k_tower_a<false><<<tower_a_grid(args->B, n_sm), TA_THREADS, tower_a_smem(args->G), (cudaStream_t)stream>>>(*args);
   g_launches += 1;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
-  return 0;
+  return launch_status();
 }
 
 }  // extern "C"

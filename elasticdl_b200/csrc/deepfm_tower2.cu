@@ -25,16 +25,12 @@
 // with straight 16-byte copies.  fp32 SIMT: the step has 1 GFLOP of first-layer work, and the kernel waits on
 // the gather round trip and on its per-tile phases and barriers, not on FMA throughput (DESIGN.md section 10:
 // a 3xTF32 mma.sync version of F / B1 / B2 measured slower).
-#include <cuda_runtime.h>
-
-#include <string>
-
-#include "../../include/b200_deepfm.h"
+#include "deepfm_common.cuh"
 
 namespace {
 
-constexpr int ND = B200_DEEPFM_NDENSE, D = B200_DEEPFM_DIM, H1 = B200_DEEPFM_H1, H2 = B200_DEEPFM_H2;
-constexpr int WD_PAD = 16;
+using namespace deepfm;
+
 constexpr int TS = 32;        // samples per tile
 constexpr int THREADS = 256;  // 8 warps
 constexpr int NKP = 8;        // column parts (warps) of phases F / B1
@@ -43,36 +39,17 @@ constexpr int NCOL = 320;     // deep 304 | dense 13 | 1 | 0 0   (G <= 38)
 constexpr int XS = 324;       // row stride: 320 + pad = 81 * 4 (odd number of 16 B quads: conflict-free 128-bit row reads)
 constexpr int RS = 39;        // rank row stride (odd): Rt[s][g]
 constexpr int RW = H1 + D + 2;  // partial record: h[16] | s[8] | q | lin
-constexpr int MS = 44;        // per-sample backward state: dh1 16 | a1 16 | dh2 4 | h2 4 | dz | pad 3
 constexpr int MAXG = 38;
-constexpr int NSMALL = H2 * H1 + 2 * H2 + ND;  // small gradients: dW2 64 | db2 4 | dw3 4 | dwd 13
 constexpr int SPART = 3;                       // threads per small gradient (255 threads, 11 samples each)
 constexpr int SPLEN = (TS + SPART - 1) / SPART;
 static_assert(NKP * KPC == NCOL && (NKP - 1) * KPC <= MAXG * D, "the last warp owns the dense block");
 
-struct Layout {
-  int in, o_wd, o_w1, o_b1, o_w2, o_b2, o_w3, total;
-};
-__host__ __device__ inline Layout layout(int G) {
-  Layout l;
-  l.in = ND + G * D;
-  l.o_wd = 0;
-  l.o_w1 = WD_PAD;
-  l.o_b1 = l.o_w1 + H1 * l.in;
-  l.o_w2 = l.o_b1 + H1;
-  l.o_b2 = l.o_w2 + H2 * H1;
-  l.o_w3 = l.o_b2 + H2;
-  l.total = l.o_w3 + H2;
-  return l;
-}
-
 long long g_launches = 0;
-thread_local std::string g_msg;
 
 // shared memory carve-up (floats)
 constexpr int SM_W1X = NCOL * H1;          // 5120
 constexpr int SM_X = TS * XS;              // 11648
-constexpr int SM_P = NKP * RW * TS;        // 6656   partial records [kp][r][s]; reused as T[r][s] + M[s][MS]
+constexpr int SM_P = NKP * RW * TS;        // 6656   partial records [kp][r][s]; reused as T[r][s] + M[s][STATE]
 constexpr int SM_R = 2 * TS * RS;          // 2496   ranks Rt[buffer][s][g]: this tile's and the prefetched next tile's
 constexpr int SM_WV = MAXG * TS;           // 1216   wide values WV[g][s]
 constexpr int SM_SMALL = 128;              // b... w2 64 | b2 4 | w3 4 | wd 16
@@ -88,15 +65,6 @@ struct TileRows {
   long long deep_stride, wide_stride;
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 // Two hidden units per call: two independent round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
   return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
@@ -114,11 +82,8 @@ __host__ __device__ inline int w1x_src(const Layout& l, int G, int c, int j) {
 __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_params, float* w1x, int main_grid) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (tid == 0 && a.loss) *a.loss = 0.f;
-  if (tid == 0 && blockIdx.y == 0) reinterpret_cast<int*>(w1x + NCOL * H1)[0] = main_grid;  // dynamic tile counter
-  if (blockIdx.y == 0) {
-    if (a.grads)
-      for (long long i = tid; i < n_params; i += stride) a.grads[i] = 0.f;
+  if (blockIdx.y == 0) {  // the dynamic tile counter and W1 in tile column order
+    if (tid == 0) reinterpret_cast<int*>(w1x + NCOL * H1)[0] = main_grid;
     const Layout l = layout(a.G);
     for (long long i = tid; i < (long long)NCOL * H1; i += stride) {
       const int c = (int)(i / H1), j = (int)(i - (long long)c * H1);
@@ -126,14 +91,7 @@ __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_p
       w1x[i] = src >= 0 ? a.params[src] : 0.f;
     }
   }
-  if (a.gsum_deep == nullptr) return;
-  for (int g = blockIdx.y; g < a.G; g += gridDim.y) {  // live rows only: rows >= n_unique[g] are never read by the push
-    const int u = a.n_unique[g];
-    float* gw = a.gsum_wide + (long long)g * a.B;
-    float4* gd = reinterpret_cast<float4*>(a.gsum_deep + (long long)g * a.B * D);
-    for (long long i = tid; i < u; i += stride) gw[i] = 0.f;
-    for (long long i = tid; i < 2LL * u; i += stride) gd[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+  zero_step_outputs(a, n_params);
 }
 
 // TABLE: the rows come straight from the tables' record slabs (TileRows) instead of bet_deep / bet_wide, which
@@ -147,7 +105,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   extern __shared__ __align__(16) float smem[];
   float* W1x = smem;                 // [NCOL][16]
   float* X = W1x + SM_W1X;           // [TS][XS]
-  float* P = X + SM_X;               // [NKP][RW][TS], later T[RW][TS] and Mst[TS][MS]
+  float* P = X + SM_X;               // [NKP][RW][TS], later T[RW][TS] and Mst[TS][STATE]
   int* Rt0 = reinterpret_cast<int*>(P + SM_P);  // [2][TS][RS] ranks
   float* WV = reinterpret_cast<float*>(Rt0 + SM_R);  // [G][TS] wide values
   float* small = WV + SM_WV;
@@ -157,7 +115,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   float* s_wd = small + 72;   // [ND]
   int* Ut = reinterpret_cast<int*>(small + SM_SMALL);  // TABLE: [TS][RS] low words of the ids (< 2^31, direct-indexed)
   float* T = P;                          // [RW][TS] summed records (first RW*TS floats of P)
-  float* Mst = P + RW * TS + 64;         // [TS][MS] per-sample backward state for B2 (after T, 16 B aligned)
+  float* Mst = P + RW * TS + 64;         // [TS][STATE] per-sample backward state for B2 (after T, 16 B aligned)
 
   const Layout l = layout(a.G);
   const int B = a.B, G = a.G;
@@ -340,25 +298,14 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
 #pragma unroll
     for (int d = 0; d < D; ++d) sd[d] = T[(H1 + d) * TS + lane];
     const float q = T[(H1 + D) * TS + lane], lin = T[(H1 + D + 1) * TS + lane];
-    float a1[H1];
-#pragma unroll
-    for (int j = 0; j < H1; ++j) a1[j] = fmaxf(hpre[j], 0.f);
-    float h2[H2], dnn = 0.f;
-#pragma unroll
-    for (int k = 0; k < H2; ++k) {
-      float accv = s_b2[k];
-#pragma unroll
-      for (int j = 0; j < H1; ++j) accv = fmaf(s_w2[k * H1 + j], a1[j], accv);
-      h2[k] = fmaxf(accv, 0.f);
-      dnn = fmaf(s_w3[k], h2[k], dnn);
-    }
-    float ss = 0.f;
-#pragma unroll
-    for (int d = 0; d < D; ++d) ss = fmaf(sd[d], sd[d], ss);
-    const float z = lin + dnn + 0.5f * (ss - q);
+    float a1[H1], h2[H2];
+    const float z = forward_tail(hpre, sd, q, lin, s_w2, s_b2, s_w3, a1, h2);
     if (warp == 0 && live && a.logits != nullptr) a.logits[b0 + lane] = z;
     float dz = 0.f, dh1[H1];
     if (BACKWARD) {
+      // The backward tail, the state record store and the dedup tree below are deepfm_common.cuh's backward_tail,
+      // store_state and dedup_red written out: called as helpers they change this kernel's register allocation
+      // (more spills in the training instances), so here they stay inline.
       const long long bb = live ? b0 + lane : B - 1;
       const float y = a.labels[bb];
       const float lb = fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));  // BCE with logits
@@ -375,8 +322,9 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         for (int k = 0; k < H2; ++k) accv = fmaf(s_w2[k * H1 + j], dh2[k], accv);
         dh1[j] = hpre[j] > 0.f ? accv : 0.f;
       }
-      if (warp == 0) {  // backward state for B2 (T's region is not overwritten: Mst lies behind it)
-        float4* m4 = reinterpret_cast<float4*>(Mst + lane * MS);
+      // backward state for B2 (T's region is not overwritten: Mst lies behind it)
+      if (warp == 0) {
+        float4* m4 = reinterpret_cast<float4*>(Mst + lane * STATE);
 #pragma unroll
         for (int qd = 0; qd < 4; ++qd) m4[qd] = make_float4(dh1[4 * qd], dh1[4 * qd + 1], dh1[4 * qd + 2], dh1[4 * qd + 3]);
 #pragma unroll
@@ -410,8 +358,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
           x[d] = fmaf(dz, sd[d] - ev[d], dt2.x + dt2.y);
         }
         x[D] = dz;  // wide row gradient
-        // warp-level id dedup: lanes hitting the same row combine pairwise up a tree threaded through the
-        // peer mask (pointer doubling): ceil(log2(max multiplicity)) rounds for the whole warp
+        // warp-level id dedup (dedup_red): lanes hitting the same row combine pairwise up a tree threaded through
+        // the peer mask (pointer doubling): ceil(log2(max multiplicity)) rounds for the whole warp
         const int r = Rt[lane * RS + g];
         const int key = live ? r : -1 - lane;
         const unsigned peers = __match_any_sync(0xffffffffu, key);
@@ -444,7 +392,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         const int c1 = 256 + (t & 63), jsel = t >> 6;
 #pragma unroll 4
         for (int s = 0; s < TS; ++s) {
-          const float4* d4 = reinterpret_cast<const float4*>(Mst + s * MS);
+          const float4* d4 = reinterpret_cast<const float4*>(Mst + s * STATE);
           const float4 q0 = d4[0], q1 = d4[1], q2 = d4[2], q3 = d4[3];
           const float dh[H1] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
           const float x0 = X[s * XS + t], x1 = X[s * XS + c1];
@@ -458,13 +406,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         if (t < SPART * NSMALL) {  // output t % NSMALL over a third of the samples
           const int o = t % NSMALL, s0 = (t / NSMALL) * SPLEN, s1 = min(TS, s0 + SPLEN);
           for (int s = s0; s < s1; ++s) {
-            const float* m = Mst + s * MS;
-            float v;
-            if (o < H2 * H1) v = m[32 + o / H1] * m[16 + o % H1];                         // dh2[k] * a1[j]
-            else if (o < H2 * H1 + H2) v = m[32 + o - H2 * H1];                            // dh2[k]
-            else if (o < H2 * H1 + 2 * H2) v = m[40] * m[36 + o - H2 * H1 - H2];           // dz * h2[k]
-            else v = m[40] * X[s * XS + MAXG * D + o - H2 * H1 - 2 * H2];                  // dz * dense[e]
-            sacc += v;
+            const float* m = Mst + s * STATE;
+            sacc += small_grad(o, m, X + s * XS + MAXG * D);
           }
         }
       }
@@ -484,19 +427,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
     }
     if (t < SPART * NSMALL) P[t] = sacc;  // P is free: every thread has left the tile loop
     __syncthreads();
-    if (t < NSMALL) {
-      const int o = t;
-      int off;
-      if (o < H2 * H1) off = l.o_w2 + o;
-      else if (o < H2 * H1 + H2) off = l.o_b2 + o - H2 * H1;
-      else if (o < H2 * H1 + 2 * H2) off = l.o_w3 + o - H2 * H1 - H2;
-      else off = l.o_wd + o - H2 * H1 - 2 * H2;
-      atomicAdd(a.grads + off, P[o] + P[NSMALL + o] + P[2 * NSMALL + o]);
-    }
-    if (warp == 0) {
-      for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_down_sync(0xffffffffu, loss_acc, o);
-      if (lane == 0) atomicAdd(a.loss, loss_acc / (float)B);
-    }
+    if (t < NSMALL) atomicAdd(a.grads + small_grad_offset(l, t), P[t] + P[NSMALL + t] + P[2 * NSMALL + t]);
+    if (warp == 0) add_warp_loss(loss_acc, a.loss, B, lane == 0);
   }
 }
 
@@ -510,29 +442,18 @@ __global__ void k_publish_loss(const float* __restrict__ loss, float* ring, int 
 }
 
 int check_args(const b200_deepfm_args_t* a, bool backward) {
-  if (!a || a->G < 1 || a->B < 1) { g_msg = "bad shape"; return -1; }
-  if (a->G > MAXG) { g_msg = "the tile tower holds at most 38 id groups"; return -1; }
-  if (!a->inv || !a->dense || !a->params || !a->scratch || (!a->rows && (!a->bet_wide || !a->bet_deep))) {
-    g_msg = "null input";
-    return -1;
-  }
-  if (backward && (!a->labels || !a->grads || !a->gsum_wide || !a->gsum_deep || !a->loss || !a->n_unique)) {
-    g_msg = "null output";
-    return -1;
-  }
+  if (check_common(a, backward)) return -1;
+  if (a->G > MAXG) return fail(-1, "the tile tower holds at most 38 id groups");
+  if (!a->scratch) return fail(-1, "null input");
   if (a->rows) {
     const b200_deepfm_rows_t* r = a->rows;
-    if (!backward) { g_msg = "the forward-only tile tower reads pulled rows only"; return -1; }
+    if (!backward) return fail(-1, "the forward-only tile tower reads pulled rows only");
     if (!r->uniq || r->deep_stride < D || r->wide_stride < 1 || r->deep_param_off < 0 || r->wide_param_off < 0 ||
-        r->deep_stride % 4 || r->deep_param_off % 4) {
-      g_msg = "bad row source";
-      return -1;
-    }
+        r->deep_stride % 4 || r->deep_param_off % 4)
+      return fail(-1, "bad row source");
     for (int g = 0; g < a->G; ++g)
-      if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15)) {
-        g_msg = "bad row source";
-        return -1;
-      }
+      if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15))
+        return fail(-1, "bad row source");
   }
   return 0;
 }
@@ -540,11 +461,7 @@ int check_args(const b200_deepfm_args_t* a, bool backward) {
 template <bool BACKWARD, bool TABLE>
 void launch_tile(int dev, unsigned grid, cudaStream_t st, const b200_deepfm_args_t& a, const float* w1x, const TileRows& rows) {
   constexpr size_t smem = SMEM_BYTES + (TABLE ? SM_U * sizeof(int) : 0);
-  static bool attr_done[64] = {};
-  if (dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(k_tower_tile<BACKWARD, TABLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    attr_done[dev] = true;
-  }
+  max_dynamic_smem_once<k_tower_tile<BACKWARD, TABLE>>(dev, (int)smem);
   k_tower_tile<BACKWARD, TABLE><<<grid, THREADS, smem, st>>>(a, w1x, rows);
 }
 
@@ -552,9 +469,8 @@ void launch_tile(int dev, unsigned grid, cudaStream_t st, const b200_deepfm_args
 template <bool BACKWARD>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
   cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  int n_sm;
+  const int dev = current_device(&n_sm);
   b200_deepfm_args_t a = *args;
   if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
   float* w1x = a.scratch;  // NCOL*16 floats at the start of the scratch buffer, then the tile counter
@@ -565,11 +481,7 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
     k_tile_prep<<<dim3(4, BACKWARD ? a.G : 1), 256, 0, st>>>(a, layout(a.G).total, w1x, (int)grid);
     g_launches += 1;
   }
-  if (!(what & 2)) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
-    return 0;
-  }
+  if (!(what & 2)) return launch_status();
   TileRows rows{};
   if constexpr (BACKWARD) {  // only the training entry points accept a row source (check_args)
     if (const b200_deepfm_rows_t* r = args->rows) {
@@ -588,9 +500,7 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
     launch_tile<false, false>(dev, (unsigned)grid, st, *args, w1x, rows);
   }
   g_launches += 1;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
-  return 0;
+  return launch_status();
 }
 
 }  // namespace
@@ -598,7 +508,6 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
 extern "C" {
 
 int64_t b200_deepfm_tile_launch_count(void) { return g_launches; }
-const char* b200_deepfm_tile_last_error(void) { return g_msg.c_str(); }
 
 int b200_deepfm_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, true)) return -1;
@@ -616,16 +525,14 @@ int b200_deepfm_tile_main(const b200_deepfm_args_t* args, void* stream) {
 }
 
 int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int ring_len, unsigned* cursor_dev, void* stream) {
-  if (!loss_dev || !ring_host_mapped || ring_len < 1 || !cursor_dev) { g_msg = "bad publish_loss arguments"; return -1; }
+  if (!loss_dev || !ring_host_mapped || ring_len < 1 || !cursor_dev) return fail(-1, "bad publish_loss arguments");
   k_publish_loss<<<1, 1, 0, (cudaStream_t)stream>>>(loss_dev, ring_host_mapped, ring_len, cursor_dev);
   g_launches += 1;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { g_msg = cudaGetErrorString(e); return -2; }
-  return 0;
+  return launch_status();
 }
 
 int b200_deepfm_forward_tile(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, false) || !args->logits) return -1;
+  if (check_args(args, false)) return -1;
   return launch<false>(args, stream);
 }
 

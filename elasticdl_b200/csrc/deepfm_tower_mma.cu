@@ -14,38 +14,17 @@
 // BCE, backward to dH1) runs one thread per sample between the GEMMs.  Embedding-row gradients
 // leave the accumulator fragments through a warp-level id dedup (equal rows of a half-tile combine
 // up a tree threaded through the __match_any_sync mask) and vector atomics.
-#include <cuda_runtime.h>
-
-#include <cstdint>
-#include <string>
-
-#include "../../include/b200_deepfm.h"
+#include "deepfm_common.cuh"
 
 namespace {
 
-constexpr int ND = B200_DEEPFM_NDENSE, D = B200_DEEPFM_DIM, H1 = B200_DEEPFM_H1, H2 = B200_DEEPFM_H2;
+using namespace deepfm;
+
 constexpr int MT = 32;                 // samples per chunk: two m16 tiles
 constexpr int THREADS = 128;           // 4 warps
 constexpr int MAX_NT_W = 12;           // dW1 n-tiles per warp (KP/8 <= 48 -> G <= 46)
 constexpr int IPT = 12;                // groups gathered per thread per chunk (4 warps x 12 >= 46)
 constexpr int HS = 17, DHS = 20, SS = 12, SMS = 8;  // strides of the small per-sample buffers
-constexpr int N_SMALL = H2 * H1 + H2 + H2 + ND;      // dW2 64 | db2 4 | dw3 4 | dw_dense 13
-
-struct Layout {
-  int in, o_wd, o_w1, o_b1, o_w2, o_b2, o_w3, total;
-};
-__host__ __device__ inline Layout layout(int G) {
-  Layout l;
-  l.in = ND + G * D;
-  l.o_wd = 0;
-  l.o_w1 = 16;
-  l.o_b1 = l.o_w1 + H1 * l.in;
-  l.o_w2 = l.o_b1 + H1;
-  l.o_b2 = l.o_w2 + H2 * H1;
-  l.o_w3 = l.o_b2 + H2;
-  l.total = l.o_w3 + H2;
-  return l;
-}
 
 struct Tile {
   int ndeep, cb, kp, xs;  // deep columns, bias column, padded K, row stride
@@ -64,13 +43,6 @@ __host__ inline size_t mma_smem_bytes(int G) {
   return f * sizeof(float) + (size_t)G * MT * sizeof(int);
 }
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  const unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-  asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-}
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -144,7 +116,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_mma(b200_deepfm_args_t a) 
   for (int q = 0; q < MAX_NT_W; ++q)
 #pragma unroll
     for (int e = 0; e < 4; ++e) acc[q][e] = 0.f;
-  float sacc = 0.f;      // small gradient owned by thread tid < N_SMALL
+  float sacc = 0.f;      // small gradient owned by thread tid < NSMALL
   float loss_acc = 0.f;  // threads < MT
   const int ntiles = KP / 8;
   const long long nchunk = ((long long)B + MT - 1) / MT;
@@ -241,39 +213,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_mma(b200_deepfm_args_t a) 
         for (int e = 0; e < ND; ++e) lt = fmaf(sp[72 + e], Xs[s * XS + NDEEP + e], lt);
         float h[H1], a1[H1];
 #pragma unroll
-        for (int j = 0; j < H1; ++j) {
-          h[j] = Hs[s * HS + j];
-          a1[j] = fmaxf(h[j], 0.f);
-        }
-        float dnn = 0.f;
-#pragma unroll
-        for (int k = 0; k < H2; ++k) {
-          float t = sp[64 + k];
-#pragma unroll
-          for (int j = 0; j < H1; ++j) t = fmaf(sp[k * H1 + j], a1[j], t);
-          h2[k] = fmaxf(t, 0.f);
-          dnn = fmaf(sp[68 + k], h2[k], dnn);
-        }
-        float ssq = 0.f;
-#pragma unroll
-        for (int d_ = 0; d_ < D; ++d_) ssq = fmaf(fs[d_], fs[d_], ssq);
-        const float z = lt + dnn + 0.5f * (ssq - q);
+        for (int j = 0; j < H1; ++j) h[j] = Hs[s * HS + j];
+        const float z = forward_tail(h, fs, q, lt, sp, sp + 64, sp + 68, a1, h2);
         if (a.logits != nullptr) a.logits[b0 + s] = z;
-        if (BACKWARD) {
-          const float y = a.labels[b0 + s];
-          loss_acc += fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));  // BCE with logits
-          const float p = 1.f / (1.f + expf(-z));
-          dz = (p - y) / (float)B;
-#pragma unroll
-          for (int k = 0; k < H2; ++k) dh2[k] = h2[k] > 0.f ? dz * sp[68 + k] : 0.f;
-#pragma unroll
-          for (int j = 0; j < H1; ++j) {
-            float t = 0.f;
-#pragma unroll
-            for (int k = 0; k < H2; ++k) t = fmaf(sp[k * H1 + j], dh2[k], t);
-            dh1[j] = h[j] > 0.f ? t : 0.f;
-          }
-        }
+        if (BACKWARD) loss_acc += backward_tail(z, a.labels[b0 + s], true, B, h, h2, sp, sp + 68, dz, dh2, dh1);
       }
       lin[s] = 0.f;  // ready for the next chunk's atomics
 #pragma unroll
@@ -365,7 +308,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_mma(b200_deepfm_args_t a) 
       }
     }
     // small gradients: dW2 64 | db2 4 | dw3 4 | dw_dense 13, thread per output
-    if (tid < N_SMALL) {
+    if (tid < NSMALL) {  // the small_grad of deepfm_common.cuh, read from this kernel's per-sample buffers
       for (int s = 0; s < n; ++s) {
         float v;
         if (tid < H2 * H1) v = Sm[s * SMS + tid / H1] * fmaxf(Hs[s * HS + tid % H1], 0.f);   // dh2[k] * a1[j]
@@ -392,36 +335,12 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_mma(b200_deepfm_args_t a) 
       if (off >= 0) atomicAdd(a.grads + off, acc[q][e]);
     }
   }
-  if (tid < N_SMALL) {
-    int off;
-    if (tid < H2 * H1) off = l.o_w2 + tid;
-    else if (tid < H2 * H1 + H2) off = l.o_b2 + tid - H2 * H1;
-    else if (tid < H2 * H1 + 2 * H2) off = l.o_w3 + tid - H2 * H1 - H2;
-    else off = l.o_wd + tid - H2 * H1 - 2 * H2;
-    atomicAdd(a.grads + off, sacc);
-  }
-  if (warp == 0) {  // MT == 32: the per-sample threads are warp 0
-    for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_down_sync(0xffffffffu, loss_acc, o);
-    if (lane == 0) atomicAdd(a.loss, loss_acc / (float)B);
-  }
+  if (tid < NSMALL) atomicAdd(a.grads + small_grad_offset(l, tid), sacc);
+  if (warp == 0) add_warp_loss(loss_acc, a.loss, B, lane == 0);  // MT == 32: the per-sample threads are warp 0
 }
 
 // zero loss / grads / the live rows of the per-unique-id gradient buffers
-__global__ void __launch_bounds__(256) k_mma_prep(b200_deepfm_args_t a, int n_params) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (blockIdx.y == 0) {
-    if (tid == 0) *a.loss = 0.f;
-    for (long long i = tid; i < n_params; i += stride) a.grads[i] = 0.f;
-  }
-  for (int g = blockIdx.y; g < a.G; g += gridDim.y) {
-    const int u = a.n_unique[g];
-    float* gw = a.gsum_wide + (long long)g * a.B;
-    float4* gd = reinterpret_cast<float4*>(a.gsum_deep + (long long)g * a.B * D);
-    for (long long i = tid; i < u; i += stride) gw[i] = 0.f;
-    for (long long i = tid; i < 2LL * u; i += stride) gd[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-}
+__global__ void __launch_bounds__(256) k_mma_prep(b200_deepfm_args_t a, int n_params) { zero_step_outputs(a, n_params); }
 
 static_assert(MT == 32, "the per-sample phase and the loss reduction assume one warp of samples");
 
@@ -432,25 +351,20 @@ extern "C" {
 int64_t b200_deepfm_mma_launch_count(void) { return g_launches_mma; }
 
 int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
-  if (!a || a->G < 1 || a->B < 1 || tile_of(a->G).kp / 8 > 4 * MAX_NT_W) return -1;
-  if (!a->inv || !a->bet_wide || !a->bet_deep || !a->dense || !a->params || !a->labels || !a->grads || !a->gsum_wide ||
-      !a->gsum_deep || !a->loss || !a->n_unique || a->rows)
-    return -1;
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  if (check_common(a, true)) return -1;
+  if (tile_of(a->G).kp / 8 > 4 * MAX_NT_W) return fail(-1, "too many id groups for the mma tower (max 46)");
+  if (a->rows) return fail(-1, "the mma tower reads pulled rows only");
   const size_t smem = mma_smem_bytes(a->G);
-  static bool attr_done[64] = {false};
-  static int per_sm[64] = {0};
-  if (smem > 100 * 1024) return -1;
-  if (dev < 64 && !attr_done[dev]) {
-    cudaFuncSetAttribute(k_tower_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+  if (smem > 100 * 1024) return fail(-1, "the mma tower's tile does not fit in shared memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  int n_sm;
+  const int dev = current_device(&n_sm);
+  max_dynamic_smem_once<k_tower_mma<true>>(dev, 100 * 1024);
+  static int per_sm[64] = {0};  // resident CTAs per SM, once per device
+  if (dev < 64 && per_sm[dev] == 0) {
     int nb = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tower_mma<true>, THREADS, smem);
-    if (e != cudaSuccess || nb < 1) nb = 1;
-    per_sm[dev] = nb;
-    attr_done[dev] = true;
+    per_sm[dev] = e != cudaSuccess || nb < 1 ? 1 : nb;
   }
   const Layout l = layout(a->G);
   k_mma_prep<<<dim3(8, a->G), 256, 0, st>>>(*a, l.total);
@@ -459,7 +373,7 @@ int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
   const unsigned grid = (unsigned)(nchunk < cap ? nchunk : cap);
   k_tower_mma<true><<<grid, THREADS, smem, st>>>(*a);
   g_launches_mma += 2;
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+  return launch_status();
 }
 
 }  // extern "C"

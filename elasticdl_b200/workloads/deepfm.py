@@ -215,6 +215,11 @@ class HostFeeder:
         return loss
 
 
+def _tower_error(lib):
+    """Why the last failed tower call failed (b200_deepfm_last_error)."""
+    return lib.b200_deepfm_last_error().decode("utf-8", "replace")
+
+
 def resolve_row_source(row_source, tower, n_shards, exchange, paired):
     """DeepFMPSEngine's row_source: "table" (the tower reads the table records) needs the tile tower and every
     record on this GPU in its own slab -- one shard, the direct exchange, unpaired tables."""
@@ -498,7 +503,7 @@ class DeepFMPSEngine:
                 check(lib.b200ps_pull_dense(h, arr, n, g._stream()))
                 rc = lib.b200_deepfm_tile_prologue(_ct.byref(a), g._stream())
                 if rc:
-                    raise RuntimeError("b200_deepfm_tile_prologue failed (%d)" % rc)
+                    raise RuntimeError("b200_deepfm_tile_prologue failed (%d): %s" % (rc, _tower_error(lib)))
                 ev_prep = torch.cuda.Event()
                 ev_prep.record(self.aux)  # the tower waits for this, not for push_begin behind it
                 g.push_begin(self.lr, self.zero_versions)
@@ -528,7 +533,7 @@ class DeepFMPSEngine:
             main.wait_event(ev_prep)
             rc = lib.b200_deepfm_tile_main(_ct.byref(a), st)
             if rc:
-                raise RuntimeError("b200_deepfm_tile_main failed (%d)" % rc)
+                raise RuntimeError("b200_deepfm_tile_main failed (%d): %s" % (rc, _tower_error(lib)))
             loss = self.loss_buf
             dense_segs = self.push_dense_segs
         elif self.tower_kind in ("tile", "fused", "mma"):
@@ -540,7 +545,7 @@ class DeepFMPSEngine:
             fn = {"mma": lib.b200_deepfm_fwd_bwd_mma, "tile": lib.b200_deepfm_fwd_bwd_tile}.get(self.tower_kind, lib.b200_deepfm_fwd_bwd)
             rc = fn(_ct.byref(a), st)
             if rc:
-                raise RuntimeError("b200_deepfm_fwd_bwd failed (%d)" % rc)
+                raise RuntimeError("b200_deepfm_fwd_bwd failed (%d): %s" % (rc, _tower_error(lib)))
             done(e_t)
             loss = self.loss_buf
             dense_segs = self.push_dense_segs
@@ -587,7 +592,7 @@ class DeepFMPSEngine:
         rc = self.group.lib.b200_deepfm_publish_loss(self.loss_buf.data_ptr(), self.loss_ring.data_ptr(), self.LOSS_RING,
                                                      self.loss_cursor.data_ptr(), st)
         if rc:
-            raise RuntimeError("b200_deepfm_publish_loss failed (%d)" % rc)
+            raise RuntimeError("b200_deepfm_publish_loss failed (%d): %s" % (rc, _tower_error(self.group.lib)))
 
     def loss_host(self, step_index):
         """Loss of step `step_index` (0-based count of steps run by this engine) from the host ring; valid once
@@ -785,7 +790,7 @@ class DeepFMPSEngine:
             a.dense = dense.data_ptr()
             fwd = lib.b200_deepfm_forward_tile if self.tower_kind == "tile" else lib.b200_deepfm_forward
             if fwd(_ct.byref(a), st):
-                raise RuntimeError("b200_deepfm_forward failed")
+                raise RuntimeError("b200_deepfm_forward failed: %s" % _tower_error(lib))
         finally:
             self.__dict__.update(saved)
         return self.logits_buf

@@ -88,7 +88,9 @@ int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int
 int b200_deepfm_tile_prologue(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_tile_main(const b200_deepfm_args_t* args, void* stream);
 int64_t b200_deepfm_tile_launch_count(void);
-const char* b200_deepfm_tile_last_error(void);
+/* Why the last call of any tower entry point (publish_loss included) that returned -1 (refused) or -2 (launch
+ * error) failed; on the calling thread. */
+const char* b200_deepfm_last_error(void);
 /* forward only (logits), for evaluation. */
 int b200_deepfm_forward(const b200_deepfm_args_t* args, void* stream);
 /* kernels launched by the two calls above so far */

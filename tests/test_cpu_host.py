@@ -33,6 +33,14 @@ def test_abi_v2_exports_every_declared_symbol():
     assert declared <= exported
 
 
+def test_build_digest_covers_every_header():
+    """The library is rebuilt when a source in its digest changes: every csrc/*.cuh must be listed in HEADERS."""
+    from elasticdl_b200 import build
+
+    cuh = {f for f in os.listdir(build.CSRC) if f.endswith(".cuh")}
+    assert cuh and cuh <= set(build.HEADERS), cuh - set(build.HEADERS)
+
+
 def test_optimizer_grammar_errors_without_a_device():
     from elasticdl_b200 import _lib
 

@@ -216,7 +216,7 @@ def run_and_check(tower, G, B, pattern="zipf", regime="base", seed=0, calls=2):
 @pytest.mark.parametrize("tower", ["tile", "fused", "mma"])
 def test_tower_shapes(tower, G, B):
     if tower == "tile" and G > 38:
-        pytest.skip("the tile tower holds at most 38 id groups (see test_group_limits)")
+        pytest.skip("the tile tower holds at most 38 id groups (see test_group_limits_and_their_messages)")
     run_and_check(tower, G, _batch(B), seed=G)
 
 
@@ -251,25 +251,26 @@ def test_forward_only(tower, G, B):
     run_and_check(tower, G, _batch(B), seed=31)
 
 
-def test_group_limits():
-    """G = 39 on the tile tower and G = 47 on the fused / mma towers are refused (-1) without a launch."""
+def test_group_limits_and_their_messages():
+    """G = 39 on the tile tower and G = 47 on the fused / mma towers are refused (-1) without a launch, and
+    b200_deepfm_last_error names the limit of the tower that refused."""
     from elasticdl_b200 import _lib
 
     L = _lib.lib()
-    for tower, G, count in (("tile", 39, L.b200_deepfm_tile_launch_count),
-                            ("split", 39, L.b200_deepfm_tile_launch_count),
-                            ("forward_tile", 39, L.b200_deepfm_tile_launch_count),
-                            ("fused", 47, L.b200_deepfm_launch_count),
-                            ("forward", 47, L.b200_deepfm_launch_count),
-                            ("mma", 47, L.b200_deepfm_mma_launch_count)):
+    for tower, G, count, limit in (("tile", 39, L.b200_deepfm_tile_launch_count, b"38"),
+                                   ("split", 39, L.b200_deepfm_tile_launch_count, b"38"),
+                                   ("forward_tile", 39, L.b200_deepfm_tile_launch_count, b"38"),
+                                   ("fused", 47, L.b200_deepfm_launch_count, b"46"),
+                                   ("forward", 47, L.b200_deepfm_launch_count, b"46"),
+                                   ("mma", 47, L.b200_deepfm_mma_launch_count, b"46")):
         buf = Buffers(G, 64)
         buf.load(make_inputs(G, 64, seed=G)[0])
         before = count()
         assert _call(tower, buf.args(not tower.startswith("forward"))) == -1, tower
+        assert limit in L.b200_deepfm_last_error(), (tower, L.b200_deepfm_last_error())
         assert count() == before, tower
         torch.cuda.synchronize()
         assert torch.isnan(buf.logits).all() and torch.isnan(buf.grads).all(), tower
-    assert b"38" in L.b200_deepfm_tile_last_error()
 
 
 @pytest.mark.parametrize("B", SHAPES_B + ["262144"])

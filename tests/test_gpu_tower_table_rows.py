@@ -137,10 +137,12 @@ def test_row_source_refused_where_it_does_not_apply():
     rows = _rows_struct(group, G, uniq)
     buf = Buffers(G, B)
     buf.load(inputs)
-    for tower in ("forward_tile", "fused", "mma"):
+    L = _lib.lib()
+    for tower, name in (("forward_tile", b"forward-only tile tower"), ("fused", b"fused tower"), ("mma", b"mma tower")):
         a = buf.args(not tower.startswith("forward"))
         a.rows = ctypes.pointer(rows)
         assert _call(tower, a) == -1, tower
+        assert name + b" reads pulled rows only" in L.b200_deepfm_last_error(), (tower, L.b200_deepfm_last_error())
     torch.cuda.synchronize()
     assert torch.isnan(buf.logits).all()
     group.close()
