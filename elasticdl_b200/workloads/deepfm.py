@@ -104,24 +104,39 @@ def packed_nbytes(G, B, widths=None):
 
 def packed_views(buf, G, B, widths=None):
     """(ids, dense fp32 [B, 13], labels fp32 [B]) views of a packed uint8 buffer; ids is an int32 [G, B] view
-    when every width is 4, else the uint8 id region itself (the dedup kernel reads it with the widths)."""
+    when every width is 4 and the segments need no padding (B % 4 == 0), else the uint8 id region itself (the
+    dedup kernel reads it with the widths)."""
     widths = widths or [4] * G
     a = _ids_layout(B, widths)[1]
     b = a + 4 * B * N_DENSE
-    ids = buf[:a].view(torch.int32).view(G, B) if all(w == 4 for w in widths) else buf[:a]
+    ids = buf[:a].view(torch.int32).view(G, B) if all(w == 4 for w in widths) and B % 4 == 0 else buf[:a]
     return ids, buf[a:b].view(torch.float32).view(B, N_DENSE), buf[b:b + 4 * B].view(torch.float32)
 
 
 _NP_UINT = {1: torch.uint8, 2: torch.int16, 4: torch.int32}
 
 
+def check_id_widths(ids, widths):
+    """Raise ValueError unless every id of group g (ids [G, B]) fits widths[g] bytes: 0 <= id < min(256**w, 2**31)
+    (4-byte ids are read back as int32 on the int32 transport).  Narrowing is a plain cast, so an id outside that
+    range would wrap around onto another, valid row; the dedup kernel can only range-check what it reads."""
+    lo, hi = (t.tolist() for t in torch.aminmax(ids, dim=1))
+    for g, (w, a, b) in enumerate(zip(widths, lo, hi)):
+        lim = min(256 ** w, 2 ** 31)
+        if a < 0 or b >= lim:
+            raise ValueError("id group %d: id %d does not fit its %d-byte ids (0 <= id < %d)"
+                             % (g, a if a < 0 else b, w, lim))
+
+
 def pack_batch(ids, dense, labels, pin=False, widths=None):
     """Pack (ids int64/int32 [G, B], dense [B, 13], labels [B]) into one uint8 buffer on the same device
     (pin=True: pinned host memory).  ids are narrowed to `widths` bytes per group (default int32: every
     dac_ctr table has fewer than 2^31 rows); the device widens them again inside the dedup kernel
-    (b200ps_unique_bounded_i32 / b200ps_unique_packed), so the PS sees the same int64 ids."""
+    (b200ps_unique_bounded_i32 / b200ps_unique_packed), so the PS sees the same int64 ids.  An id that does
+    not fit its group's width raises ValueError (check_id_widths)."""
     G, B = ids.shape
     widths = widths or [4] * G
+    check_id_widths(ids, widths)
     layout, a = _ids_layout(B, widths)
     buf = torch.zeros(packed_nbytes(G, B, widths), dtype=torch.uint8, device="cpu" if pin else ids.device)
     if pin:
@@ -677,13 +692,17 @@ class DeepFMPSEngine:
         return self.graphs_ahead
 
     def _fill(self, dst, batch):
-        """dst: static packed buffer; batch: (packed,) or (ids, dense, labels) -- device or pinned host."""
+        """dst: static packed buffer; batch: (packed,) or (ids, dense, labels) -- device or pinned host.  Separate
+        ids are range-checked against the widths first (check_id_widths); a packed buffer is already narrowed."""
         if len(batch) == 1:
             dst.copy_(batch[0], non_blocking=True)
-        elif all(w == 4 for w in self.widths):
-            for d, src in zip(packed_views(dst, self.G, self.B), batch):
+            return
+        check_id_widths(batch[0], self.widths)
+        views = packed_views(dst, self.G, self.B, self.widths)
+        if views[0].dtype == torch.int32:  # an unpadded int32 [G, B] id region: copy into the views
+            for d, src in zip(views, batch):
                 d.copy_(src, non_blocking=True)
-        else:  # separate tensors into a narrow layout: pack on the device (compatibility path)
+        else:  # separate tensors into a narrow or padded layout: pack on the device (compatibility path)
             ids, dense, labels = batch
             dst.copy_(pack_batch(ids.to(self.device), dense.to(self.device), labels.to(self.device), widths=self.widths),
                       non_blocking=True)

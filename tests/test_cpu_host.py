@@ -137,6 +137,62 @@ def test_deepfm_workload_shapes_cpu():
     assert torch.allclose(tw(dense, wide, deep), want, atol=1e-5)
 
 
+def test_pack_batch_refuses_ids_that_do_not_fit_their_width():
+    """pack_batch narrows ids with a plain cast, so an id that is negative or too wide for its group would wrap onto
+    another, valid row (300 -> 44 in a 1-byte group, -1 -> 65535 in a 2-byte one, 2^32 + 5 -> 5).  Such an id is
+    refused with ValueError naming the group and the value: narrow widths and the int32 default, int64 and int32
+    ids, at every position of the batch."""
+    from elasticdl_b200.workloads.deepfm import id_widths, pack_batch
+
+    rows, B = [200, 5000, 1000000], 33
+    narrow = id_widths(rows)
+    assert narrow == [1, 2, 4]
+    dense, labels = torch.randn(B, 13), torch.rand(B)
+    cases = [(narrow, 0, 300), (narrow, 0, 256), (narrow, 0, -1), (narrow, 1, 70000), (narrow, 1, 65536),
+             (narrow, 1, -1), (narrow, 2, 2 ** 32 + 5), (narrow, 2, 2 ** 31), (narrow, 2, -1),
+             (None, 0, 2 ** 31), (None, 1, -1), (None, 2, 2 ** 32 + 5)]
+    for widths, g, bad in cases:
+        for pos in (0, B // 2, B - 1):
+            ids = torch.zeros(3, B, dtype=torch.int64)
+            ids[g, pos] = bad
+            with pytest.raises(ValueError, match="id group %d: id %d " % (g, bad)):
+                pack_batch(ids, dense, labels, widths=widths)
+            if -2 ** 31 <= bad < 2 ** 31:
+                with pytest.raises(ValueError, match="id group %d: id %d " % (g, bad)):
+                    pack_batch(ids.to(torch.int32), dense, labels, widths=widths)
+
+
+def test_pack_batch_round_trips_ids_at_every_width_boundary():
+    """id_widths picks 1 / 2 / 4 bytes at <= 256 / <= 65536 / larger rows, and every id that fits its width --
+    both sides of each byte and of the int16 / int32 sign bits -- reads back unsigned from the packed buffer as it
+    went in (segments padded to 16 bytes), for int64 and int32 ids; dense and labels follow the ids."""
+    from elasticdl_b200.workloads.deepfm import N_DENSE, id_widths, pack_batch, packed_views
+
+    assert id_widths([1, 2, 255, 256, 257, 65535, 65536, 65537, 2 ** 31]) == [1, 1, 1, 1, 2, 2, 2, 4, 4]
+    edges = {1: [0, 1, 127, 128, 254, 255], 2: [0, 255, 256, 32767, 32768, 65534, 65535],
+             4: [0, 65535, 65536, 2 ** 31 - 2, 2 ** 31 - 1]}
+    # B = 9: every segment padded to 16 bytes, the int32 layout too (its ids come back as the uint8 region);
+    # B = 8: no padding, the int32 layout is an int32 [G, B] view
+    for widths, B in (([1, 2, 4, 2, 1], 9), ([4, 4, 4], 9), ([4, 4, 4], 8), ([1, 2, 4], 8)):
+        ids = torch.zeros(len(widths), B, dtype=torch.int64)
+        for g, w in enumerate(widths):
+            ids[g, :len(edges[w])] = torch.tensor(edges[w])
+        dense, labels = torch.randn(B, N_DENSE), torch.rand(B)
+        for dtype in (torch.int64, torch.int32):
+            buf = pack_batch(ids.to(dtype), dense, labels, widths=widths)
+            region, d, lab = packed_views(buf, len(widths), B, widths)
+            assert torch.equal(d, dense) and torch.equal(lab, labels)
+            if all(w == 4 for w in widths) and B % 4 == 0:
+                assert region.dtype == torch.int32 and torch.equal(region.to(torch.int64), ids)
+                continue
+            raw, off = region.numpy(), 0
+            for g, w in enumerate(widths):
+                got = raw[off:off + B * w].view({1: np.uint8, 2: np.uint16, 4: np.uint32}[w]).astype(np.int64)
+                assert np.array_equal(got, ids[g].numpy()), (widths, B, g, got)
+                off += (B * w + 15) // 16 * 16
+            assert off == raw.size
+
+
 _GLOO_WORKER = r"""
 import os, sys
 sys.path.insert(0, sys.argv[1])

@@ -299,78 +299,6 @@ def _ps_reference(group, eng, ids, dense, labels):
     return inputs, T.tower_reference(*inputs)
 
 
-@pytest.mark.parametrize("path", ["step", "lookahead_graphs"])
-def test_deepfm_engine_benchmark_shape_matches_float64(path):
-    """The benchmark's configuration -- B = 32768, the 38 dac_ctr groups at full size, tile tower -- one step
-    through step() (the branched prologue / main path) or through the captured lookahead graphs bench.py
-    times: loss, per-unique-id gradient sums and parameter gradients within the float64 reference's bound,
-    and the PS state after the push == the oracle's Adam applied to what the engine pushed, bit for bit.
-    The batch is a Zipf synthetic_batch conditioned as in test_gpu_tower_reference.py (dense rows of samples
-    with a pre-activation within 1e-4 * M of a ReLU kink are redrawn)."""
-    from elasticdl_b200.ps import PSGroup
-    from elasticdl_b200.workloads.deepfm import GROUP_ROWS, DeepFMPSEngine, HostFeeder, synthetic_batch
-    from oracle import tower_oracle as T
-
-    B, G, D = 32768, len(GROUP_ROWS), 8
-    dev = torch.device("cuda", 0)
-    group = PSGroup(1, *ADAM, device=0)
-    eng = DeepFMPSEngine(group, B)
-    assert eng.tower_kind == "tile"
-    ids, dense, labels = synthetic_batch(B, 9, dev, "zipf")
-    gen = torch.Generator(device=dev).manual_seed(9)
-    for _ in range(40):
-        inputs, ref = _ps_reference(group, eng, ids, dense, labels)
-        near = T.near_relu_kink(ref)
-        if not bool(near.any()):
-            break
-        dense[near] = torch.randn((int(near.sum()), T.ND), generator=gen, device=dev)
-    else:
-        raise AssertionError("conditioning did not converge")
-    inv, n_unique_ref, bet_w0, bet_d0, _, _, params0 = inputs
-    p = eng.cur
-    if path == "step":
-        eng.step(ids, dense, labels)
-    else:
-        feeder = HostFeeder(eng, 3, lookahead=True)
-        nxt = synthetic_batch(B, 10, dev, "zipf")
-        feeder.submit(*(t.cpu().pin_memory() for t in (ids, dense, labels)))
-        feeder.submit(*(t.cpu().pin_memory() for t in nxt))
-        feeder.run_next()
-        assert eng.cur != p  # the current plan already holds the next batch's dedup
-    torch.cuda.synchronize()
-    group.check()
-    plan = eng.plans[p]  # the dedup of the batch that trained
-    n_unique = plan["n_unique"]
-    assert torch.equal(n_unique, n_unique_ref)
-    assert torch.equal(plan["inv"].view(G, B), inv)
-    got = {"loss": eng.loss_buf, "grads": eng.flat_grads, "gsum_wide": eng.gsum_w.view(G, B),
-           "gsum_deep": eng.gsum_d.view(G, B, D)}
-    T.check(got, ref, families=("loss", "grads", "gsum_wide", "gsum_deep"), label=path,
-            n_sm=torch.cuda.get_device_properties(0).multi_processor_count)
-    # PS state == oracle Adam (step 1) on the gradients the engine pushed
-    uniq = plan["uniq"].view(G, B).cpu().numpy()
-    n_u = n_unique.cpu().numpy()
-    gsum_w = eng.gsum_w.view(G, B).cpu().numpy()
-    gsum_d = eng.gsum_d.view(G, B, D).cpu().numpy()
-    for names, t0, gsum, dim in ((eng.wide_names, bet_w0, gsum_w[..., None], 1), (eng.deep_names, bet_d0, gsum_d, D)):
-        for g in range(G):
-            u = int(n_u[g])
-            touched = uniq[g, :u]
-            prow = t0[g, :u].reshape(u, dim).cpu().numpy().copy()
-            m, v = np.zeros_like(prow), np.zeros_like(prow)
-            O.np_adam(gsum[g, :u].reshape(u, dim).copy(), prow, m, v, 0.001, 1, 0.9, 0.999, 1e-7)
-            assert np.array_equal(group.pull_rows([(names[g], torch.from_numpy(touched))])[0].cpu().numpy().reshape(u, dim), prow)
-            assert np.array_equal(group.slot_rows(names[g], touched, 1).cpu().numpy().reshape(u, dim), m)
-            assert np.array_equal(group.slot_rows(names[g], touched, 2).cpu().numpy().reshape(u, dim), v)
-    flat_g = eng.flat_grads.cpu().numpy()
-    for (name, _), (off, n) in zip(eng.params, eng.flat_views):
-        want = params0[off:off + n].cpu().numpy().copy()
-        m, v = np.zeros_like(want), np.zeros_like(want)
-        O.np_adam(flat_g[off:off + n].copy(), want, m, v, 0.001, 1, 0.9, 0.999, 1e-7)
-        assert np.array_equal(group.pull_dense([name])[name].cpu().numpy().reshape(-1), want), name
-    group.close()
-
-
 def _engine_state(group, eng, rows):
     t = [group.pull_rows([(n, torch.arange(r))])[0].cpu().numpy() for n, r in zip(eng.wide_names + eng.deep_names, rows + rows)]
     d = group.pull_dense([n for n, _ in eng.params])
