@@ -36,13 +36,13 @@ def _n_sm():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _condition(group, eng, ids, dense, labels, seed):
+def _condition(group, eng, ids, dense, labels, seed, dense_params=None):
     """Redraw, in place, the dense rows of the samples whose float64 pre-activation lies near a ReLU kink under the
-    state the PS holds now: their fp32 mask may flip, which no rounding bound covers.  Returns the float64
-    reference of the conditioned batch (_ps_reference)."""
+    state the PS holds now (dense parameters: `dense_params` where given): their fp32 mask may flip, which no
+    rounding bound covers.  Returns the float64 reference of the conditioned batch (_ps_reference)."""
     gen = torch.Generator(device=DEV).manual_seed(seed)
     for _ in range(40):
-        _, ref = _ps_reference(group, eng, ids, dense, labels)
+        _, ref = _ps_reference(group, eng, ids, dense, labels, dense_params)
         near = T.near_relu_kink(ref)
         if not bool(near.any()):
             return ref

@@ -276,9 +276,10 @@ def test_deepfm_engine_step_matches_oracle_adam(n_shards, B, rows, tower_kind, p
     group.close()
 
 
-def _ps_reference(group, eng, ids, dense, labels):
+def _ps_reference(group, eng, ids, dense, labels, dense_params=None):
     """The float64 tower reference (oracle/tower_oracle.py) of one batch from what the PS holds now: the
-    rows of the batch's ids only (first-occurrence order, like the engine's dedup) and the dense parameters.
+    rows of the batch's ids only (first-occurrence order, like the engine's dedup) and the dense parameters
+    (or `dense_params`, {name: values}, where the PS holds none yet).
     Returns ((inv, n_unique, bet_wide, bet_deep, dense, labels, params), reference)."""
     from oracle import tower_oracle as T
 
@@ -291,10 +292,10 @@ def _ps_reference(group, eng, ids, dense, labels):
         touched = uniq[g, :u].cpu()
         bet_w[g, :u] = group.pull_rows([(eng.wide_names[g], touched)])[0].reshape(u).to(dev)
         bet_d[g, :u] = group.pull_rows([(eng.deep_names[g], touched)])[0].reshape(u, T.D).to(dev)
-    d = group.pull_dense([n for n, _ in eng.params])
+    d = group.pull_dense([n for n, _ in eng.params]) if dense_params is None else dense_params
     params = torch.zeros(T.layout(G)["total"], dtype=torch.float32, device=dev)
     for (name, _), (off, n) in zip(eng.params, eng.flat_views):
-        params[off:off + n] = d[name].reshape(-1).to(dev)
+        params[off:off + n] = torch.as_tensor(d[name]).reshape(-1).to(dev)
     inputs = (inv, n_unique, bet_w, bet_d, dense, labels, params)
     return inputs, T.tower_reference(*inputs)
 
