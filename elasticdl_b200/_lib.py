@@ -147,6 +147,12 @@ SYMBOLS = {
     "b200_deepfm_tile_main": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
     "b200_deepfm_tile_launch_count": (_i64, []),
     "b200_deepfm_last_error": (ctypes.c_char_p, []),
+    "b200_deepfm_dcn_param_count": (_sz, [_i]),
+    "b200_deepfm_dcn_fwd_bwd_tile": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_dcn_tile_prologue": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_dcn_tile_main": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_dcn_forward_tile": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_dcn_launch_count": (_i64, []),
     # include/b200_features.h
     "b200feat_last_error": (ctypes.c_char_p, []),
     "b200feat_transform": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i64, _vp, _i, _vp, _vp]),

@@ -57,6 +57,48 @@ class DeepFMTower(torch.nn.Module):
         return linear_logit + dnn_logit + fm
 
 
+class DCNTower(torch.nn.Module):
+    """dcn_model.py:53-95 without the embedding lookups: the same DNN[16, 4] and linear part as DeepFMTower, FM
+    replaced by a CrossNet over x0 = [dense | deep] (deepctr's CrossNet, "vector" parameterization, DCN paper eq. 3:
+    x_{l+1} = x0 * (x_l . w_l) + b_l + x_l; kernels glorot-normal, biases zero) and one bias-free output unit over
+    [dnn_out | x_L].  regularization() is the l2 term the model adds to its loss (model.losses)."""
+
+    def __init__(self, n_groups=N_GROUPS, deep_dim=DEEP_DIM, n_dense=N_DENSE, hidden=(16, 4), cross_layers=2,
+                 l2_reg=1e-5):
+        super().__init__()
+        self.n_groups, self.deep_dim, self.l2_reg = n_groups, deep_dim, l2_reg
+        n_in = n_dense + n_groups * deep_dim
+        self.dense_linear = torch.nn.Linear(n_dense, 1, bias=False)
+        dims = [n_in] + list(hidden)
+        self.dnn = torch.nn.ModuleList([torch.nn.Linear(a, b) for a, b in zip(dims[:-1], dims[1:])])
+        self.out = torch.nn.Linear(dims[-1] + n_in, 1, bias=False)
+        # keras glorot_normal of a [n_in, 1] kernel: truncated normal, std sqrt(2 / (n_in + 1)) / 0.8796
+        std = math.sqrt(2.0 / (n_in + 1)) / 0.87962566103423978
+        self.cross_w = torch.nn.Parameter(torch.nn.init.trunc_normal_(torch.empty(cross_layers, n_in), 0.0, std,
+                                                                      -2 * std, 2 * std))
+        self.cross_b = torch.nn.Parameter(torch.zeros(cross_layers, n_in))
+
+    def forward(self, dense, wide, deep):
+        """dense [B,13], wide [B,G], deep [B,G,D] -> logits [B]."""
+        B = dense.shape[0]
+        x0 = torch.cat([dense, deep.reshape(B, -1)], 1)
+        h = x0
+        for layer in self.dnn:
+            h = torch.relu(layer(h))
+        x = x0
+        for w, b in zip(self.cross_w, self.cross_b):
+            x = x0 * (x @ w).unsqueeze(1) + b + x
+        deep_cross_logit = self.out(torch.cat([h, x], 1)).squeeze(1)
+        linear_logit = wide.sum(1) + self.dense_linear(dense).squeeze(1)
+        return linear_logit + deep_cross_logit
+
+    def regularization(self):
+        return self.l2_reg * (self.cross_w * self.cross_w).sum()
+
+
+TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower}
+
+
 def synthetic_batch(batch, seed, device, dist="zipf", zipf_s=1.05, group_rows=GROUP_ROWS):
     """SURVEY.md section 8d config 2: bucket ids uniform, categorical ids Zipf(s) over the
     table's rows (or uniform), dense features N(0,1), labels Bernoulli(0.25).
@@ -154,11 +196,20 @@ def pack_batch(ids, dense, labels, pin=False, widths=None):
     return buf
 
 
+def flat_order(tower):
+    """[(parameter, padded size or None)] of the tower in its flat layout (include/b200_deepfm.h)."""
+    order = [(tower.dense_linear.weight, 16), (tower.dnn[0].weight, None), (tower.dnn[0].bias, None),
+             (tower.dnn[1].weight, None), (tower.dnn[1].bias, None)]
+    if isinstance(tower, DCNTower):
+        return order + [(tower.out.weight, None), (tower.cross_w, None), (tower.cross_b, None)]
+    return order + [(tower.dnn_logit.weight, None)]
+
+
 def flatten_tower(tower, flat):
     """Re-point the tower's parameters at views of one flat buffer laid out as
-    include/b200_deepfm.h documents: [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w3]."""
-    order = [(tower.dense_linear.weight, 16), (tower.dnn[0].weight, None), (tower.dnn[0].bias, None),
-             (tower.dnn[1].weight, None), (tower.dnn[1].bias, None), (tower.dnn_logit.weight, None)]
+    include/b200_deepfm.h documents: DeepFM [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w3], DCN
+    [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w_out | w_0 w_1 | b_0 b_1]."""
+    order = flat_order(tower)
     off, views = 0, []
     with torch.no_grad():
         for p, padded in order:
@@ -249,7 +300,8 @@ def resolve_row_source(row_source, tower, n_shards, exchange, paired):
 
 class DeepFMPSEngine:
     def __init__(self, group, batch, lr=1e-3, init_std=0.01, seed=7, group_rows=GROUP_ROWS, deep_dim=DEEP_DIM,
-                 init_rows=True, tower="tile", paired=None, exchange=None, id_transport="int32", row_source="auto"):
+                 init_rows=True, tower="tile", paired=None, exchange=None, id_transport="int32", row_source="auto",
+                 model="deepfm"):
         """tower="tile": rows of 32 samples gathered once into shared memory, forward / backward / parameter
         gradients from the tile (csrc/deepfm_tower2.cu);
         tower="fused": round 1's hand-written CUDA tower (csrc/deepfm_tower.cu, three row gathers);
@@ -258,8 +310,18 @@ class DeepFMPSEngine:
         row_source="table": the tile tower reads each sample's rows straight from the table records
         (b200_deepfm_rows_t) and step() launches no row pull; "pull": the rows of the unique ids are first
         pulled into bet_w / bet_d.  "auto" takes "table" where it applies: tile tower, one shard, direct
-        exchange, tables not paired."""
+        exchange, tables not paired.
+        model="deepfm" (DeepFMTower) or "dcn" (DCNTower, the dac_ctr Deep & Cross Network: csrc/dcn_tower.cu);
+        the dedup, the rows, the push and the pipelines are the same for both.  "dcn" runs on tower="tile" or
+        "torch" and at most 38 id groups, and raises ValueError otherwise."""
         assert tower in ("tile", "fused", "mma", "torch")
+        if model not in TOWERS:
+            raise ValueError("model must be one of %s, not %r" % (sorted(TOWERS), model))
+        if model == "dcn" and tower not in ("tile", "torch"):
+            raise ValueError('model="dcn" runs on tower="tile" or "torch", not %r' % tower)
+        if model == "dcn" and len(group_rows) > 38:
+            raise ValueError('model="dcn" holds at most 38 id groups, not %d' % len(group_rows))
+        self.model = model
         if tower == "tile" and len(group_rows) > 38:
             tower = "fused"  # the tile tower holds at most 38 id groups in its shared-memory row
         self.tower_kind = tower
@@ -299,16 +361,14 @@ class DeepFMPSEngine:
             self.wide_ids = [group.register_table(n, 1, "zero", r) for n, r in zip(self.wide_names, group_rows)]
             self.deep_ids = [group.register_table(n, D, "zero", r) for n, r in zip(self.deep_names, group_rows)]
         torch.manual_seed(seed)
-        self.tower = DeepFMTower(G, D).to(dev)
-        n_flat = int(group.lib.b200_deepfm_param_count(G))
+        self.tower = TOWERS[model](G, D).to(dev)
+        n_flat = int((group.lib.b200_deepfm_dcn_param_count if model == "dcn" else group.lib.b200_deepfm_param_count)(G))
         self.flat_params = torch.zeros(n_flat, dtype=torch.float32, device=dev)
         self.flat_grads = torch.zeros(n_flat, dtype=torch.float32, device=dev)
         self.flat_views = flatten_tower(self.tower, self.flat_params)
         # named_parameters order != flat order: keep both
-        flat_order = [self.tower.dense_linear.weight, self.tower.dnn[0].weight, self.tower.dnn[0].bias,
-                      self.tower.dnn[1].weight, self.tower.dnn[1].bias, self.tower.dnn_logit.weight]
         names = {id(p): n for n, p in self.tower.named_parameters()}
-        self.params = [(names[id(p)], p) for p in flat_order]
+        self.params = [(names[id(p)], p) for p, _ in flat_order(self.tower)]
         from elasticdl_b200.common.hash_utils import string_to_id
 
         self.dense_ids = []
@@ -357,7 +417,10 @@ class DeepFMPSEngine:
         self.act_d = torch.empty((G * B, D), **f32)
         self.gsum_w = torch.zeros((G * B, 1), **f32)
         self.gsum_d = torch.zeros((G * B, D), **f32)
-        self.scratch = torch.empty(max(B * 44 + 16 * (N_DENSE + D * G), 320 * 16 + 16), **f32)  # b200_deepfm.h: backward state + W1^T | tile tower: W1 tile + counter
+        n_scratch = max(B * 44 + 16 * (N_DENSE + D * G), 320 * 16 + 16)  # b200_deepfm.h: backward state + W1^T | tile tower: W1 tile + counter
+        if model == "dcn":
+            n_scratch = max(n_scratch, 320 * 20 + 16)  # B200_DEEPFM_DCN_SCRATCH
+        self.scratch = torch.empty(n_scratch, **f32)
         self.loss_buf = torch.zeros(1, **f32)
         # the loss of every step also lands in a ring of pinned host memory, written by a 1-thread kernel at the end
         # of the step (b200_deepfm_publish_loss): loss_host(k) reads step k's value after a synchronize, no D2H copy
@@ -516,9 +579,10 @@ class DeepFMPSEngine:
             with torch.cuda.stream(self.aux):
                 arr, n = self.pull_dense_segs
                 check(lib.b200ps_pull_dense(h, arr, n, g._stream()))
-                rc = lib.b200_deepfm_tile_prologue(_ct.byref(a), g._stream())
+                prologue = lib.b200_deepfm_dcn_tile_prologue if self.model == "dcn" else lib.b200_deepfm_tile_prologue
+                rc = prologue(_ct.byref(a), g._stream())
                 if rc:
-                    raise RuntimeError("b200_deepfm_tile_prologue failed (%d): %s" % (rc, _tower_error(lib)))
+                    raise RuntimeError("%s failed (%d): %s" % (prologue.__name__, rc, _tower_error(lib)))
                 ev_prep = torch.cuda.Event()
                 ev_prep.record(self.aux)  # the tower waits for this, not for push_begin behind it
                 g.push_begin(self.lr, self.zero_versions)
@@ -546,9 +610,10 @@ class DeepFMPSEngine:
                     done(e)
         if branch:
             main.wait_event(ev_prep)
-            rc = lib.b200_deepfm_tile_main(_ct.byref(a), st)
+            tile_main = lib.b200_deepfm_dcn_tile_main if self.model == "dcn" else lib.b200_deepfm_tile_main
+            rc = tile_main(_ct.byref(a), st)
             if rc:
-                raise RuntimeError("b200_deepfm_tile_main failed (%d): %s" % (rc, _tower_error(lib)))
+                raise RuntimeError("%s failed (%d): %s" % (tile_main.__name__, rc, _tower_error(lib)))
             loss = self.loss_buf
             dense_segs = self.push_dense_segs
         elif self.tower_kind in ("tile", "fused", "mma"):
@@ -558,6 +623,8 @@ class DeepFMPSEngine:
             a.dense, a.labels = dense.data_ptr(), labels.data_ptr()
 
             fn = {"mma": lib.b200_deepfm_fwd_bwd_mma, "tile": lib.b200_deepfm_fwd_bwd_tile}.get(self.tower_kind, lib.b200_deepfm_fwd_bwd)
+            if self.model == "dcn":
+                fn = lib.b200_deepfm_dcn_fwd_bwd_tile
             rc = fn(_ct.byref(a), st)
             if rc:
                 raise RuntimeError("b200_deepfm_fwd_bwd failed (%d): %s" % (rc, _tower_error(lib)))
@@ -767,6 +834,8 @@ class DeepFMPSEngine:
         deep = act_d.view(G, B, D).permute(1, 0, 2)
         logits = self.tower(dense, wide, deep)
         loss = self.loss_fn(logits, labels)
+        if self.model == "dcn":
+            loss = loss + self.tower.regularization()
         plist = [p for _, p in self.params]
         grads = torch.autograd.grad(loss, plist + [act_w, act_d])
         gw, gd = grads[-2].contiguous(), grads[-1].contiguous()
@@ -808,6 +877,8 @@ class DeepFMPSEngine:
             a = self.tower_args
             a.dense = dense.data_ptr()
             fwd = lib.b200_deepfm_forward_tile if self.tower_kind == "tile" else lib.b200_deepfm_forward
+            if self.model == "dcn":
+                fwd = lib.b200_deepfm_dcn_forward_tile
             if fwd(_ct.byref(a), st):
                 raise RuntimeError("b200_deepfm_forward failed: %s" % _tower_error(lib))
         finally:
@@ -829,7 +900,8 @@ class DeepFMPSEngine:
                 "push": U * (8 + 4 * 1 + (1 + opt_slots) * 8 * 1) + U * (8 + 4 * D + (1 + opt_slots) * 8 * D),
                 # tower: per (sample, group) one rank read + one deep row + one wide value gathered, the
                 # embedding gradient scattered back (reduced per unique id), + the dense inputs / labels
-                # (row_source "table": + the low word of the row's id)
+                # (row_source "table": + the low word of the row's id); the same for DeepFM and DCN, whose cross
+                # network reads the tile's rows a second time from shared memory only
                 "tower_fwd_bwd": k * (4 + 4 * D + 4 + (4 if self.row_source == "table" else 0)) + U * (4 * D + 4)
                 + self.B * 4 * (N_DENSE + 1),
                 "pull_pair": U * (8 + 8 * D + 8 * 1), "pull_exchange": U * (8 + 8 * D + 8 * 1),

@@ -88,6 +88,23 @@ int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int
 int b200_deepfm_tile_prologue(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_tile_main(const b200_deepfm_args_t* args, void* stream);
 int64_t b200_deepfm_tile_launch_count(void);
+
+/* The dac_ctr Deep & Cross Network (model_zoo/dac_ctr/dcn_model.py:53-95) on the same tile design
+ * (csrc/dcn_tower.cu): the DNN 16 -> 4 over x0 = [dense 13 | deep 8G] as above, a two-layer CrossNet over x0
+ * ("vector" parameterization: x_{l+1} = x0 (x_l . w_l) + b_l + x_l), and
+ *   logit = sum(wide) + w_dense . dense + w_out . [dnn_out 4 | x_2],
+ *   loss  = mean BCE with logits + 1e-5 (|w_0|^2 + |w_1|^2)   (the gradients include 2e-5 w_l).
+ * Parameter / gradient layout (floats), in = 13 + 8G:
+ *   [ w_dense 13 (+3 pad) | w1 16 x in | b1 16 | w2 4 x 16 | b2 4 | w_out 4 + in | w_0 in | w_1 in | b_0 in | b_1 in ]
+ * Same arguments and outputs as the DeepFM tile entry points (`loss` includes the L2 term); `scratch` needs
+ * B200_DEEPFM_DCN_SCRATCH floats; at most 38 id groups, a larger G is refused (-1, b200_deepfm_last_error). */
+#define B200_DEEPFM_DCN_SCRATCH (320 * 20 + 16) /* W1 and the cross weights in tile column order, counters */
+size_t b200_deepfm_dcn_param_count(int G);
+int b200_deepfm_dcn_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_dcn_tile_prologue(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_dcn_tile_main(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_dcn_forward_tile(const b200_deepfm_args_t* args, void* stream);
+int64_t b200_deepfm_dcn_launch_count(void);
 /* Why the last call of any tower entry point (publish_loss included) that returned -1 (refused) or -2 (launch
  * error) failed; on the calling thread. */
 const char* b200_deepfm_last_error(void);
