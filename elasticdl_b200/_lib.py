@@ -26,7 +26,11 @@ class Seg(ctypes.Structure):
     ]
 
 
-DEEPFM_TILE_MAXG = 38
+DEEPFM_TILE_MAXG = 38  # B200_DEEPFM_TILE_MAXG: id groups the tile towers hold
+# floats of `scratch` the tile towers need: W1 in tile column order and the tile counter (DeepFM), W1 and the cross
+# weights and the counters (B200_DEEPFM_DCN_SCRATCH)
+DEEPFM_TILE_SCRATCH = 320 * 16 + 16
+DEEPFM_DCN_SCRATCH = 320 * 20 + 16
 
 
 class DeepFMRows(ctypes.Structure):  # b200_deepfm_rows_t (include/b200_deepfm.h)

@@ -7,7 +7,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(CSRC, "libb200ps.so")
 SOURCES = ["b200ps.cu", "deepfm_tower.cu", "deepfm_tower_mma.cu", "deepfm_tower2.cu", "dcn_tower.cu", "feature_ids.cu"]
 HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "ps_unique.cuh", "deepfm_common.cuh",
-           os.path.join("..", "..", "include", "b200ps.h"),
+           "tile_tower.cuh", os.path.join("..", "..", "include", "b200ps.h"),
            os.path.join("..", "..", "include", "b200_deepfm.h"),
            os.path.join("..", "..", "include", "b200_features.h")]
 NVCC_FLAGS = [

@@ -15,25 +15,18 @@
 // The dZ^T X contraction gives the sums over x0; the two batch sums sum g e and sum g ride along with the small
 // gradients, and each CTA folds its own share of the rank-1 terms into the atomics it makes anyway.
 //
-// The tile machinery is deepfm_tower2.cu's: 32-sample tiles gathered once into shared memory with cp.async
-// (pulled bet_* rows, or TABLE: straight from the record slabs with the next tile's ids prefetched), tiles handed
-// out dynamically, phases G / F / M / B1 / B2 with the same warp roles, 2 CTAs per SM.  The units of W1x are
+// The tile machinery is tile_tower.cuh's, shared with the DeepFM tile tower (deepfm_tower2.cu): 32-sample tiles
+// gathered once into shared memory with cp.async (pulled bet_* rows, or TABLE: straight from the record slabs with
+// the next tile's ids prefetched), tiles handed out dynamically, phases G and M, the argument checks and the
+// launches; this file adds phases F / B1 / B2 with the same warp roles, 2 CTAs per SM.  The units of W1x are
 //     [ a c e 0 | h1 0 .. 15 ]   (row stride 20 floats = 5 x 16 B; unit 3 has weight 0)
 // and the FM sums of DeepFM are gone: their shared-memory and register room holds the three cross units.
-#include "deepfm_common.cuh"
+#include "tile_tower.cuh"
 
 namespace {
 
 using namespace deepfm;
 
-constexpr int TS = 32;        // samples per tile
-constexpr int THREADS = 256;  // 8 warps
-constexpr int NKP = 8;        // column parts (warps) of phases F / B1
-constexpr int KPC = 40;       // tile columns per part = 5 id groups
-constexpr int NCOL = 320;     // deep 304 | dense 13 | 1 | 0 0   (G <= 38)
-constexpr int XS = 324;       // row stride (odd number of 16 B quads: conflict-free 128-bit row reads)
-constexpr int RS = 39;        // rank row stride (odd): Rt[s][g]
-constexpr int MAXG = 38;
 constexpr int NX = 4;             // cross quad of a W1x row / of dZ: a c e | 0 (W1x) or g e (state record)
 constexpr int UP = NX + H1;       // 20 units per W1x row
 constexpr int RW = UP;            // partial record: a c e lin | h[16]
@@ -43,22 +36,15 @@ constexpr int DSTATE = NX + STATE;  // 48
 constexpr int NSMALL_X = NSMALL + 2;  // + sum g e, sum g
 constexpr int SPART = 2;              // threads per small gradient (174 threads, 16 samples each)
 constexpr int SPLEN = TS / SPART;
-static_assert(NKP * KPC == NCOL && (NKP - 1) * KPC <= MAXG * D, "the last warp owns the dense block");
 static_assert(DSTATE % 4 == 0 && SPART * NSMALL_X <= THREADS, "state record / small gradients");
 
 long long g_launches = 0;
 
 // shared memory carve-up (floats)
 constexpr int SM_W1X = NCOL * UP;          // 6400
-constexpr int SM_X = TS * XS;              // 10368
 constexpr int SM_P = NKP * RW * TS;        // 5120   partial records [kp][r][s]; reused as T[r][s] + M[s][DSTATE]
-constexpr int SM_R = 2 * TS * RS;          // 2496   ranks Rt[buffer][s][g]: this tile's and the prefetched next tile's
-constexpr int SM_WV = MAXG * TS;           // 1216   wide values WV[g][s]
-constexpr int SM_SMALL = 128;              // w2 64 | b2 4 | w3 4 | wd 16 | beta gamma
 constexpr size_t SMEM_BYTES = (size_t)(SM_W1X + SM_X + SM_P + SM_R + SM_WV + SM_SMALL) * sizeof(float);
-constexpr int SM_U = TS * RS;              // 1248   table rows only: ids Ut[s][g] of the next tile, behind the rest
 static_assert(RW * TS + DSTATE * TS <= SM_P, "T and the state records share P");
-static_assert(MAXG == B200_DEEPFM_TILE_MAXG, "include/b200_deepfm.h");
 // scratch: W1x [NCOL][UP] | tile counter | beta | gamma | pad
 constexpr int SCR_CNT = SM_W1X, SCR_BETA = SM_W1X + 1, SCR_GAMMA = SM_W1X + 2;
 static_assert(SM_W1X + 16 == B200_DEEPFM_DCN_SCRATCH, "include/b200_deepfm.h");
@@ -96,19 +82,6 @@ __host__ __device__ inline int w1x_src(const DcnLayout& d, int G, int c, int u) 
   }
   if (i < 0 || u == 3) return -1;
   return u == 0 ? d.o_cw + i : (u == 1 ? d.o_cw + d.l.in + i : d.o_wc + i);
-}
-
-// b200_deepfm_rows_t as the kernel reads it (parameter space): the param offsets folded into the bases.
-struct TileRows {
-  const int64_t* uniq;
-  const float* deep[MAXG];
-  const float* wide[MAXG];
-  long long deep_stride, wide_stride;
-};
-
-// Two units per call: two independent round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ float block_sum(float v, float* red) {  // all threads of a 256-thread block call it
@@ -211,76 +184,17 @@ __global__ void __launch_bounds__(THREADS, 2) k_dcn_tile(b200_deepfm_args_t a, c
   float loss_acc = 0.f;
   __syncthreads();
 
-  const long long ntile = ((long long)B + TS - 1) / TS;
-  const int g0 = warp * (KPC / D);
-  const int gl = max(0, min(G - g0, KPC / D));  // live groups of this warp
-  auto fetch_ranks = [&](const long long tl, int* dst) {
-    long long b = tl * TS + lane;
-    if (b >= B) b = B - 1;  // dead samples replay the last one, their results are masked
-    for (int k = 0; k < gl; ++k) cp_async4(dst + lane * RS + g0 + k, a.inv + (long long)(g0 + k) * B + b);
-  };
-  auto fetch_ids = [&](const int* R) {
-    for (int k = 0; k < gl; ++k) {
-      const int g = g0 + k;
-      cp_async4(Ut + lane * RS + g, rows.uniq + (long long)g * B + R[lane * RS + g]);
-    }
-  };
-  // dynamic tiles: s_tile[k & 1] = tile of iteration k, written during iteration k - 2 by thread 0
   __shared__ int s_tile[2];
-  int* tile_counter = reinterpret_cast<int*>(const_cast<float*>(w1x_g) + SCR_CNT);
-  if (t == 0) {
-    s_tile[0] = (int)blockIdx.x;
-    s_tile[1] = atomicAdd(tile_counter, 1);
-  }
+  const TileLoop<TABLE> tl(a, rows, X, WV, Rt0, Ut, s_tile, reinterpret_cast<int*>(const_cast<float*>(w1x_g) + SCR_CNT));
+  tl.start();
   int cur = 0;
-  if ((long long)blockIdx.x < ntile) fetch_ranks(blockIdx.x, Rt0);
-  cp_async_wait_all();
-  if (TABLE && (long long)blockIdx.x < ntile) {
-    fetch_ids(Rt0);
-    cp_async_wait_all();
-  }
-  __syncthreads();
   for (int iter = 0;; ++iter, cur ^= 1) {
     const int tile = s_tile[iter & 1], tile_next = s_tile[(iter + 1) & 1];
-    if (tile >= ntile) break;
+    if (tile >= tl.ntile) break;
     const long long b0 = (long long)tile * TS;
     int* Rt = Rt0 + cur * (TS * RS);
-    // ---------------- G: gather the tile once (each warp its own groups' rows) ----------------
     const bool live = b0 + lane < B;
-    {
-      if (TABLE) {
-        cp_async_wait_all();
-        __syncwarp();
-      }
-      float* xrow = X + lane * XS;
-      for (int k = 0; k < gl; ++k) {  // a lane pair copies one 32 B row
-        const int g = g0 + k;
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const int s = 16 * q + (lane >> 1), h = lane & 1;
-          const float* src = TABLE ? rows.deep[g] + Ut[s * RS + g] * rows.deep_stride
-                                   : a.bet_deep + ((long long)g * B + Rt[s * RS + g]) * D;
-          cp_async16(X + s * XS + g * D + 4 * h, src + 4 * h);
-        }
-        cp_async4(WV + g * TS + lane, TABLE ? rows.wide[g] + Ut[lane * RS + g] * rows.wide_stride
-                                            : a.bet_wide + (long long)g * B + Rt[lane * RS + g]);
-      }
-      if (tile_next < ntile) fetch_ranks(tile_next, Rt0 + (cur ^ 1) * (TS * RS));
-      for (int g = g0 + gl; g < min(g0 + KPC / D, MAXG); ++g) {  // unused group columns (G < 38): zeros
-        *reinterpret_cast<float4*>(xrow + g * D) = make_float4(0.f, 0.f, 0.f, 0.f);
-        *reinterpret_cast<float4*>(xrow + g * D + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (warp == NKP - 1) {  // tile columns 304..319: dense 13 | 1 | 0 | 0
-        const float* dense = a.dense + (live ? b0 + lane : B - 1) * ND;
-        for (int c = 0; c < ND; ++c) cp_async4(xrow + MAXG * D + c, dense + c);
-        xrow[MAXG * D + ND] = 1.0f;
-        xrow[MAXG * D + ND + 1] = 0.f;
-        xrow[MAXG * D + ND + 2] = 0.f;
-      }
-      cp_async_wait_all();
-      __syncwarp();
-      if (TABLE && tile_next < ntile) fetch_ids(Rt0 + (cur ^ 1) * (TS * RS));
-    }
+    tl.gather(b0, live, tile_next, Rt, cur);
     // ---------------- F: partial H1 / a c e / linear term over this warp's 40 columns ----------------
     {
       float2 h2[H1 / 2], hx = make_float2(0.f, 0.f);
@@ -332,26 +246,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_dcn_tile(b200_deepfm_args_t a, c
       }
     }
     __syncthreads();
-    if (t == 0) s_tile[iter & 1] = atomicAdd(tile_counter, 1);  // tile of iteration iter + 2
-    // ---------------- M: sum the 8 partial records ----------------
-    float tsum[3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      const int r = warp + 8 * i;
-      float v = 0.f;
-      if (r < RW) {
-#pragma unroll
-        for (int kp = 0; kp < NKP; ++kp) v += P[(kp * RW + r) * TS + lane];
-      }
-      tsum[i] = v;
-    }
-    __syncthreads();  // all partials read before T (aliasing P) is written
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      const int r = warp + 8 * i;
-      if (r < RW) T[r * TS + lane] = tsum[i];
-    }
-    __syncthreads();
+    tl.hand_out(iter);
+    sum_partials<RW>(P, warp, lane);
     // every warp: the per-sample tail (lane = sample)
     float hpre[H1], zero8[D];
 #pragma unroll
@@ -475,66 +371,16 @@ __global__ void __launch_bounds__(THREADS, 2) k_dcn_tile(b200_deepfm_args_t a, c
   }
 }
 
-int check_args(const b200_deepfm_args_t* a, bool backward) {
-  if (check_common(a, backward)) return -1;
-  if (a->G > MAXG) return fail(-1, "the DCN tile tower holds at most 38 id groups");
-  if (!a->scratch) return fail(-1, "null input");
-  if (a->rows) {
-    const b200_deepfm_rows_t* r = a->rows;
-    if (!backward) return fail(-1, "the forward-only DCN tile tower reads pulled rows only");
-    if (!r->uniq || r->deep_stride < D || r->wide_stride < 1 || r->deep_param_off < 0 || r->wide_param_off < 0 ||
-        r->deep_stride % 4 || r->deep_param_off % 4)
-      return fail(-1, "bad row source");
-    for (int g = 0; g < a->G; ++g)
-      if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15))
-        return fail(-1, "bad row source");
-  }
-  return 0;
-}
-
-template <bool BACKWARD, bool TABLE>
-void launch_tile(int dev, unsigned grid, cudaStream_t st, const b200_deepfm_args_t& a, const float* w1x, const TileRows& rows) {
-  constexpr size_t smem = SMEM_BYTES + (TABLE ? SM_U * sizeof(int) : 0);
-  max_dynamic_smem_once<k_dcn_tile<BACKWARD, TABLE>>(dev, (int)smem);
-  k_dcn_tile<BACKWARD, TABLE><<<grid, THREADS, smem, st>>>(a, w1x, rows);
+void prep(dim3 grid, cudaStream_t st, const b200_deepfm_args_t& a, float* w1x, int main_grid) {
+  k_dcn_prep<<<grid, THREADS, 0, st>>>(a, w1x, main_grid);
 }
 
 // what: 1 = prologue only (k_dcn_prep), 2 = tile kernel only, 3 = both
 template <bool BACKWARD>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
-  cudaStream_t st = (cudaStream_t)stream;
-  int n_sm;
-  const int dev = current_device(&n_sm);
-  b200_deepfm_args_t a = *args;
-  if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
-  float* w1x = a.scratch;
-  const long long ntile = ((long long)a.B + TS - 1) / TS;
-  long long grid = (long long)n_sm * 2;  // the 2 CTAs per SM of k_dcn_tile's __launch_bounds__
-  if (grid > ntile) grid = ntile;
-  if (what & 1) {
-    k_dcn_prep<<<dim3(4, BACKWARD ? a.G : 1), THREADS, 0, st>>>(a, w1x, (int)grid);
-    g_launches += 1;
-  }
-  if (!(what & 2)) return launch_status();
-  TileRows rows{};
-  if constexpr (BACKWARD) {
-    if (const b200_deepfm_rows_t* r = args->rows) {
-      rows.uniq = r->uniq;
-      for (int g = 0; g < a.G; ++g) {
-        rows.deep[g] = r->deep_base[g] + r->deep_param_off;
-        rows.wide[g] = r->wide_base[g] + r->wide_param_off;
-      }
-      rows.deep_stride = r->deep_stride;
-      rows.wide_stride = r->wide_stride;
-      launch_tile<true, true>(dev, (unsigned)grid, st, *args, w1x, rows);
-    } else {
-      launch_tile<true, false>(dev, (unsigned)grid, st, *args, w1x, rows);
-    }
-  } else {
-    launch_tile<false, false>(dev, (unsigned)grid, st, a, w1x, rows);
-  }
-  g_launches += 1;
-  return launch_status();
+  if (check_tile_args(args, BACKWARD, "DCN tile tower")) return -1;
+  return launch_tile_tower<BACKWARD, k_dcn_tile<BACKWARD, false>, k_dcn_tile<true, true>>(args, stream, what, SMEM_BYTES,
+                                                                                          prep, g_launches);
 }
 
 }  // namespace
@@ -546,22 +392,18 @@ size_t b200_deepfm_dcn_param_count(int G) { return G < 1 ? 0 : (size_t)dcn_layou
 int64_t b200_deepfm_dcn_launch_count(void) { return g_launches; }
 
 int b200_deepfm_dcn_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream);
 }
 
 int b200_deepfm_dcn_tile_prologue(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream, 1);
 }
 
 int b200_deepfm_dcn_tile_main(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream, 2);
 }
 
 int b200_deepfm_dcn_forward_tile(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, false)) return -1;
   return launch<false>(args, stream);
 }
 

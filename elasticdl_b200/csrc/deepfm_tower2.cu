@@ -3,11 +3,10 @@
 // Round 1's tower gathered every embedding row three times (forward, backward, parameter-gradient
 // kernel) with one dependent global gather chain per lane at low occupancy, most of the
 // step.  Here a CTA owns a tile of 32 samples and gathers the tile's 38 x 32 rows ONCE, with
-// cp.async (16 B, L2 -> shared memory, no registers held while in flight), into
-//     X[s] = [ deep 38 x 8 | dense 13 | 1 (bias column) | 0 0 | pad ]     (row stride 324 floats = 81 x 16 B,
-//            odd, so a warp's 32 rows are bank-conflict free for 128-bit reads; wide values in WV[g][s])
-// and everything else -- H1 = X W1x, the FM sums, the per-sample middle, dX = dH1 W1x^T + FM term with the
-// per-unique-id reduction, dW1x += dH1^T X and the small gradients -- runs out of shared memory:
+// cp.async (16 B, L2 -> shared memory, no registers held while in flight), into X (tile_tower.cuh: the tile
+// design this tower shares with dcn_tower.cu), and everything else -- H1 = X W1x, the FM sums, the per-sample
+// middle, dX = dH1 W1x^T + FM term with the per-unique-id reduction, dW1x += dH1^T X and the small gradients --
+// runs out of shared memory:
 //   G  gather             warp = the 5 id groups it reads in F (and the last warp the dense block), a lane pair
 //                         per 32 B row; F waits for the warp's own copies only (no CTA barrier between G and F)
 //   F  forward            warp = 40 tile columns (5 id groups), lane = sample: 16 accumulators + FM partials
@@ -25,50 +24,22 @@
 // with straight 16-byte copies.  fp32 SIMT: the step has 1 GFLOP of first-layer work, and the kernel waits on
 // the gather round trip and on its per-tile phases and barriers, not on FMA throughput (DESIGN.md section 10:
 // a 3xTF32 mma.sync version of F / B1 / B2 measured slower).
-#include "deepfm_common.cuh"
+#include "tile_tower.cuh"
 
 namespace {
 
 using namespace deepfm;
 
-constexpr int TS = 32;        // samples per tile
-constexpr int THREADS = 256;  // 8 warps
-constexpr int NKP = 8;        // column parts (warps) of phases F / B1
-constexpr int KPC = 40;       // tile columns per part = 5 id groups
-constexpr int NCOL = 320;     // deep 304 | dense 13 | 1 | 0 0   (G <= 38)
-constexpr int XS = 324;       // row stride: 320 + pad = 81 * 4 (odd number of 16 B quads: conflict-free 128-bit row reads)
-constexpr int RS = 39;        // rank row stride (odd): Rt[s][g]
 constexpr int RW = H1 + D + 2;  // partial record: h[16] | s[8] | q | lin
-constexpr int MAXG = 38;
 constexpr int SPART = 3;                       // threads per small gradient (255 threads, 11 samples each)
 constexpr int SPLEN = (TS + SPART - 1) / SPART;
-static_assert(NKP * KPC == NCOL && (NKP - 1) * KPC <= MAXG * D, "the last warp owns the dense block");
 
 long long g_launches = 0;
 
 // shared memory carve-up (floats)
 constexpr int SM_W1X = NCOL * H1;          // 5120
-constexpr int SM_X = TS * XS;              // 11648
 constexpr int SM_P = NKP * RW * TS;        // 6656   partial records [kp][r][s]; reused as T[r][s] + M[s][STATE]
-constexpr int SM_R = 2 * TS * RS;          // 2496   ranks Rt[buffer][s][g]: this tile's and the prefetched next tile's
-constexpr int SM_WV = MAXG * TS;           // 1216   wide values WV[g][s]
-constexpr int SM_SMALL = 128;              // b... w2 64 | b2 4 | w3 4 | wd 16
 constexpr size_t SMEM_BYTES = (size_t)(SM_W1X + SM_X + SM_P + SM_R + SM_WV + SM_SMALL) * sizeof(float);
-constexpr int SM_U = TS * RS;              // 1248   table rows only: ids Ut[s][g] of the next tile, behind the rest
-static_assert(MAXG == B200_DEEPFM_TILE_MAXG, "include/b200_deepfm.h");
-
-// b200_deepfm_rows_t as the kernel reads it (parameter space): the param offsets folded into the bases.
-struct TileRows {
-  const int64_t* uniq;
-  const float* deep[MAXG];
-  const float* wide[MAXG];
-  long long deep_stride, wide_stride;
-};
-
-// Two hidden units per call: two independent round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
 
 // Tile column c of W1x -> index into the flat parameter / gradient layout, or -1 (padding).
 __host__ __device__ inline int w1x_src(const Layout& l, int G, int c, int j) {
@@ -94,11 +65,6 @@ __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_p
   zero_step_outputs(a, n_params);
 }
 
-// TABLE: the rows come straight from the tables' record slabs (TileRows) instead of bet_deep / bet_wide, which
-// saves the step a separate pull kernel.  The id of a (sample, group) is one more dependent read between the
-// rank and the row, so the ids of tile i + 1 are fetched right after the ranks of tile i + 1 land (end of G)
-// and fly during the compute of tile i: G stays one round trip, and only a CTA's first tile pays
-// rank -> id -> row back to back.
 template <bool BACKWARD, bool TABLE>
 __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a, const float* __restrict__ w1x_g,
                                                            const __grid_constant__ TileRows rows) {
@@ -138,87 +104,17 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
   float loss_acc = 0.f;
   __syncthreads();
 
-  const long long ntile = ((long long)B + TS - 1) / TS;
-  // Warp w owns id groups g0 .. g0 + 4 (tile columns 40 w .. 40 w + 39) in G, F and B1, and warp NKP - 1 also the
-  // dense | 1 | 0 0 block: each warp gathers exactly what it reads in F, so F waits for the warp's own copies
-  // only, not for the whole tile behind a CTA barrier.
-  const int g0 = warp * (KPC / D);
-  const int gl = max(0, min(G - g0, KPC / D));  // live groups of this warp
-  // ranks of a tile: 4-byte cp.async, lane = sample, coalesced reads of inv (32 consecutive samples of one group)
-  auto fetch_ranks = [&](const long long tl, int* dst) {
-    long long b = tl * TS + lane;
-    if (b >= B) b = B - 1;  // dead samples replay the last one, their results are masked
-    for (int k = 0; k < gl; ++k) cp_async4(dst + lane * RS + g0 + k, a.inv + (long long)(g0 + k) * B + b);
-  };
-  // TABLE: the ids of a tile from its ranks, lane = sample; each lane reads the ranks its own copies wrote
-  auto fetch_ids = [&](const int* R) {
-    for (int k = 0; k < gl; ++k) {
-      const int g = g0 + k;
-      cp_async4(Ut + lane * RS + g, rows.uniq + (long long)g * B + R[lane * RS + g]);
-    }
-  };
-  // Tiles are handed out dynamically (one atomic per tile on a counter the prologue set to gridDim.x): with
-  // 1024 tiles on 296 resident CTAs a static round-robin leaves SMs with 8 tiles next to SMs with 6.  A CTA
-  // needs the index of its NEXT tile while it gathers the current one (rank prefetch), so two slots rotate:
-  // s_tile[k & 1] = tile of iteration k, written during iteration k - 2 (slot reuse) by thread 0.
   __shared__ int s_tile[2];
-  int* tile_counter = reinterpret_cast<int*>(const_cast<float*>(w1x_g) + SM_W1X);
-  if (t == 0) {
-    s_tile[0] = (int)blockIdx.x;
-    s_tile[1] = atomicAdd(tile_counter, 1);
-  }
+  const TileLoop<TABLE> tl(a, rows, X, WV, Rt0, Ut, s_tile, reinterpret_cast<int*>(const_cast<float*>(w1x_g) + SM_W1X));
+  tl.start();
   int cur = 0;
-  if ((long long)blockIdx.x < ntile) fetch_ranks(blockIdx.x, Rt0);
-  cp_async_wait_all();
-  if (TABLE && (long long)blockIdx.x < ntile) {
-    fetch_ids(Rt0);
-    cp_async_wait_all();
-  }
-  __syncthreads();
   for (int iter = 0;; ++iter, cur ^= 1) {
     const int tile = s_tile[iter & 1], tile_next = s_tile[(iter + 1) & 1];
-    if (tile >= ntile) break;
+    if (tile >= tl.ntile) break;
     const long long b0 = (long long)tile * TS;
     int* Rt = Rt0 + cur * (TS * RS);
-    // ---------------- G: gather the tile once ----------------
-    // The tile's ranks are already in Rt (prefetched while the previous tile was computed), so the gather is
-    // ONE global round trip: the row copies of this tile and the rank prefetch of the next one fly together.
-    // Each warp copies its own groups' rows.
     const bool live = b0 + lane < B;
-    {
-      if (TABLE) {  // this tile's ids (fetched during the previous tile's compute) from every lane of the warp
-        cp_async_wait_all();
-        __syncwarp();
-      }
-      float* xrow = X + lane * XS;
-      for (int k = 0; k < gl; ++k) {  // a lane pair copies one 32 B row: one request per row sector
-        const int g = g0 + k;
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const int s = 16 * q + (lane >> 1), h = lane & 1;
-          const float* src = TABLE ? rows.deep[g] + Ut[s * RS + g] * rows.deep_stride
-                                   : a.bet_deep + ((long long)g * B + Rt[s * RS + g]) * D;
-          cp_async16(X + s * XS + g * D + 4 * h, src + 4 * h);
-        }
-        cp_async4(WV + g * TS + lane, TABLE ? rows.wide[g] + Ut[lane * RS + g] * rows.wide_stride
-                                            : a.bet_wide + (long long)g * B + Rt[lane * RS + g]);
-      }
-      if (tile_next < ntile) fetch_ranks(tile_next, Rt0 + (cur ^ 1) * (TS * RS));
-      for (int g = g0 + gl; g < min(g0 + KPC / D, MAXG); ++g) {  // unused group columns (G < 38): zeros
-        *reinterpret_cast<float4*>(xrow + g * D) = make_float4(0.f, 0.f, 0.f, 0.f);
-        *reinterpret_cast<float4*>(xrow + g * D + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (warp == NKP - 1) {  // tile columns 304..319: dense 13 | 1 | 0 | 0
-        const float* dense = a.dense + (live ? b0 + lane : B - 1) * ND;
-        for (int c = 0; c < ND; ++c) cp_async4(xrow + MAXG * D + c, dense + c);
-        xrow[MAXG * D + ND] = 1.0f;
-        xrow[MAXG * D + ND + 1] = 0.f;
-        xrow[MAXG * D + ND + 2] = 0.f;
-      }
-      cp_async_wait_all();
-      __syncwarp();  // (TABLE: also orders this tile's reads of Ut before the overwrite below)
-      if (TABLE && tile_next < ntile) fetch_ids(Rt0 + (cur ^ 1) * (TS * RS));
-    }
+    tl.gather(b0, live, tile_next, Rt, cur);
     // ---------------- F: partial H1 / FM sums over this warp's 40 columns ----------------
     {
       float2 h2[H1 / 2];
@@ -271,26 +167,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
       mine[(H1 + D + 1) * TS] = lin;
     }
     __syncthreads();
-    if (t == 0) s_tile[iter & 1] = atomicAdd(tile_counter, 1);  // tile of iteration iter + 2 (every thread has read the slot)
-    // ---------------- M: sum the 8 partial records ----------------
-    float tsum[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = warp + 8 * i;
-      float v = 0.f;
-      if (r < RW) {
-#pragma unroll
-        for (int kp = 0; kp < NKP; ++kp) v += P[(kp * RW + r) * TS + lane];
-      }
-      tsum[i] = v;
-    }
-    __syncthreads();  // all partials read before T (aliasing P) is written
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = warp + 8 * i;
-      if (r < RW) T[r * TS + lane] = tsum[i];
-    }
-    __syncthreads();
+    tl.hand_out(iter);
+    sum_partials<RW>(P, warp, lane);
     // every warp: the per-sample tail (lane = sample)
     float hpre[H1], sd[D];
 #pragma unroll
@@ -441,66 +319,16 @@ __global__ void k_publish_loss(const float* __restrict__ loss, float* ring, int 
   *cursor = at + 1;
 }
 
-int check_args(const b200_deepfm_args_t* a, bool backward) {
-  if (check_common(a, backward)) return -1;
-  if (a->G > MAXG) return fail(-1, "the tile tower holds at most 38 id groups");
-  if (!a->scratch) return fail(-1, "null input");
-  if (a->rows) {
-    const b200_deepfm_rows_t* r = a->rows;
-    if (!backward) return fail(-1, "the forward-only tile tower reads pulled rows only");
-    if (!r->uniq || r->deep_stride < D || r->wide_stride < 1 || r->deep_param_off < 0 || r->wide_param_off < 0 ||
-        r->deep_stride % 4 || r->deep_param_off % 4)
-      return fail(-1, "bad row source");
-    for (int g = 0; g < a->G; ++g)
-      if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15))
-        return fail(-1, "bad row source");
-  }
-  return 0;
-}
-
-template <bool BACKWARD, bool TABLE>
-void launch_tile(int dev, unsigned grid, cudaStream_t st, const b200_deepfm_args_t& a, const float* w1x, const TileRows& rows) {
-  constexpr size_t smem = SMEM_BYTES + (TABLE ? SM_U * sizeof(int) : 0);
-  max_dynamic_smem_once<k_tower_tile<BACKWARD, TABLE>>(dev, (int)smem);
-  k_tower_tile<BACKWARD, TABLE><<<grid, THREADS, smem, st>>>(a, w1x, rows);
+void prep(dim3 grid, cudaStream_t st, const b200_deepfm_args_t& a, float* w1x, int main_grid) {
+  k_tile_prep<<<grid, 256, 0, st>>>(a, layout(a.G).total, w1x, main_grid);
 }
 
 // what: 1 = prologue only (k_tile_prep), 2 = tile kernel only, 3 = both
 template <bool BACKWARD>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
-  cudaStream_t st = (cudaStream_t)stream;
-  int n_sm;
-  const int dev = current_device(&n_sm);
-  b200_deepfm_args_t a = *args;
-  if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
-  float* w1x = a.scratch;  // NCOL*16 floats at the start of the scratch buffer, then the tile counter
-  const long long ntile = ((long long)a.B + TS - 1) / TS;
-  long long grid = (long long)n_sm * 2;  // the 2 CTAs per SM of k_tower_tile's __launch_bounds__
-  if (grid > ntile) grid = ntile;
-  if (what & 1) {
-    k_tile_prep<<<dim3(4, BACKWARD ? a.G : 1), 256, 0, st>>>(a, layout(a.G).total, w1x, (int)grid);
-    g_launches += 1;
-  }
-  if (!(what & 2)) return launch_status();
-  TileRows rows{};
-  if constexpr (BACKWARD) {  // only the training entry points accept a row source (check_args)
-    if (const b200_deepfm_rows_t* r = args->rows) {
-      rows.uniq = r->uniq;
-      for (int g = 0; g < a.G; ++g) {
-        rows.deep[g] = r->deep_base[g] + r->deep_param_off;
-        rows.wide[g] = r->wide_base[g] + r->wide_param_off;
-      }
-      rows.deep_stride = r->deep_stride;
-      rows.wide_stride = r->wide_stride;
-      launch_tile<true, true>(dev, (unsigned)grid, st, *args, w1x, rows);
-    } else {
-      launch_tile<true, false>(dev, (unsigned)grid, st, *args, w1x, rows);
-    }
-  } else {
-    launch_tile<false, false>(dev, (unsigned)grid, st, *args, w1x, rows);
-  }
-  g_launches += 1;
-  return launch_status();
+  if (check_tile_args(args, BACKWARD, "tile tower")) return -1;
+  return launch_tile_tower<BACKWARD, k_tower_tile<BACKWARD, false>, k_tower_tile<true, true>>(args, stream, what,
+                                                                                              SMEM_BYTES, prep, g_launches);
 }
 
 }  // namespace
@@ -510,17 +338,14 @@ extern "C" {
 int64_t b200_deepfm_tile_launch_count(void) { return g_launches; }
 
 int b200_deepfm_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream);
 }
 
 int b200_deepfm_tile_prologue(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream, 1);
 }
 
 int b200_deepfm_tile_main(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, true)) return -1;
   return launch<true>(args, stream, 2);
 }
 
@@ -532,7 +357,6 @@ int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int
 }
 
 int b200_deepfm_forward_tile(const b200_deepfm_args_t* args, void* stream) {
-  if (check_args(args, false)) return -1;
   return launch<false>(args, stream);
 }
 

@@ -15,11 +15,13 @@ fwd/bwd (torch, library GEMMs) -> segment-sum of per-occurrence gradients -> pus
 76 tables, fused Adam) -> version++.  No host sync inside the step; nothing but
 ids/features/labels comes from the host.
 """
+import collections
+import ctypes
 import math
 
 import torch
 
-from elasticdl_b200._lib import MAX_SEGS, check
+from elasticdl_b200._lib import DEEPFM_DCN_SCRATCH, DEEPFM_TILE_MAXG, DEEPFM_TILE_SCRATCH, MAX_SEGS, check
 
 # model_zoo/dac_ctr/feature_config.py:61-75 (len(boundaries)+1 buckets; I4 is not in FEATURE_GROUPS)
 INT_BUCKETS = [5, 10, 9, 10, 9, 9, 10, 10, 3, 6, 2, 9]
@@ -286,6 +288,30 @@ def _tower_error(lib):
     return lib.b200_deepfm_last_error().decode("utf-8", "replace")
 
 
+# What DeepFMPSEngine calls for its model on its tower kind (tower_calls): fwd_bwd, the one-call training step (None
+# on tower="torch"); prologue / main, the tile tower's training step split in two (None elsewhere); forward,
+# predict()'s tower; param_count(G), the flat parameter count; scratch, the floats the tile tower needs of `scratch`;
+# regularized, whether the torch loss adds tower.regularization().
+TowerCalls = collections.namedtuple("TowerCalls", "fwd_bwd prologue main forward param_count scratch regularized")
+
+
+def tower_calls(lib, model, tower):
+    tile = tower == "tile"
+    return {
+        "deepfm": TowerCalls(
+            {"tile": lib.b200_deepfm_fwd_bwd_tile, "fused": lib.b200_deepfm_fwd_bwd,
+             "mma": lib.b200_deepfm_fwd_bwd_mma}.get(tower),
+            lib.b200_deepfm_tile_prologue if tile else None, lib.b200_deepfm_tile_main if tile else None,
+            lib.b200_deepfm_forward_tile if tile else lib.b200_deepfm_forward,
+            lib.b200_deepfm_param_count, DEEPFM_TILE_SCRATCH, False),
+        "dcn": TowerCalls(
+            lib.b200_deepfm_dcn_fwd_bwd_tile if tile else None,
+            lib.b200_deepfm_dcn_tile_prologue if tile else None, lib.b200_deepfm_dcn_tile_main if tile else None,
+            lib.b200_deepfm_dcn_forward_tile,
+            lib.b200_deepfm_dcn_param_count, DEEPFM_DCN_SCRATCH, True),
+    }[model]
+
+
 def resolve_row_source(row_source, tower, n_shards, exchange, paired):
     """DeepFMPSEngine's row_source: "table" (the tower reads the table records) needs the tile tower and every
     record on this GPU in its own slab -- one shard, the direct exchange, unpaired tables."""
@@ -319,12 +345,13 @@ class DeepFMPSEngine:
             raise ValueError("model must be one of %s, not %r" % (sorted(TOWERS), model))
         if model == "dcn" and tower not in ("tile", "torch"):
             raise ValueError('model="dcn" runs on tower="tile" or "torch", not %r' % tower)
-        if model == "dcn" and len(group_rows) > 38:
-            raise ValueError('model="dcn" holds at most 38 id groups, not %d' % len(group_rows))
+        if model == "dcn" and len(group_rows) > DEEPFM_TILE_MAXG:
+            raise ValueError('model="dcn" holds at most %d id groups, not %d' % (DEEPFM_TILE_MAXG, len(group_rows)))
         self.model = model
-        if tower == "tile" and len(group_rows) > 38:
+        if tower == "tile" and len(group_rows) > DEEPFM_TILE_MAXG:
             tower = "fused"  # the tile tower holds at most 38 id groups in its shared-memory row
         self.tower_kind = tower
+        self.calls = tower_calls(group.lib, model, tower)
         # paired=True: the deep (dim 8) and wide (dim 1) tables of an id group share one record
         # per id, so one request per id serves both (ps_kernels.cuh "Paired tables")
         # (default: when rows live on peer GPUs -- remote reads are bounded by requests in flight)
@@ -362,7 +389,7 @@ class DeepFMPSEngine:
             self.deep_ids = [group.register_table(n, D, "zero", r) for n, r in zip(self.deep_names, group_rows)]
         torch.manual_seed(seed)
         self.tower = TOWERS[model](G, D).to(dev)
-        n_flat = int((group.lib.b200_deepfm_dcn_param_count if model == "dcn" else group.lib.b200_deepfm_param_count)(G))
+        n_flat = int(self.calls.param_count(G))
         self.flat_params = torch.zeros(n_flat, dtype=torch.float32, device=dev)
         self.flat_grads = torch.zeros(n_flat, dtype=torch.float32, device=dev)
         self.flat_views = flatten_tower(self.tower, self.flat_params)
@@ -417,10 +444,8 @@ class DeepFMPSEngine:
         self.act_d = torch.empty((G * B, D), **f32)
         self.gsum_w = torch.zeros((G * B, 1), **f32)
         self.gsum_d = torch.zeros((G * B, D), **f32)
-        n_scratch = max(B * 44 + 16 * (N_DENSE + D * G), 320 * 16 + 16)  # b200_deepfm.h: backward state + W1^T | tile tower: W1 tile + counter
-        if model == "dcn":
-            n_scratch = max(n_scratch, 320 * 20 + 16)  # B200_DEEPFM_DCN_SCRATCH
-        self.scratch = torch.empty(n_scratch, **f32)
+        # b200_deepfm.h: backward state + W1^T (fused / mma) | the tile tower's
+        self.scratch = torch.empty(max(B * 44 + 16 * (N_DENSE + D * G), self.calls.scratch), **f32)
         self.loss_buf = torch.zeros(1, **f32)
         # the loss of every step also lands in a ring of pinned host memory, written by a 1-thread kernel at the end
         # of the step (b200_deepfm_publish_loss): loss_host(k) reads step k's value after a synchronize, no D2H copy
@@ -553,7 +578,6 @@ class DeepFMPSEngine:
         def done(e):
             if e is not None:
                 e[1].record()
-        import ctypes as _ct
 
         # Branches: the step has six launch-bound kernels (pull_dense, tower prologue, push_begin, push_dense,
         # push_end) that do not depend on the row kernels beside them.  With
@@ -579,10 +603,7 @@ class DeepFMPSEngine:
             with torch.cuda.stream(self.aux):
                 arr, n = self.pull_dense_segs
                 check(lib.b200ps_pull_dense(h, arr, n, g._stream()))
-                prologue = lib.b200_deepfm_dcn_tile_prologue if self.model == "dcn" else lib.b200_deepfm_tile_prologue
-                rc = prologue(_ct.byref(a), g._stream())
-                if rc:
-                    raise RuntimeError("%s failed (%d): %s" % (prologue.__name__, rc, _tower_error(lib)))
+                self._tower_call(self.calls.prologue, a, g._stream())
                 ev_prep = torch.cuda.Event()
                 ev_prep.record(self.aux)  # the tower waits for this, not for push_begin behind it
                 g.push_begin(self.lr, self.zero_versions)
@@ -610,24 +631,15 @@ class DeepFMPSEngine:
                     done(e)
         if branch:
             main.wait_event(ev_prep)
-            tile_main = lib.b200_deepfm_dcn_tile_main if self.model == "dcn" else lib.b200_deepfm_tile_main
-            rc = tile_main(_ct.byref(a), st)
-            if rc:
-                raise RuntimeError("%s failed (%d): %s" % (tile_main.__name__, rc, _tower_error(lib)))
+            self._tower_call(self.calls.main, a, st)
             loss = self.loss_buf
             dense_segs = self.push_dense_segs
-        elif self.tower_kind in ("tile", "fused", "mma"):
+        elif self.calls.fwd_bwd is not None:
             # (4-6) gather + tower forward/backward + per-unique-id gradient sums: three launches
             e_t = mark("tower_fwd_bwd")
             a = self.tower_args
             a.dense, a.labels = dense.data_ptr(), labels.data_ptr()
-
-            fn = {"mma": lib.b200_deepfm_fwd_bwd_mma, "tile": lib.b200_deepfm_fwd_bwd_tile}.get(self.tower_kind, lib.b200_deepfm_fwd_bwd)
-            if self.model == "dcn":
-                fn = lib.b200_deepfm_dcn_fwd_bwd_tile
-            rc = fn(_ct.byref(a), st)
-            if rc:
-                raise RuntimeError("b200_deepfm_fwd_bwd failed (%d): %s" % (rc, _tower_error(lib)))
+            self._tower_call(self.calls.fwd_bwd, a, st)
             done(e_t)
             loss = self.loss_buf
             dense_segs = self.push_dense_segs
@@ -667,6 +679,13 @@ class DeepFMPSEngine:
         g.push_end(sync=False)
         self.steps += 1
         return loss.detach().reshape(())
+
+    def _tower_call(self, fn, args, st):
+        """One tower entry point on `args` (DeepFMArgs); RuntimeError with its return code and
+        b200_deepfm_last_error if it fails."""
+        rc = fn(ctypes.byref(args), st)
+        if rc:
+            raise RuntimeError("%s failed (%d): %s" % (fn.__name__, rc, _tower_error(self.group.lib)))
 
     def _publish_loss(self, loss, st):
         if loss is not self.loss_buf:  # torch tower: its loss tensor is not persistent
@@ -834,7 +853,7 @@ class DeepFMPSEngine:
         deep = act_d.view(G, B, D).permute(1, 0, 2)
         logits = self.tower(dense, wide, deep)
         loss = self.loss_fn(logits, labels)
-        if self.model == "dcn":
+        if self.calls.regularized:
             loss = loss + self.tower.regularization()
         plist = [p for _, p in self.params]
         grads = torch.autograd.grad(loss, plist + [act_w, act_d])
@@ -872,15 +891,9 @@ class DeepFMPSEngine:
                                     self.n_unique.data_ptr(), ws.data_ptr(), ws.numel(), st))
             for arr, n in self.pull_segs:
                 check(lib.b200ps_pull_rows(h, arr, n, st))
-            import ctypes as _ct
-
             a = self.tower_args
             a.dense = dense.data_ptr()
-            fwd = lib.b200_deepfm_forward_tile if self.tower_kind == "tile" else lib.b200_deepfm_forward
-            if self.model == "dcn":
-                fwd = lib.b200_deepfm_dcn_forward_tile
-            if fwd(_ct.byref(a), st):
-                raise RuntimeError("b200_deepfm_forward failed: %s" % _tower_error(lib))
+            self._tower_call(self.calls.forward, a, st)
         finally:
             self.__dict__.update(saved)
         return self.logits_buf
