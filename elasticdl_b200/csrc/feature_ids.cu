@@ -10,6 +10,7 @@
 #include <cstdint>
 #include <cstring>
 #include <string>
+#include <type_traits>
 
 #include "../../include/b200_features.h"
 
@@ -142,9 +143,10 @@ struct Plan {  // passed by value (< 4 KB): the launch is self-contained and cap
   int G, n_dense;
 };
 
-__global__ void __launch_bounds__(256) k_feature_transform(Plan p, const void* numeric,
-                                                           int numeric_is_float, const uint8_t* __restrict__ strings, int W,
-                                                           long long B, void* ids_out, int ids32, float* dense_out) {
+// T: the numeric columns' type (long long or float)
+template <typename T>
+__global__ void __launch_bounds__(256) k_feature_transform(Plan p, const T* numeric, const uint8_t* __restrict__ strings,
+                                                           int W, long long B, void* ids_out, int ids32, float* dense_out) {
   __shared__ float s_bnd[kMaxBoundaries];
   const int g = blockIdx.y;
   if (g < p.G) {
@@ -158,18 +160,14 @@ __global__ void __launch_bounds__(256) k_feature_transform(Plan p, const void* n
       long long id;
       if (gr.kind == B200FEAT_DISCRETIZE) {
         // int64 inputs compare against float boundaries in float, like TF's BucketizeOp<T>
-        const float x = numeric_is_float ? reinterpret_cast<const float*>(numeric)[(long long)gr.column * B + b]
-                                         : (float)reinterpret_cast<const long long*>(numeric)[(long long)gr.column * B + b];
-        id = bucketize(x, s_bnd, gr.n_boundaries);
+        id = bucketize((float)numeric[(long long)gr.column * B + b], s_bnd, gr.n_boundaries);
       } else {
         unsigned char buf[kMaxW];
-        int len;
+        int len = 0;
         if (gr.kind == B200FEAT_HASH_STRING) {
           len = load_string(strings + ((long long)gr.column * B + b) * W, W, buf);
-        } else {
-          const long long v = numeric_is_float ? (long long)reinterpret_cast<const float*>(numeric)[(long long)gr.column * B + b]
-                                               : reinterpret_cast<const long long*>(numeric)[(long long)gr.column * B + b];
-          len = as_string(v, buf);
+        } else if constexpr (std::is_same<T, long long>::value) {  // the host refuses HASH_INT over float columns
+          len = as_string(numeric[(long long)gr.column * B + b], buf);
         }
         id = (long long)(fingerprint64(buf, len) % (uint64_t)gr.num_bins);
       }
@@ -182,8 +180,7 @@ __global__ void __launch_bounds__(256) k_feature_transform(Plan p, const void* n
     const b200feat_dense_t& d = p.dense[j];
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += stride) {
-      const double x = numeric_is_float ? (double)reinterpret_cast<const float*>(numeric)[(long long)d.column * B + b]
-                                        : (double)reinterpret_cast<const long long*>(numeric)[(long long)d.column * B + b];
+      const double x = (double)numeric[(long long)d.column * B + b];
       dense_out[b * p.n_dense + j] = (float)((x - d.subtractor) / d.divisor);
     }
   }
@@ -224,7 +221,9 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
                        const b200feat_dense_t* dense, int n_dense, const void* numeric_dev, int n_numeric,
                        int numeric_is_float, const uint8_t* strings_dev, int n_string, int W, int64_t B,
                        void* ids_out_dev, int ids32, float* dense_out_dev, void* stream) {
-  if (G < 0 || G > kMaxGroups || n_dense < 0 || n_dense > kMaxDense || B < 1) return fail(-1, "bad transform shape");
+  if (G < 0 || G > kMaxGroups) return fail(-1, "bad group count (max 64)");
+  if (n_dense < 0 || n_dense > kMaxDense) return fail(-1, "bad dense column count (max 32)");
+  if (B < 1) return fail(-1, "bad batch size");
   if (n_boundaries < 0 || n_boundaries > kMaxBoundaries) return fail(-1, "too many boundaries (max 256)");
   if (G > 0 && (!groups || !ids_out_dev)) return fail(-1, "groups / ids_out is null");
   if (n_dense > 0 && (!dense || !dense_out_dev)) return fail(-1, "dense / dense_out is null");
@@ -235,19 +234,31 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
   p.n_dense = dense_out_dev ? n_dense : 0;
   for (int g = 0; g < p.G; ++g) {
     const b200feat_group_t& gr = groups[g];
+    int64_t span;  // largest id before the offset
     if (gr.kind == B200FEAT_DISCRETIZE) {
       if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "discretize: bad numeric column");
       if (gr.n_boundaries < 0 || gr.boundary_off < 0 || gr.boundary_off + gr.n_boundaries > n_boundaries || (gr.n_boundaries && !boundaries))
         return fail(-1, "discretize: boundaries out of range");
+      // the kernel binary-searches them; TF's Bucketize refuses unsorted boundaries
+      for (int i = gr.boundary_off; i < gr.boundary_off + gr.n_boundaries; ++i)
+        if (boundaries[i] != boundaries[i] || (i > gr.boundary_off && boundaries[i] < boundaries[i - 1]))
+          return fail(-1, "discretize: boundaries are not sorted in ascending order (or hold a NaN)");
+      span = gr.n_boundaries;
     } else if (gr.kind == B200FEAT_HASH_STRING) {
       if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1) return fail(-1, "hash: bad string column");
       if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");  // hashing.py:53-56
+      span = gr.num_bins - 1;
     } else if (gr.kind == B200FEAT_HASH_INT) {
       if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "hash: bad numeric column");
       if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");
+      // Hashing converts integer inputs only (hashing.py:63-72); to_hash_bucket_fast refuses float tensors
+      if (numeric_is_float) return fail(-1, "hash_int: Hashing takes integer columns, these numeric columns are float32");
+      span = gr.num_bins - 1;
     } else {
       return fail(-1, "unknown group kind");
     }
+    if (ids32 && (gr.offset < INT32_MIN || gr.offset > (int64_t)INT32_MAX - span))
+      return fail(-1, "int32 ids: offset + id range of a group does not fit int32");
     p.group[g] = gr;
   }
   for (int j = 0; j < p.n_dense; ++j) {
@@ -262,8 +273,12 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
   const int per = (max_blocks() + p.G + p.n_dense - 1) / (p.G + p.n_dense);
   if (gx > per) gx = per < 1 ? 1 : per;
   dim3 grid(gx, p.G + p.n_dense);
-  k_feature_transform<<<grid, 256, 0, st>>>(p, numeric_dev, numeric_is_float, strings_dev, W, (long long)B, ids_out_dev,
-                                            ids32, dense_out_dev);
+  if (numeric_is_float)
+    k_feature_transform<<<grid, 256, 0, st>>>(p, (const float*)numeric_dev, strings_dev, W, (long long)B, ids_out_dev,
+                                              ids32, dense_out_dev);
+  else
+    k_feature_transform<<<grid, 256, 0, st>>>(p, (const long long*)numeric_dev, strings_dev, W, (long long)B, ids_out_dev,
+                                              ids32, dense_out_dev);
   g_launches++;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(-2, cudaGetErrorString(e));

@@ -14,7 +14,8 @@
  *
  * Inputs are FEATURE-MAJOR device arrays, like the reference's one-Keras-input-per-feature tensors:
  *   numeric  [n_numeric][B]      int64 (dac_ctr: tf.io.FixedLenFeature((1,), tf.int64)) or float32
- *   strings  [n_string][B][W]    zero-padded byte strings of at most W <= 64 bytes
+ *   strings  [n_string][B][W]    zero-padded byte strings of at most W <= 64 bytes (a string ends at its
+ *                                first NUL, so a string holding a NUL byte cannot be carried)
  * Outputs: ids [G][B] (int64 or int32), the layout b200ps_unique takes; dense [B][n_dense] float32.
  *
  * Parity: Fingerprint64 is third-party arithmetic (TensorFlow / FarmHash, not under /root/reference).
@@ -36,7 +37,7 @@ extern "C" {
 enum {
   B200FEAT_DISCRETIZE = 0,  /* Discretization(bins) of numeric column `column` */
   B200FEAT_HASH_STRING = 1, /* Hashing(num_bins) of string column `column` */
-  B200FEAT_HASH_INT = 2     /* Hashing(num_bins) of numeric (integer) column `column`: tf.as_string, then hash */
+  B200FEAT_HASH_INT = 2     /* Hashing(num_bins) of numeric column `column`: tf.as_string, then hash (int64 columns only) */
 };
 
 /* One output id group = one feature transformed + its ConcatenateWithOffset offset
@@ -44,7 +45,7 @@ enum {
 typedef struct {
   int32_t kind;
   int32_t column;
-  int32_t n_boundaries; /* DISCRETIZE: boundaries_dev[boundary_off .. boundary_off + n_boundaries), ascending */
+  int32_t n_boundaries; /* DISCRETIZE: boundaries[boundary_off .. boundary_off + n_boundaries), ascending, no NaN */
   int32_t boundary_off;
   int64_t num_bins;     /* HASH_*: > 0 */
   int64_t offset;       /* added to the id (ConcatenateWithOffset) */
@@ -63,8 +64,10 @@ const char* b200feat_last_error(void);
 /* One fused launch: ids_out_dev[g*B + b] for every group, dense_out_dev[b*n_dense + j] for every
  * normalised column.  groups / dense descriptors and boundaries are HOST arrays (copied by value into
  * the launch, G <= 64, n_dense <= 32, total boundaries <= 256).  numeric_is_float: 0 = int64 columns,
- * 1 = float32 columns.  ids32: 0 = int64 ids, 1 = int32 ids (narrow transport into
- * b200ps_unique_bounded_i32).  Any of the two outputs may be NULL. */
+ * 1 = float32 columns (Discretization compares them in float, like int64 columns; HASH_INT refuses them).
+ * ids32: 0 = int64 ids, 1 = int32 ids (narrow transport into b200ps_unique_bounded_i32); a group whose
+ * ids [offset, offset + num_bins) or [offset, offset + n_boundaries] leave int32 is refused.
+ * Any of the two outputs may be NULL. */
 int b200feat_transform(const b200feat_group_t* groups, int G, const float* boundaries, int n_boundaries,
                        const b200feat_dense_t* dense, int n_dense, const void* numeric_dev, int n_numeric,
                        int numeric_is_float, const uint8_t* strings_dev, int n_string, int W, int64_t B,

@@ -5,7 +5,7 @@ Follows (paths relative to /root/reference/):
   * elasticdl_preprocessing/layers/hashing.py:61-92       Hashing: tf.as_string for ints, then
         tf.strings.to_hash_bucket_fast = FarmHash Fingerprint64(bytes) % num_bins (unsigned)
   * elasticdl_preprocessing/layers/discretization.py:60-78 Discretization: math_ops._bucketize =
-        std::upper_bound over the boundaries (bins include their left boundary), cast to int64
+        std::upper_bound over the float32 boundaries (bins include their left boundary), cast to int64
   * elasticdl_preprocessing/layers/concatenate_with_offset.py:50-87
   * elasticdl_preprocessing/layers/normalizer.py          (x - subtractor) / divisor in float64
   * model_zoo/dac_ctr/feature_transform.py:36-118         their composition
@@ -109,11 +109,15 @@ def hashing(values, num_bins):
 
 
 def discretize(values, bins):
-    """Discretization(bins)(values): id = number of boundaries <= x; int64 inputs compare in float32
-    like TF's BucketizeOp<T> (std::upper_bound with float boundaries)."""
-    x = np.asarray(values)
-    b = np.asarray(bins, dtype=np.float32)
-    xf = x.astype(np.float32)
+    """Discretization(bins)(values): id = number of boundaries <= x, compared in float32 for every input.
+    The layer is a Keras Layer of the default float32 dtype policy: its __call__ autocasts floating inputs
+    (float64 and Python floats too) to float32, and BucketizeOp<int64> compares `int64 < float boundary` in
+    float (std::upper_bound with float boundaries).  Unsorted (or NaN) boundaries are refused, as Bucketize
+    refuses them."""
+    b = np.asarray(bins, dtype=np.float32).reshape(-1)
+    if np.isnan(b).any() or np.any(b[1:] < b[:-1]):
+        raise ValueError("boundaries must be sorted in ascending order")
+    xf = np.asarray(values).astype(np.float32)
     return np.searchsorted(b, xf, side="right").astype(np.int64)
 
 

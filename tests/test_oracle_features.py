@@ -51,3 +51,32 @@ def test_normalizer_example():
     assert np.allclose(FO.normalize([[3.0], [5.0], [7.0]], 1.0, 2.0), [[1.0], [2.0], [3.0]])  # normalizer.py docstring
     with pytest.raises(ValueError):
         FO.normalize([1.0], 0.0, 0)
+
+
+def test_discretize_compares_every_input_in_float32():
+    # the reference layer's Keras __call__ autocasts floating inputs to its float32 compute dtype, so a float64
+    # value next to a boundary rounds onto it before math_ops._bucketize sees it
+    x64 = np.array([0.99999999, np.nextafter(1.0, 0.0), 1.0, np.nextafter(1.0, 2.0), 0.9999999], dtype=np.float64)
+    assert np.array_equal(FO.discretize(x64, [1.0]), [1, 1, 1, 1, 0])
+    assert np.array_equal(FO.discretize(x64.astype(np.float32), [1.0]), [1, 1, 1, 1, 0])
+    assert np.array_equal(FO.discretize([0.99999999], [1.0]), [1])  # Python floats are float32 tensors too
+    assert np.array_equal(FO.discretize(np.array([0.1]), [0.1]), [1])  # both round to float32(0.1)
+    # int64 values round to float32 before the comparison: 16777217 -> 16777216.0f, 16777219 -> 16777220.0f
+    ints = np.array([16777215, 16777216, 16777217, 16777218, 16777219], dtype=np.int64)
+    assert np.array_equal(FO.discretize(ints, [16777216.0]), [0, 1, 1, 1, 1])
+    assert np.array_equal(FO.discretize(ints, [16777217.0, 16777220.0]), [0, 1, 1, 1, 2])
+    assert np.array_equal(FO.discretize(ints.astype(np.int32), [16777217.0]), [0, 1, 1, 1, 1])
+    # NaN sorts past every boundary (upper_bound: NaN < b is false), -0.0 == 0.0 lands right of a 0 boundary
+    for dt in (np.float32, np.float64):
+        v = np.array([np.nan, -0.0, 0.0, -np.inf, np.inf], dtype=dt)
+        assert np.array_equal(FO.discretize(v, [-1.0, 0.0, 1.0]), [3, 2, 2, 0, 3])
+    assert np.array_equal(FO.discretize([1.5, -3.0], []), [0, 0])
+
+
+def test_discretize_refuses_unsorted_boundaries():
+    with pytest.raises(ValueError, match="sorted"):
+        FO.discretize([1.0], [0.0, 2.0, 1.0])
+    with pytest.raises(ValueError, match="sorted"):
+        FO.discretize([1.0], [0.0, np.nan])
+    # repeated boundaries and -0.0 next to 0.0 are sorted
+    assert np.array_equal(FO.discretize([0.0, 1.0], [-0.0, 0.0, 1.0, 1.0]), [2, 4])
