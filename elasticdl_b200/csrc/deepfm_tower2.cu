@@ -1,4 +1,5 @@
-// DeepFM tower, tile version (include/b200_deepfm.h: b200_deepfm_fwd_bwd_tile / b200_deepfm_forward_tile).
+// DeepFM tower, tile version (include/b200_deepfm.h: b200_deepfm_fwd_bwd_tile / b200_deepfm_forward_tile), and the
+// Wide & Deep tower (b200_deepfm_wide_deep_*) as its instances without the FM term (k_tower_tile<..., FM = false>).
 //
 // Round 1's tower gathered every embedding row three times (forward, backward, parameter-gradient
 // kernel) with one dependent global gather chain per lane at low occupancy, most of the
@@ -65,7 +66,9 @@ __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_p
   zero_step_outputs(a, n_params);
 }
 
-template <bool BACKWARD, bool TABLE>
+// FM = false is the Wide & Deep model (b200_deepfm_wide_deep_*): DeepFM without its FM term, so F does not sum the
+// FM partials (their records stay 0), the tail gets zero FM sums and B1's row gradient is the DNN's alone.
+template <bool BACKWARD, bool TABLE, bool FM>
 __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a, const float* __restrict__ w1x_g,
                                                            const __grid_constant__ TileRows rows) {
   extern __shared__ __align__(16) float smem[];
@@ -133,8 +136,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         const float xv[D] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
         const int g = c / D;
         if (g < G) {  // an embedding group: FM sums + the wide value
+          if constexpr (FM) {
 #pragma unroll
-          for (int d = 0; d < D; ++d) { sd[d] += xv[d]; q = fmaf(xv[d], xv[d], q); }
+            for (int d = 0; d < D; ++d) { sd[d] += xv[d]; q = fmaf(xv[d], xv[d], q); }
+          }
           lin += WV[g * TS + lane];
         } else if (c == MAXG * D) {  // dense columns 304..311 and (next chunk) 312..316: the linear part
 #pragma unroll
@@ -174,10 +179,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
 #pragma unroll
     for (int j = 0; j < H1; ++j) hpre[j] = T[j * TS + lane];
 #pragma unroll
-    for (int d = 0; d < D; ++d) sd[d] = T[(H1 + d) * TS + lane];
-    const float q = T[(H1 + D) * TS + lane], lin = T[(H1 + D + 1) * TS + lane];
+    for (int d = 0; d < D; ++d) sd[d] = FM ? T[(H1 + d) * TS + lane] : 0.f;
+    const float q = FM ? T[(H1 + D) * TS + lane] : 0.f, lin = T[(H1 + D + 1) * TS + lane];
     float a1[H1], h2[H2];
-    const float z = forward_tail(hpre, sd, q, lin, s_w2, s_b2, s_w3, a1, h2);
+    const float z = forward_tail(hpre, sd, q, lin, s_w2, s_b2, s_w3, a1, h2);  // FM = false: lin + w3 . h2
     if (warp == 0 && live && a.logits != nullptr) a.logits[b0 + lane] = z;
     float dz = 0.f, dh1[H1];
     if (BACKWARD) {
@@ -219,7 +224,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
         const int g = warp * (KPC / D) + gi;
         if (g >= G) break;  // warp-uniform
         const int c = g * D;
-        const float4 xa = *reinterpret_cast<const float4*>(xrow + c);
+        const float4 xa = *reinterpret_cast<const float4*>(xrow + c);  // the group's row: the FM term (unused without)
         const float4 xb = *reinterpret_cast<const float4*>(xrow + c + 4);
         const float ev[D] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
         float x[D + 1];
@@ -233,7 +238,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
             dt2 = ffma2(make_float2(w.x, w.y), make_float2(dh1[4 * qd + 0], dh1[4 * qd + 1]), dt2);
             dt2 = ffma2(make_float2(w.z, w.w), make_float2(dh1[4 * qd + 2], dh1[4 * qd + 3]), dt2);
           }
-          x[d] = fmaf(dz, sd[d] - ev[d], dt2.x + dt2.y);
+          if constexpr (FM)
+            x[d] = fmaf(dz, sd[d] - ev[d], dt2.x + dt2.y);
+          else
+            x[d] = dt2.x + dt2.y;
         }
         x[D] = dz;  // wide row gradient
         // warp-level id dedup (dedup_red): lanes hitting the same row combine pairwise up a tree threaded through
@@ -323,12 +331,12 @@ void prep(dim3 grid, cudaStream_t st, const b200_deepfm_args_t& a, float* w1x, i
   k_tile_prep<<<grid, 256, 0, st>>>(a, layout(a.G).total, w1x, main_grid);
 }
 
-// what: 1 = prologue only (k_tile_prep), 2 = tile kernel only, 3 = both
-template <bool BACKWARD>
+// what: 1 = prologue only (k_tile_prep), 2 = tile kernel only, 3 = both.  FM: DeepFM, else Wide & Deep.
+template <bool BACKWARD, bool FM = true>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
-  if (check_tile_args(args, BACKWARD, "tile tower")) return -1;
-  return launch_tile_tower<BACKWARD, k_tower_tile<BACKWARD, false>, k_tower_tile<true, true>>(args, stream, what,
-                                                                                              SMEM_BYTES, prep, g_launches);
+  if (check_tile_args(args, BACKWARD, FM ? "tile tower" : "Wide & Deep tile tower")) return -1;
+  return launch_tile_tower<BACKWARD, k_tower_tile<BACKWARD, false, FM>, k_tower_tile<true, true, FM>>(
+      args, stream, what, SMEM_BYTES, prep, g_launches);
 }
 
 }  // namespace
@@ -358,6 +366,22 @@ int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int
 
 int b200_deepfm_forward_tile(const b200_deepfm_args_t* args, void* stream) {
   return launch<false>(args, stream);
+}
+
+int b200_deepfm_wide_deep_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
+  return launch<true, false>(args, stream);
+}
+
+int b200_deepfm_wide_deep_tile_prologue(const b200_deepfm_args_t* args, void* stream) {
+  return launch<true, false>(args, stream, 1);
+}
+
+int b200_deepfm_wide_deep_tile_main(const b200_deepfm_args_t* args, void* stream) {
+  return launch<true, false>(args, stream, 2);
+}
+
+int b200_deepfm_wide_deep_forward_tile(const b200_deepfm_args_t* args, void* stream) {
+  return launch<false, false>(args, stream);
 }
 
 }  // extern "C"

@@ -59,6 +59,21 @@ class DeepFMTower(torch.nn.Module):
         return linear_logit + dnn_logit + fm
 
 
+class WideDeepTower(DeepFMTower):
+    """wide_deep_model.py:62-107 without the embedding lookups: DeepFMTower without the FM term (the same
+    parameters, under the same names, so the flat layout is DeepFM's)."""
+
+    def forward(self, dense, wide, deep):
+        """dense [B,13], wide [B,G], deep [B,G,D] -> logits [B]."""
+        B = dense.shape[0]
+        x = torch.cat([dense, deep.reshape(B, -1)], 1)
+        for layer in self.dnn:
+            x = torch.relu(layer(x))
+        dnn_logit = self.dnn_logit(x).squeeze(1)
+        linear_logit = wide.sum(1) + self.dense_linear(dense).squeeze(1)
+        return linear_logit + dnn_logit
+
+
 class DCNTower(torch.nn.Module):
     """dcn_model.py:53-95 without the embedding lookups: the same DNN[16, 4] and linear part as DeepFMTower, FM
     replaced by a CrossNet over x0 = [dense | deep] (deepctr's CrossNet, "vector" parameterization, DCN paper eq. 3:
@@ -98,7 +113,7 @@ class DCNTower(torch.nn.Module):
         return self.l2_reg * (self.cross_w * self.cross_w).sum()
 
 
-TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower}
+TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower, "wide_deep": WideDeepTower}
 
 
 def synthetic_batch(batch, seed, device, dist="zipf", zipf_s=1.05, group_rows=GROUP_ROWS):
@@ -209,7 +224,7 @@ def flat_order(tower):
 
 def flatten_tower(tower, flat):
     """Re-point the tower's parameters at views of one flat buffer laid out as
-    include/b200_deepfm.h documents: DeepFM [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w3], DCN
+    include/b200_deepfm.h documents: DeepFM and Wide & Deep [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w3], DCN
     [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w_out | w_0 w_1 | b_0 b_1]."""
     order = flat_order(tower)
     off, views = 0, []
@@ -309,6 +324,12 @@ def tower_calls(lib, model, tower):
             lib.b200_deepfm_dcn_tile_prologue if tile else None, lib.b200_deepfm_dcn_tile_main if tile else None,
             lib.b200_deepfm_dcn_forward_tile,
             lib.b200_deepfm_dcn_param_count, DEEPFM_DCN_SCRATCH, True),
+        "wide_deep": TowerCalls(
+            lib.b200_deepfm_wide_deep_fwd_bwd_tile if tile else None,
+            lib.b200_deepfm_wide_deep_tile_prologue if tile else None,
+            lib.b200_deepfm_wide_deep_tile_main if tile else None,
+            lib.b200_deepfm_wide_deep_forward_tile,
+            lib.b200_deepfm_param_count, DEEPFM_TILE_SCRATCH, False),
     }[model]
 
 
@@ -337,16 +358,18 @@ class DeepFMPSEngine:
         (b200_deepfm_rows_t) and step() launches no row pull; "pull": the rows of the unique ids are first
         pulled into bet_w / bet_d.  "auto" takes "table" where it applies: tile tower, one shard, direct
         exchange, tables not paired.
-        model="deepfm" (DeepFMTower) or "dcn" (DCNTower, the dac_ctr Deep & Cross Network: csrc/dcn_tower.cu);
-        the dedup, the rows, the push and the pipelines are the same for both.  "dcn" runs on tower="tile" or
-        "torch" and at most 38 id groups, and raises ValueError otherwise."""
+        model="deepfm" (DeepFMTower), "dcn" (DCNTower, the dac_ctr Deep & Cross Network: csrc/dcn_tower.cu) or
+        "wide_deep" (WideDeepTower, the dac_ctr Wide & Deep model: DeepFM without the FM term, on the tile tower's
+        kernel without it); the dedup, the rows, the push and the pipelines are the same for all three.  "dcn" and
+        "wide_deep" run on tower="tile" or "torch" and at most 38 id groups, and raise ValueError otherwise (the
+        fused and mma towers compute DeepFM only)."""
         assert tower in ("tile", "fused", "mma", "torch")
         if model not in TOWERS:
             raise ValueError("model must be one of %s, not %r" % (sorted(TOWERS), model))
-        if model == "dcn" and tower not in ("tile", "torch"):
-            raise ValueError('model="dcn" runs on tower="tile" or "torch", not %r' % tower)
-        if model == "dcn" and len(group_rows) > DEEPFM_TILE_MAXG:
-            raise ValueError('model="dcn" holds at most %d id groups, not %d' % (DEEPFM_TILE_MAXG, len(group_rows)))
+        if model != "deepfm" and tower not in ("tile", "torch"):
+            raise ValueError('model="%s" runs on tower="tile" or "torch", not %r' % (model, tower))
+        if model != "deepfm" and len(group_rows) > DEEPFM_TILE_MAXG:
+            raise ValueError('model="%s" holds at most %d id groups, not %d' % (model, DEEPFM_TILE_MAXG, len(group_rows)))
         self.model = model
         if tower == "tile" and len(group_rows) > DEEPFM_TILE_MAXG:
             tower = "fused"  # the tile tower holds at most 38 id groups in its shared-memory row

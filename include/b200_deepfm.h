@@ -105,6 +105,17 @@ int b200_deepfm_dcn_tile_prologue(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_dcn_tile_main(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_dcn_forward_tile(const b200_deepfm_args_t* args, void* stream);
 int64_t b200_deepfm_dcn_launch_count(void);
+/* The dac_ctr Wide & Deep model (model_zoo/dac_ctr/wide_deep_model.py:62-107): DeepFM without its FM term,
+ *   logit = sum(wide) + w_dense . dense + w3 . relu(W2 relu(W1 [dense | deep] + b1) + b2),
+ *   loss  = mean BCE with logits   (no regularization term).
+ * It has DeepFM's parameters: the DeepFM flat layout above and b200_deepfm_param_count.  Computed by the tile
+ * tower's kernel without the FM term (csrc/deepfm_tower2.cu), with the same arguments, outputs, `scratch` and
+ * refusals as the DeepFM tile entry points (at most 38 id groups; -1 and b200_deepfm_last_error); its launches
+ * are counted by b200_deepfm_tile_launch_count. */
+int b200_deepfm_wide_deep_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_wide_deep_tile_prologue(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_wide_deep_tile_main(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_wide_deep_forward_tile(const b200_deepfm_args_t* args, void* stream);
 /* Why the last call of any tower entry point (publish_loss included) that returned -1 (refused) or -2 (launch
  * error) failed; on the calling thread. */
 const char* b200_deepfm_last_error(void);

@@ -1,6 +1,7 @@
-"""DeepFM and DCN engine steps side by side: bench.py's workload (B = 32768, the 38 dac_ctr groups, Adam, its Zipf
-batches, narrow packed ids, the graphed lookahead pipeline) run for DeepFMPSEngine(model="deepfm") and
-DeepFMPSEngine(model="dcn"), alternating in one process over several repeats.
+"""DeepFM, DCN and Wide & Deep engine steps side by side: bench.py's workload (B = 32768, the 38 dac_ctr groups, Adam,
+its Zipf batches, narrow packed ids, the graphed lookahead pipeline) run for DeepFMPSEngine(model="deepfm"),
+DeepFMPSEngine(model="dcn") and DeepFMPSEngine(model="wide_deep"), alternating in one process over several repeats
+(the order rotates from repeat to repeat).
 
 Prints, per model, ms/step and samples/s of the graphed steps (median and spread over the repeats) and the
 tower's CUDA-event time (eager steps with event pairs, each step queued behind a spin kernel as bench.py does),
@@ -52,7 +53,7 @@ def main():
 
     dev = torch.device("cuda", 0)
     B = args.batch
-    models = ("deepfm", "dcn")
+    models = ("deepfm", "dcn", "wide_deep")
     groups, engines, devb, devp = {}, {}, {}, {}
     for m in models:
         groups[m] = PSGroup(1, "Adam", ADAM_ARGS, device=0)
@@ -82,7 +83,7 @@ def main():
     ms = {m: [] for m in models}
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for r in range(args.repeats):
-        for m in (models if r % 2 == 0 else models[::-1]):
+        for m in models[r % len(models):] + models[:r % len(models)]:
             eng = engines[m]
             for _ in range(args.warmup):
                 pos[m] += 1
@@ -103,7 +104,7 @@ def main():
         result["models"][m] = {"ms_per_step": med, "ms_min": min(ms[m]), "ms_max": max(ms[m]),
                                "samples_per_s": B / (med * 1e-3), "tower_ms": tower_ms[m],
                                "final_loss": engines[m].loss_host(engines[m].steps - 1)}
-        print("%-6s  %.4f ms/step (min %.4f, max %.4f over %d repeats)  %.3g samples/s  tower %.4f ms" % (
+        print("%-9s  %.4f ms/step (min %.4f, max %.4f over %d repeats)  %.3g samples/s  tower %.4f ms" % (
             m, med, min(ms[m]), max(ms[m]), args.repeats, B / (med * 1e-3), tower_ms[m]))
     print("card: %s, power limit %s, max SM clock %s" % (info["name"], info.get("power_limit"), info.get("max_sm_clock")))
     for g in groups.values():
