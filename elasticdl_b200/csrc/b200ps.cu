@@ -1723,11 +1723,16 @@ static int dim_class(int dim, const void* a, const void* b) {
 int b200ps_segment_sum(b200ps_t* ps, const float* values_dev, const int32_t* inv_dev, int T, int64_t k, int dim,
                        float* out_dev, void* stream) {
   if (T < 1 || T > 65535 || k < 1 || dim < 1) return fail(B200PS_EINVAL, "bad segment_sum shape");
+  int c = dim_class(dim, values_dev, out_dev);
+  int W = c == 0 ? 1 : 4 * c;
+  // the kernel's 32-bit warp key is row * chunks + chunk (a 64-bit one made the dim-1 sum of a DeepFM batch 17 %
+  // slower): refuse what would wrap it
+  if (k * (dim / W) > INT32_MAX)
+    return fail(B200PS_EINVAL, "segment_sum: k * (dim / " + std::to_string(W) + ") = " + std::to_string(k * (dim / W)) +
+                                   " work items per segment, more than INT32_MAX (2147483647)");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_OK(cudaMemsetAsync(out_dev, 0, (size_t)T * k * dim * sizeof(float), st));
-  int c = dim_class(dim, values_dev, out_dev);
-  int W = c == 0 ? 1 : 4 * c;
   dim3 grid(grid_for(ps, k * (dim / W)), T);
   if (c == 2) k_segment_sum<2><<<grid, 256, 0, st>>>(values_dev, inv_dev, k, dim, out_dev);
   else if (c == 1) k_segment_sum<1><<<grid, 256, 0, st>>>(values_dev, inv_dev, k, dim, out_dev);

@@ -715,6 +715,7 @@ __global__ void __launch_bounds__(256) k_segment_sum(const float* values, const 
 #pragma unroll
       for (int e = 0; e < W; ++e) x[e] = 0.f;
     }
+    // dst * chunks + c < k * chunks <= INT32_MAX (b200ps_segment_sum refuses more): no live key wraps onto another
     const int key = live ? dst * chunks + c : -1 - (int)(threadIdx.x & 31);
     const unsigned peers = __match_any_sync(0xffffffffu, key);
     const int lane = threadIdx.x & 31;

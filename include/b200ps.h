@@ -299,7 +299,9 @@ size_t b200ps_packed_ids_bytes(const int32_t* widths, int T, int64_t k);
 int b200ps_debug_buffer(void* dev_ptr, size_t bytes);
 /* deduplicate_indexed_slices' sum (tensor_utils.py:39-60) / gather backward:
  * out[t][inv[t][i], :] += values[t][i, :] with warp-level id dedup; out is
- * zeroed first for rows < k. */
+ * zeroed first for rows < k.  Refuses k * (dim / W) > INT32_MAX work items per
+ * segment (W = 8 / 4 floats for 16 B aligned pointers and dim % 8 / % 4 == 0,
+ * else 1). */
 int b200ps_segment_sum(b200ps_t* ps, const float* values_dev, const int32_t* inv_dev, int T, int64_t k,
                        int dim, float* out_dev, void* stream);
 /* forward of the layer's gather: out[t][i,:] = bet[t][inv[t][i], :]. */
