@@ -161,6 +161,13 @@ SYMBOLS = {
     "b200_deepfm_wide_deep_tile_prologue": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
     "b200_deepfm_wide_deep_tile_main": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
     "b200_deepfm_wide_deep_forward_tile": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_xdeepfm_param_count": (_sz, [_i]),
+    "b200_deepfm_xdeepfm_scratch_floats": (_sz, [_i, _i]),
+    "b200_deepfm_xdeepfm_fwd_bwd_tile": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_xdeepfm_tile_prologue": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_xdeepfm_tile_main": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_xdeepfm_forward_tile": (_i, [ctypes.POINTER(DeepFMArgs), _vp]),
+    "b200_deepfm_xdeepfm_launch_count": (_i64, []),
     # include/b200_features.h
     "b200feat_last_error": (ctypes.c_char_p, []),
     "b200feat_transform": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i64, _vp, _i, _vp, _vp]),

@@ -1,5 +1,6 @@
 // DeepFM tower, tile version (include/b200_deepfm.h: b200_deepfm_fwd_bwd_tile / b200_deepfm_forward_tile), and the
-// Wide & Deep tower (b200_deepfm_wide_deep_*) as its instances without the FM term (k_tower_tile<..., FM = false>).
+// Wide & Deep tower (b200_deepfm_wide_deep_*) as its instances without the FM term (k_tower_tile<..., FM = false>), and
+// xDeepFM's Wide & Deep part (b200_deepfm_xdeepfm_*, k_tower_tile<..., FM = false, CIN = true>).
 //
 // Round 1's tower gathered every embedding row three times (forward, backward, parameter-gradient
 // kernel) with one dependent global gather chain per lane at low occupancy, most of the
@@ -25,7 +26,7 @@
 // with straight 16-byte copies.  fp32 SIMT: the step has 1 GFLOP of first-layer work, and the kernel waits on
 // the gather round trip and on its per-tile phases and barriers, not on FMA throughput (DESIGN.md section 10:
 // a 3xTF32 mma.sync version of F / B1 / B2 measured slower).
-#include "tile_tower.cuh"
+#include "xdeepfm.cuh"
 
 namespace {
 
@@ -68,7 +69,9 @@ __global__ void __launch_bounds__(256) k_tile_prep(b200_deepfm_args_t a, int n_p
 
 // FM = false is the Wide & Deep model (b200_deepfm_wide_deep_*): DeepFM without its FM term, so F does not sum the
 // FM partials (their records stay 0), the tail gets zero FM sums and B1's row gradient is the DNN's alone.
-template <bool BACKWARD, bool TABLE, bool FM>
+// CIN (with FM = false) is xDeepFM: the CIN forward (xdeepfm_cin.cu) left each sample's CIN logit in the scratch
+// buffer, the tail adds it to z, and training stores dz there for the CIN's backward.
+template <bool BACKWARD, bool TABLE, bool FM, bool CIN = false>
 __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a, const float* __restrict__ w1x_g,
                                                            const __grid_constant__ TileRows rows) {
   extern __shared__ __align__(16) float smem[];
@@ -182,7 +185,8 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
     for (int d = 0; d < D; ++d) sd[d] = FM ? T[(H1 + d) * TS + lane] : 0.f;
     const float q = FM ? T[(H1 + D) * TS + lane] : 0.f, lin = T[(H1 + D + 1) * TS + lane];
     float a1[H1], h2[H2];
-    const float z = forward_tail(hpre, sd, q, lin, s_w2, s_b2, s_w3, a1, h2);  // FM = false: lin + w3 . h2
+    float z = forward_tail(hpre, sd, q, lin, s_w2, s_b2, s_w3, a1, h2);  // FM = false: lin + w3 . h2
+    if constexpr (CIN) z += a.scratch[cin_scratch(G, B).o_logit + (live ? b0 + lane : B - 1)];
     if (warp == 0 && live && a.logits != nullptr) a.logits[b0 + lane] = z;
     float dz = 0.f, dh1[H1];
     if (BACKWARD) {
@@ -195,6 +199,9 @@ __global__ void __launch_bounds__(THREADS, 2) k_tower_tile(b200_deepfm_args_t a,
       if (warp == 0 && live) loss_acc += lb;
       const float pr = 1.f / (1.f + expf(-z));
       dz = live ? (pr - y) / (float)B : 0.f;
+      if constexpr (CIN) {
+        if (warp == 0 && live) a.scratch[cin_scratch(G, B).o_dz + b0 + lane] = dz;
+      }
       float dh2[H2];
 #pragma unroll
       for (int k = 0; k < H2; ++k) dh2[k] = h2[k] > 0.f ? dz * s_w3[k] : 0.f;
@@ -340,6 +347,18 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
 }
 
 }  // namespace
+
+namespace deepfm {
+
+template <bool BACKWARD>
+int launch_xdeepfm_tile(const b200_deepfm_args_t* args, void* stream, int what, long long& launches) {
+  return launch_tile_tower<BACKWARD, k_tower_tile<BACKWARD, false, false, true>, k_tower_tile<true, true, false, true>>(
+      args, stream, what, SMEM_BYTES, prep, launches);
+}
+template int launch_xdeepfm_tile<true>(const b200_deepfm_args_t*, void*, int, long long&);
+template int launch_xdeepfm_tile<false>(const b200_deepfm_args_t*, void*, int, long long&);
+
+}  // namespace deepfm
 
 extern "C" {
 

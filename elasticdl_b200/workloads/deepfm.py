@@ -113,7 +113,54 @@ class DCNTower(torch.nn.Module):
         return self.l2_reg * (self.cross_w * self.cross_w).sum()
 
 
-TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower, "wide_deep": WideDeepTower}
+class XDeepFMTower(WideDeepTower):
+    """xdeepfm_model.py:55-107 without the embedding lookups: WideDeepTower (its parameters under the same names)
+    plus a Compressed Interaction Network over the deep rows X0 = deep [B, G, D] (deepctr's CIN with
+    layer_size=(128, 128), activation="relu", split_half=True) and its Dense(1) over the 192 pooled channels:
+        Z_k[b, d, i H_k + j] = X0[b, i, d] X_k[b, j, d],   C_k = relu(W_k Z_k + b_k)   [B, 128, D],
+        X_1 = C_0[:, :64],  p = [C_0[:, 64:] | C_1].sum(d),  logit = Wide & Deep + exfm(p).
+    Filters glorot-uniform over (K, 128), biases zero.  regularization() is the filters' l2 term.  Needs G >= 2: with
+    one field the reference builds a different model (no CIN)."""
+
+    def __init__(self, n_groups=N_GROUPS, deep_dim=DEEP_DIM, n_dense=N_DENSE, hidden=(16, 4), layer_size=(128, 128),
+                 l2_reg=1e-5):
+        super().__init__(n_groups, deep_dim, n_dense, hidden)
+        self.l2_reg = l2_reg
+        h0, h1 = layer_size
+        k0, k1 = n_groups * n_groups, n_groups * (h0 // 2)
+
+        def glorot(rows, cols):
+            lim = math.sqrt(6.0 / (rows + cols))
+            return torch.nn.Parameter(torch.empty(rows, cols).uniform_(-lim, lim))
+
+        self.cin_w0, self.cin_b0 = glorot(h0, k0), torch.nn.Parameter(torch.zeros(h0))
+        self.cin_w1, self.cin_b1 = glorot(h1, k1), torch.nn.Parameter(torch.zeros(h1))
+        self.exfm = torch.nn.Linear(h0 // 2 + h1, 1)
+        with torch.no_grad():
+            self.exfm.weight.copy_(glorot(1, h0 // 2 + h1))
+            self.exfm.bias.zero_()
+
+    def cin(self, deep):
+        """deep [B, G, D] -> p [B, 192]."""
+        B, G, D = deep.shape
+        x, direct = deep, []
+        for k, (w, b) in enumerate(((self.cin_w0, self.cin_b0), (self.cin_w1, self.cin_b1))):
+            z = torch.einsum("bid,bjd->bdij", deep, x).reshape(B, D, G * x.shape[1])
+            c = torch.relu(torch.matmul(z, w.t()) + b).transpose(1, 2)  # [B, 128, D]
+            if k == 0:
+                x, c = c[:, :c.shape[1] // 2], c[:, c.shape[1] // 2:]
+            direct.append(c)
+        return torch.cat(direct, 1).sum(2)
+
+    def forward(self, dense, wide, deep):
+        """dense [B,13], wide [B,G], deep [B,G,D] -> logits [B]."""
+        return super().forward(dense, wide, deep) + self.exfm(self.cin(deep)).squeeze(1)
+
+    def regularization(self):
+        return self.l2_reg * ((self.cin_w0 * self.cin_w0).sum() + (self.cin_w1 * self.cin_w1).sum())
+
+
+TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower, "wide_deep": WideDeepTower, "xdeepfm": XDeepFMTower}
 
 
 def synthetic_batch(batch, seed, device, dist="zipf", zipf_s=1.05, group_rows=GROUP_ROWS):
@@ -219,13 +266,18 @@ def flat_order(tower):
              (tower.dnn[1].weight, None), (tower.dnn[1].bias, None)]
     if isinstance(tower, DCNTower):
         return order + [(tower.out.weight, None), (tower.cross_w, None), (tower.cross_b, None)]
-    return order + [(tower.dnn_logit.weight, None)]
+    order.append((tower.dnn_logit.weight, None))
+    if isinstance(tower, XDeepFMTower):
+        order += [(tower.cin_w0, None), (tower.cin_b0, None), (tower.cin_w1, None), (tower.cin_b1, None),
+                  (tower.exfm.weight, None), (tower.exfm.bias, None)]
+    return order
 
 
 def flatten_tower(tower, flat):
     """Re-point the tower's parameters at views of one flat buffer laid out as
     include/b200_deepfm.h documents: DeepFM and Wide & Deep [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w3], DCN
-    [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w_out | w_0 w_1 | b_0 b_1]."""
+    [w_dense 13 (+3 pad) | w1 | b1 | w2 | b2 | w_out | w_0 w_1 | b_0 b_1], xDeepFM Wide & Deep's then
+    [W_0 | b_0 | W_1 | b_1 | w_ex | b_ex]."""
     order = flat_order(tower)
     off, views = 0, []
     with torch.no_grad():
@@ -305,8 +357,8 @@ def _tower_error(lib):
 
 # What DeepFMPSEngine calls for its model on its tower kind (tower_calls): fwd_bwd, the one-call training step (None
 # on tower="torch"); prologue / main, the tile tower's training step split in two (None elsewhere); forward,
-# predict()'s tower; param_count(G), the flat parameter count; scratch, the floats the tile tower needs of `scratch`;
-# regularized, whether the torch loss adds tower.regularization().
+# predict()'s tower; param_count(G), the flat parameter count; scratch(G, B), the floats the tile tower needs of
+# `scratch`; regularized, whether the torch loss adds tower.regularization().
 TowerCalls = collections.namedtuple("TowerCalls", "fwd_bwd prologue main forward param_count scratch regularized")
 
 
@@ -318,18 +370,24 @@ def tower_calls(lib, model, tower):
              "mma": lib.b200_deepfm_fwd_bwd_mma}.get(tower),
             lib.b200_deepfm_tile_prologue if tile else None, lib.b200_deepfm_tile_main if tile else None,
             lib.b200_deepfm_forward_tile if tile else lib.b200_deepfm_forward,
-            lib.b200_deepfm_param_count, DEEPFM_TILE_SCRATCH, False),
+            lib.b200_deepfm_param_count, lambda G, B: DEEPFM_TILE_SCRATCH, False),
         "dcn": TowerCalls(
             lib.b200_deepfm_dcn_fwd_bwd_tile if tile else None,
             lib.b200_deepfm_dcn_tile_prologue if tile else None, lib.b200_deepfm_dcn_tile_main if tile else None,
             lib.b200_deepfm_dcn_forward_tile,
-            lib.b200_deepfm_dcn_param_count, DEEPFM_DCN_SCRATCH, True),
+            lib.b200_deepfm_dcn_param_count, lambda G, B: DEEPFM_DCN_SCRATCH, True),
         "wide_deep": TowerCalls(
             lib.b200_deepfm_wide_deep_fwd_bwd_tile if tile else None,
             lib.b200_deepfm_wide_deep_tile_prologue if tile else None,
             lib.b200_deepfm_wide_deep_tile_main if tile else None,
             lib.b200_deepfm_wide_deep_forward_tile,
-            lib.b200_deepfm_param_count, DEEPFM_TILE_SCRATCH, False),
+            lib.b200_deepfm_param_count, lambda G, B: DEEPFM_TILE_SCRATCH, False),
+        "xdeepfm": TowerCalls(
+            lib.b200_deepfm_xdeepfm_fwd_bwd_tile if tile else None,
+            lib.b200_deepfm_xdeepfm_tile_prologue if tile else None,
+            lib.b200_deepfm_xdeepfm_tile_main if tile else None,
+            lib.b200_deepfm_xdeepfm_forward_tile,
+            lib.b200_deepfm_xdeepfm_param_count, lib.b200_deepfm_xdeepfm_scratch_floats, True),
     }[model]
 
 
@@ -360,9 +418,10 @@ class DeepFMPSEngine:
         exchange, tables not paired.
         model="deepfm" (DeepFMTower), "dcn" (DCNTower, the dac_ctr Deep & Cross Network: csrc/dcn_tower.cu) or
         "wide_deep" (WideDeepTower, the dac_ctr Wide & Deep model: DeepFM without the FM term, on the tile tower's
-        kernel without it); the dedup, the rows, the push and the pipelines are the same for all three.  "dcn" and
-        "wide_deep" run on tower="tile" or "torch" and at most 38 id groups, and raise ValueError otherwise (the
-        fused and mma towers compute DeepFM only)."""
+        kernel without it) or "xdeepfm" (XDeepFMTower, the model the dac_ctr training script runs: Wide & Deep plus
+        a CIN, csrc/xdeepfm_cin.cu); the dedup, the rows, the push and the pipelines are the same for all four.
+        The models other than "deepfm" run on tower="tile" or "torch" and at most 38 id groups, "xdeepfm" on at
+        least 2, and raise ValueError otherwise (the fused and mma towers compute DeepFM only)."""
         assert tower in ("tile", "fused", "mma", "torch")
         if model not in TOWERS:
             raise ValueError("model must be one of %s, not %r" % (sorted(TOWERS), model))
@@ -370,6 +429,9 @@ class DeepFMPSEngine:
             raise ValueError('model="%s" runs on tower="tile" or "torch", not %r' % (model, tower))
         if model != "deepfm" and len(group_rows) > DEEPFM_TILE_MAXG:
             raise ValueError('model="%s" holds at most %d id groups, not %d' % (model, DEEPFM_TILE_MAXG, len(group_rows)))
+        if model == "xdeepfm" and len(group_rows) < 2:
+            raise ValueError('model="xdeepfm" needs at least 2 id groups (its CIN crosses fields), not %d'
+                             % len(group_rows))
         self.model = model
         if tower == "tile" and len(group_rows) > DEEPFM_TILE_MAXG:
             tower = "fused"  # the tile tower holds at most 38 id groups in its shared-memory row
@@ -468,7 +530,7 @@ class DeepFMPSEngine:
         self.gsum_w = torch.zeros((G * B, 1), **f32)
         self.gsum_d = torch.zeros((G * B, D), **f32)
         # b200_deepfm.h: backward state + W1^T (fused / mma) | the tile tower's
-        self.scratch = torch.empty(max(B * 44 + 16 * (N_DENSE + D * G), self.calls.scratch), **f32)
+        self.scratch = torch.empty(max(B * 44 + 16 * (N_DENSE + D * G), self.calls.scratch(G, B)), **f32)
         self.loss_buf = torch.zeros(1, **f32)
         # the loss of every step also lands in a ring of pinned host memory, written by a 1-thread kernel at the end
         # of the step (b200_deepfm_publish_loss): loss_host(k) reads step k's value after a synchronize, no D2H copy

@@ -116,6 +116,29 @@ int b200_deepfm_wide_deep_fwd_bwd_tile(const b200_deepfm_args_t* args, void* str
 int b200_deepfm_wide_deep_tile_prologue(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_wide_deep_tile_main(const b200_deepfm_args_t* args, void* stream);
 int b200_deepfm_wide_deep_forward_tile(const b200_deepfm_args_t* args, void* stream);
+/* The dac_ctr xDeepFM model (model_zoo/dac_ctr/xdeepfm_model.py:55-107): Wide & Deep plus a Compressed Interaction
+ * Network over the deep rows X0 = [G fields x 8] (layer_size (128, 128), relu, split_half, l2_reg 1e-5):
+ *   Z_k[b, d, i H_k + j] = X0[b, i, d] X_k[b, j, d]   (H_0 = G, H_1 = 64),
+ *   C_k[b, h, d] = relu(sum_K W_k[h, K] Z_k[b, d, K] + b_k[h]),  X_1 = C_0 channels 0..63,
+ *   p = sum_d [C_0 channels 64..127 | C_1]  (192),
+ *   logit = (the Wide & Deep logit) + w_ex . p + b_ex,
+ *   loss  = mean BCE with logits + 1e-5 (|W_0|^2 + |W_1|^2)   (the gradients include 2e-5 W_k).
+ * Parameter / gradient layout (floats): the DeepFM / Wide & Deep layout above, then
+ *   [ W_0 128 x G^2 | b_0 128 | W_1 128 x 64G | b_1 128 | w_ex 192 | b_ex 1 ]
+ * filter row h contiguous over K = i H_k + j (501,753 floats at G = 38, 496,577 of them the CIN's).
+ * Computed by csrc/xdeepfm_cin.cu (the CIN, 3xTF32 mma.sync) and the Wide & Deep tile kernel with the CIN logit
+ * (csrc/deepfm_tower2.cu), with the DeepFM tile entry points' arguments and outputs; `scratch` needs
+ * b200_deepfm_xdeepfm_scratch_floats(G, B) floats (about 170 MB at G = 38, B = 32768).  The prologue reads only
+ * `params` and `n_unique`.  Refused (-1, b200_deepfm_last_error, nothing launched): G < 2 (with one field the
+ * model has no CIN), G > 38, a row source on the forward-only entry, a null scratch.  Its launches, the tile
+ * kernel's included, are counted by b200_deepfm_xdeepfm_launch_count. */
+size_t b200_deepfm_xdeepfm_param_count(int G);
+size_t b200_deepfm_xdeepfm_scratch_floats(int G, int B);
+int b200_deepfm_xdeepfm_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_xdeepfm_tile_prologue(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_xdeepfm_tile_main(const b200_deepfm_args_t* args, void* stream);
+int b200_deepfm_xdeepfm_forward_tile(const b200_deepfm_args_t* args, void* stream);
+int64_t b200_deepfm_xdeepfm_launch_count(void);
 /* Why the last call of any tower entry point (publish_loss included) that returned -1 (refused) or -2 (launch
  * error) failed; on the calling thread. */
 const char* b200_deepfm_last_error(void);

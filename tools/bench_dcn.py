@@ -1,11 +1,13 @@
-"""DeepFM, DCN and Wide & Deep engine steps side by side: bench.py's workload (B = 32768, the 38 dac_ctr groups, Adam,
-its Zipf batches, narrow packed ids, the graphed lookahead pipeline) run for DeepFMPSEngine(model="deepfm"),
-DeepFMPSEngine(model="dcn") and DeepFMPSEngine(model="wide_deep"), alternating in one process over several repeats
-(the order rotates from repeat to repeat).
+"""DeepFM, DCN, Wide & Deep and xDeepFM engine steps side by side: bench.py's workload (B = 32768, the 38 dac_ctr
+groups, Adam, its Zipf batches, narrow packed ids, the graphed lookahead pipeline) run for DeepFMPSEngine(model=m),
+m in MODELS, alternating in one process over several repeats (the order rotates from repeat to repeat).
 
 Prints, per model, ms/step and samples/s of the graphed steps (median and spread over the repeats) and the
 tower's CUDA-event time (eager steps with event pairs, each step queued behind a spin kernel as bench.py does),
-plus the card's name and power limit read in the same run.  One JSON line at the end.
+plus the card's name and power limit read in the same run.  For xDeepFM also the CIN's algorithmic rate,
+2 x 128 x 8 x (G^2 + 64 G) x 3 x B FLOP (forward, data and weight passes) over the tower's event time, the 3xTF32
+tensor rate that implies (three TF32 products per fp32 product) against the 495 TF/s dense TF32 data-sheet peak,
+and the same steps on tower="torch" (eager, same batches).  One JSON line at the end.
 
     python tools/bench_dcn.py [--steps 50] [--warmup 10] [--repeats 5] [--pool 8]
 """
@@ -19,6 +21,15 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+
+MODELS = ("deepfm", "dcn", "wide_deep", "xdeepfm")
+TF32_PEAK = 495e12  # H100 SXM data sheet, dense TF32
+
+
+def cin_flop(G, B):
+    """The CIN's algorithmic FLOP of one training step: three contractions of 2 x 128 x 8 x (G^2 + 64 G) per sample."""
+    return 2 * 128 * 8 * (G * G + 64 * G) * 3 * B
 
 
 def card():
@@ -53,7 +64,7 @@ def main():
 
     dev = torch.device("cuda", 0)
     B = args.batch
-    models = ("deepfm", "dcn", "wide_deep")
+    models = MODELS
     groups, engines, devb, devp = {}, {}, {}, {}
     for m in models:
         groups[m] = PSGroup(1, "Adam", ADAM_ARGS, device=0)
@@ -74,6 +85,23 @@ def main():
         torch.cuda.synchronize(dev)
         groups[m].check()
         tower_ms[m] = eng.kernel_report(ev, [1])["tower_fwd_bwd"]["ms"]
+
+    # xDeepFM on the torch tower, eager, same batches: the tile tower's step must beat it
+    tg = PSGroup(1, "Adam", ADAM_ARGS, device=0)
+    te = DeepFMPSEngine(tg, B, id_transport="narrow", model="xdeepfm", tower="torch")
+    for i in range(2):
+        te.step(*devb["xdeepfm"][i % args.pool])
+    torch.cuda.synchronize(dev)
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    n_torch = max(3, args.steps // 10)
+    for i in range(n_torch):
+        te.step(*devb["xdeepfm"][i % args.pool])
+    t1.record()
+    torch.cuda.synchronize(dev)
+    torch_ms = t0.elapsed_time(t1) / n_torch
+    tg.check()
+    tg.close()
 
     # the graphed lookahead step, the models alternating repeat by repeat
     for m in models:
@@ -107,6 +135,14 @@ def main():
         print("%-9s  %.4f ms/step (min %.4f, max %.4f over %d repeats)  %.3g samples/s  tower %.4f ms" % (
             m, med, min(ms[m]), max(ms[m]), args.repeats, B / (med * 1e-3), tower_ms[m]))
     print("card: %s, power limit %s, max SM clock %s" % (info["name"], info.get("power_limit"), info.get("max_sm_clock")))
+    G = engines["xdeepfm"].G
+    rate = cin_flop(G, B) / (tower_ms["xdeepfm"] * 1e-3)
+    x = result["models"]["xdeepfm"]
+    x.update({"torch_tower_ms_per_step": torch_ms, "cin_tflops": rate / 1e12, "tf32_tensor_tflops": 3 * rate / 1e12,
+              "tf32_share_of_peak": 3 * rate / TF32_PEAK})
+    print("xdeepfm CIN: %.1f GFLOP per step, %.1f TFLOP/s algorithmic over the tower time, %.1f TFLOP/s of TF32 "
+          "products = %.1f%% of the 495 TF/s data-sheet peak; tower=\"torch\" eager step %.3f ms" % (
+              cin_flop(G, B) / 1e9, rate / 1e12, 3 * rate / 1e12, 100 * 3 * rate / TF32_PEAK, torch_ms))
     for g in groups.values():
         g.close()
     print(json.dumps(result))
