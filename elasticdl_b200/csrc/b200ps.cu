@@ -1758,6 +1758,97 @@ int b200ps_gather_rows(b200ps_t* ps, const float* bet_dev, const int32_t* inv_de
   return B200PS_OK;
 }
 
+// ---- pooled lookup of sparse input --------------------------------------------
+
+static int sparse_shape(int64_t B, int64_t nnz, int dim, const void* ws, size_t ws_bytes) {
+  if (B < 1 || nnz < 0 || dim < 1) return fail(B200PS_EINVAL, "sparse lookup: bad shape (B >= 1, nnz >= 0, dim >= 1)");
+  if (nnz + B > INT32_MAX)
+    return fail(B200PS_EINVAL, "sparse lookup: nnz + B = " + std::to_string(nnz + B) + " filled entries, more than INT32_MAX");
+  if (!ws || ((uintptr_t)ws & 15u)) return fail(B200PS_EINVAL, "sparse lookup: workspace null or not 16 B aligned");
+  if (ws_bytes < b200ps_sparse_workspace(B, nnz, dim))
+    return fail(B200PS_EINVAL, "sparse lookup: workspace smaller than b200ps_sparse_workspace(B, nnz, dim)");
+  return B200PS_OK;
+}
+
+size_t b200ps_sparse_workspace(int64_t B, int64_t nnz, int dim) {
+  if (B < 1 || nnz < 0 || dim < 1) return 0;
+  return (size_t)SparseLayout(B, nnz, dim).words * sizeof(int);
+}
+
+int b200ps_sparse_prep(b200ps_t* ps, const int64_t* rows_dev, const void* vals_dev, int vals_are_int32, int64_t B,
+                       int64_t nnz, int dim, int64_t* ids_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
+  if (!ids_dev || (nnz > 0 && (!rows_dev || !vals_dev))) return fail(B200PS_EINVAL, "sparse_prep: null pointer");
+  DeviceGuard g(client_dev(ps));
+  cudaStream_t st = (cudaStream_t)stream;
+  const SparseLayout L(B, nnz, dim);
+  int* w = (int*)ws;
+  CUDA_OK(cudaMemsetAsync(w, 0, (size_t)L.off * sizeof(int), st));  // bad count and cnt
+  const int gc = grid_for(ps, L.NT * 256), gs = grid_for(ps, L.K);
+  long long* ids = (long long*)ids_dev;
+  const long long* rows = (const long long*)rows_dev;
+  if (vals_are_int32) {
+    const int* v = (const int*)vals_dev;
+    k_sparse_count<<<gc, 256, 0, st>>>(rows, v, L, w);
+    k_sparse_scan<<<1, kSpScanThreads, 0, st>>>(v, L, w);
+    k_sparse_scatter<<<gs, 256, 0, st>>>(rows, v, L, w, ids);
+  } else {
+    const long long* v = (const long long*)vals_dev;
+    k_sparse_count<<<gc, 256, 0, st>>>(rows, v, L, w);
+    k_sparse_scan<<<1, kSpScanThreads, 0, st>>>(v, L, w);
+    k_sparse_scatter<<<gs, 256, 0, st>>>(rows, v, L, w, ids);
+  }
+  count_launch(ps, 3);
+  CUDA_OK(cudaGetLastError());
+  return B200PS_OK;
+}
+
+int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, void* ws, size_t ws_bytes,
+                          int64_t B, int64_t nnz, int dim, int combiner, float* out_dev, void* stream) {
+  if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
+  if (combiner < kSpSum || combiner > kSpSqrtn) return fail(B200PS_EINVAL, "sparse_combine: combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+  if (!bet_dev || !inv_dev || !out_dev) return fail(B200PS_EINVAL, "sparse_combine: null pointer");
+  DeviceGuard g(client_dev(ps));
+  cudaStream_t st = (cudaStream_t)stream;
+  const SparseLayout L(B, nnz, dim);
+  const int c = dim_class(dim, bet_dev, out_dev);
+  const int grid = grid_for(ps, L.PB * 32);
+  int* w = (int*)ws;
+  if (c == 2) k_sparse_combine<2><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
+  else if (c == 1) k_sparse_combine<1><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
+  else k_sparse_combine<0><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
+  count_launch(ps, 1);
+  CUDA_OK(cudaGetLastError());
+  return B200PS_OK;
+}
+
+int b200ps_sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev, const void* ws,
+                               size_t ws_bytes, int64_t B, int64_t nnz, int dim, int combiner, int64_t n_unique,
+                               float* gbet_dev, void* stream) {
+  if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
+  if (combiner < kSpSum || combiner > kSpSqrtn)
+    return fail(B200PS_EINVAL, "sparse_combine_grad: combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+  if (n_unique < 1 || n_unique > nnz + B) return fail(B200PS_EINVAL, "sparse_combine_grad: n_unique outside [1, nnz + B]");
+  if (!gout_dev || !inv_dev || !gbet_dev) return fail(B200PS_EINVAL, "sparse_combine_grad: null pointer");
+  const SparseLayout L(B, nnz, dim);
+  const int c = dim_class(dim, gout_dev, gbet_dev);
+  const int W = c == 0 ? 1 : 4 * c;
+  if (L.K * (dim / W) > INT32_MAX)  // segment_sum_loop's 32-bit warp key, as in b200ps_segment_sum
+    return fail(B200PS_EINVAL, "sparse_combine_grad: (nnz + B) * (dim / " + std::to_string(W) + ") = " +
+                                   std::to_string(L.K * (dim / W)) + " work items, more than INT32_MAX (2147483647)");
+  DeviceGuard g(client_dev(ps));
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_OK(cudaMemsetAsync(gbet_dev, 0, (size_t)n_unique * dim * sizeof(float), st));
+  const int grid = grid_for(ps, L.K * (dim / W));
+  const int* w = (const int*)ws;
+  if (c == 2) k_sparse_combine_grad<2><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
+  else if (c == 1) k_sparse_combine_grad<1><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
+  else k_sparse_combine_grad<0><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
+  count_launch(ps, 1);
+  CUDA_OK(cudaGetLastError());
+  return B200PS_OK;
+}
+
 // ---- state ---------------------------------------------------------------------
 
 int b200ps_shard_state(b200ps_t* ps, int shard, int32_t* version, int64_t* step, int32_t* initialized) {

@@ -687,30 +687,39 @@ __global__ void __launch_bounds__(256) k_present_ids(const uint32_t* present, lo
 // same output row combine through shuffles (lane order) and the lowest lane
 // issues ONE vector reduction to global memory.
 // ---------------------------------------------------------------------------
+// The row source of a segment sum: LOAD.live(row) says whether entry `row` contributes, LOAD.load(row, c, x) reads
+// its W floats of chunk c.
 template <int VPT>
-__global__ void __launch_bounds__(256) k_segment_sum(const float* values, const int* inv, long long k, int dim,
-                                                     float* out) {
+struct RowsLoad {  // values[row, :]
+  const float* V;
+  int dim;
+  __device__ __forceinline__ bool live(long long) const { return true; }
+  __device__ __forceinline__ void load(long long row, int c, float* x) const {
+    constexpr int W = VPT == 0 ? 1 : 4 * VPT;
+    if (VPT == 0) x[0] = V[row * dim + c];
+    else {
+#pragma unroll
+      for (int v = 0; v < VPT; ++v) *reinterpret_cast<float4*>(&x[4 * v]) = ld_f4(V + row * dim + c * W + 4 * v);
+    }
+  }
+};
+
+template <int VPT, class LOAD>
+__device__ __forceinline__ void segment_sum_loop(const LOAD& ld, const int* I, long long k, int dim, float* O) {
   constexpr int W = VPT == 0 ? 1 : 4 * VPT;
-  const int t = blockIdx.y;
   const int chunks = dim / W;
   const long long work = k * chunks;
   const long long stride = (long long)gridDim.x * blockDim.x;
-  const float* V = values + (long long)t * k * dim;
-  float* O = out + (long long)t * k * dim;
-  const int* I = inv + (long long)t * k;
   const long long wmax = (work + 31) / 32 * 32;  // keep warps converged for the shuffles
   for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < wmax; w += stride) {
-    const bool live = w < work;
-    const long long row = live ? (chunks == 1 ? w : w / chunks) : 0;
+    const bool in = w < work;
+    const long long row = in ? (chunks == 1 ? w : w / chunks) : 0;
+    const bool live = in && ld.live(row);
     const int c = live ? (int)(w - row * chunks) : 0;
     const int dst = live ? I[row] : -1;
     float x[W];
     if (live) {
-      if (VPT == 0) x[0] = V[row * dim + c];
-      else {
-#pragma unroll
-        for (int v = 0; v < VPT; ++v) *reinterpret_cast<float4*>(&x[4 * v]) = ld_f4(V + row * dim + c * W + 4 * v);
-      }
+      ld.load(row, c, x);
     } else {
 #pragma unroll
       for (int e = 0; e < W; ++e) x[e] = 0.f;
@@ -742,6 +751,14 @@ __global__ void __launch_bounds__(256) k_segment_sum(const float* values, const 
   }
 }
 
+template <int VPT>
+__global__ void __launch_bounds__(256) k_segment_sum(const float* values, const int* inv, long long k, int dim,
+                                                     float* out) {
+  const int t = blockIdx.y;
+  const RowsLoad<VPT> ld{values + (long long)t * k * dim, dim};
+  segment_sum_loop<VPT>(ld, inv + (long long)t * k, k, dim, out + (long long)t * k * dim);
+}
+
 // gather_rows: out[t][i, :] = bet[t][inv[i], :]  (tf.gather(batch_embedding, idx),
 // embedding_delegate.py:95)
 template <int VPT>
@@ -771,6 +788,364 @@ __global__ void __launch_bounds__(256) k_gather_rows(const float* bet, const int
 __global__ void __launch_bounds__(256) k_zero(float* p, long long n) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) p[i] = 0.f;
+}
+
+// ---------------------------------------------------------------------------
+// Pooled lookup of a sparse [B, L] input (safe_embedding_lookup_sparse without weights,
+// embedding_delegate.py:108-230): prune ids < 0, give each empty row the id 0, combine per row
+// (sum / mean / sqrtn), write 0 for the rows that were empty.
+//
+// Workspace (int32 words, offsets from SparseLayout; n = nnz, K = nnz + B filled entries):
+//   bad[4]      entries whose row lies outside [0, B) (dropped)
+//   cnt[B]      kept ids per row
+//   off[B+1]    CSR offsets of the filled stream, off[b] = sum_{r<b} max(cnt[r], 1)
+//   ebef[B]     empty rows before row b
+//   poff[B+1]   piece offsets: row b is combined in np_b = ceil(max(cnt, 1) / kSpPiece) pieces
+//   moff[B+1]   partial-sum slots of the rows with np_b > 1
+//   arrive[B]   pieces of row b that have finished (forward of a multi-piece row)
+//   prow[PB]    row of each piece
+//   tkept[NT], tbase[NT], tlast[NT]   per input tile: kept entries, kept entries before it, last kept index
+//   last[2]     the last filled id (int64), copied into the tail [off[B], K)
+//   rowf[K]     row of each filled entry, -1 for the fill of an empty row and for the tail
+//   part[MB*dim] float partial sums of multi-piece rows
+// ---------------------------------------------------------------------------
+constexpr int kSpPiece = 256;  // filled entries one warp sums before a row is split across warps
+constexpr int kSpTile = 1024;  // input entries per block and tile of the prep's count and scatter passes
+constexpr int kSpScanThreads = 1024;
+
+enum { kSpSum = 0, kSpMean = 1, kSpSqrtn = 2 };
+
+struct SparseLayout {
+  long long B, nnz, K, PB, MB, NT;
+  long long cnt, off, ebef, poff, moff, arrive, prow, tkept, tbase, tlast, last, rowf, part, words;
+  __host__ __device__ static long long up4(long long x) { return (x + 3) / 4 * 4; }
+  __host__ __device__ SparseLayout(long long B_, long long nnz_, int dim) : B(B_), nnz(nnz_) {
+    K = nnz + B;
+    PB = B + K / kSpPiece + 1;      // sum_b ceil(len_b / P) <= K / P + B
+    MB = 2 * (K / kSpPiece) + 1;    // a row with np > 1 has len > P, so np < 2 len / P
+    NT = (nnz + kSpTile - 1) / kSpTile;
+    cnt = 4;
+    off = up4(cnt + B);
+    ebef = up4(off + B + 1);
+    poff = up4(ebef + B);
+    moff = up4(poff + B + 1);
+    arrive = up4(moff + B + 1);
+    prow = up4(arrive + B);
+    tkept = up4(prow + PB);
+    tbase = up4(tkept + NT);
+    tlast = up4(tbase + NT);
+    last = up4(tlast + NT);
+    rowf = up4(last + 2);
+    part = up4(rowf + K);
+    words = up4(part + MB * (long long)dim);
+  }
+};
+
+__device__ __forceinline__ int sp_pieces(int cnt) { return ((cnt > 1 ? cnt : 1) + kSpPiece - 1) / kSpPiece; }
+
+// Pass 1: count kept ids per row (warp-aggregated atomics: a coalesced input is row-major), kept entries and the
+// last kept index per tile; report rows outside [0, B).
+template <typename V>
+__global__ void __launch_bounds__(256) k_sparse_count(const long long* rows, const V* vals, SparseLayout L, int* ws) {
+  int* cnt = ws + L.cnt;
+  __shared__ int s_kept, s_last;
+  const int lane = threadIdx.x & 31;
+  for (long long t = blockIdx.x; t < L.NT; t += gridDim.x) {
+    if (threadIdx.x == 0) { s_kept = 0; s_last = -1; }
+    __syncthreads();
+    int kept = 0, last = -1, bad = 0;
+    for (int q = 0; q < kSpTile / 256; ++q) {
+      const long long i = t * kSpTile + q * 256 + threadIdx.x;
+      long long r = -1;
+      bool keep = false;
+      if (i < L.nnz) {
+        r = rows[i];
+        const bool rok = r >= 0 && r < L.B;
+        bad += !rok;
+        keep = rok && (long long)vals[i] >= 0;
+      }
+      const unsigned km = __ballot_sync(0xffffffffu, keep);
+      const unsigned peers = __match_any_sync(0xffffffffu, keep ? r : -1LL) & km;
+      if (keep && (__ffs(peers) - 1) == lane) atomicAdd(cnt + r, __popc(peers));
+      kept += keep;
+      if (keep) last = (int)i;
+    }
+    kept = __reduce_add_sync(0xffffffffu, kept);
+    last = (int)__reduce_max_sync(0xffffffffu, (unsigned)(last + 1)) - 1;
+    bad = __reduce_add_sync(0xffffffffu, bad);
+    if (lane == 0) {
+      atomicAdd(&s_kept, kept);
+      atomicMax(&s_last, last);
+      if (bad) atomicAdd(ws, bad);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      ws[L.tkept + t] = s_kept;
+      ws[L.tlast + t] = s_last;
+    }
+    __syncthreads();
+  }
+}
+
+// Block-wide exclusive scan of int4 (one value per thread, kSpScanThreads threads) and the block total.
+struct SpScan {
+  int4 excl, tot;
+};
+__device__ __forceinline__ SpScan sp_block_scan(int4 v) {
+  __shared__ int4 s_w[kSpScanThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int4 x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int a = __shfl_up_sync(0xffffffffu, x.x, o), b = __shfl_up_sync(0xffffffffu, x.y, o);
+    const int c = __shfl_up_sync(0xffffffffu, x.z, o), d = __shfl_up_sync(0xffffffffu, x.w, o);
+    if (lane >= o) { x.x += a; x.y += b; x.z += c; x.w += d; }
+  }
+  if (lane == 31) s_w[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int4 y = lane < kSpScanThreads / 32 ? s_w[lane] : make_int4(0, 0, 0, 0);
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int a = __shfl_up_sync(0xffffffffu, y.x, o), b = __shfl_up_sync(0xffffffffu, y.y, o);
+      const int c = __shfl_up_sync(0xffffffffu, y.z, o), d = __shfl_up_sync(0xffffffffu, y.w, o);
+      if (lane >= o) { y.x += a; y.y += b; y.z += c; y.w += d; }
+    }
+    if (lane < kSpScanThreads / 32) s_w[lane] = y;  // inclusive warp totals
+  }
+  __syncthreads();
+  const int4 wb = warp ? s_w[warp - 1] : make_int4(0, 0, 0, 0);
+  const int4 tot = s_w[kSpScanThreads / 32 - 1];
+  __syncthreads();
+  return SpScan{make_int4(wb.x + x.x - v.x, wb.y + x.y - v.y, wb.z + x.z - v.z, wb.w + x.w - v.w), tot};
+}
+
+// Pass 2 (one block): the per-row offsets (off, ebef, poff, moff), the arrival counters, the tiles' kept bases and
+// the last filled id.  Each thread scans a contiguous run of rows.
+template <typename V>
+__global__ void __launch_bounds__(kSpScanThreads) k_sparse_scan(const V* vals, SparseLayout L, int* ws) {
+  const int* cnt = ws + L.cnt;
+  const long long per = (L.B + kSpScanThreads - 1) / kSpScanThreads;
+  const long long b0 = threadIdx.x * per, b1 = b0 + per < L.B ? b0 + per : L.B;
+  int4 s = make_int4(0, 0, 0, 0);  // filled length, empty rows, pieces, multi-piece slots
+  for (long long b = b0; b < b1; ++b) {
+    const int c = cnt[b], np = sp_pieces(c);
+    s.x += c > 1 ? c : 1; s.y += c == 0; s.z += np; s.w += np > 1 ? np : 0;
+  }
+  const SpScan sc = sp_block_scan(s);
+  int4 e = sc.excl;
+  const int4 tot = sc.tot;
+  for (long long b = b0; b < b1; ++b) {
+    const int c = cnt[b], np = sp_pieces(c);
+    ws[L.off + b] = e.x; ws[L.ebef + b] = e.y; ws[L.poff + b] = e.z; ws[L.moff + b] = e.w;
+    ws[L.arrive + b] = 0;
+    e.x += c > 1 ? c : 1; e.y += c == 0; e.z += np; e.w += np > 1 ? np : 0;
+  }
+  if (threadIdx.x == 0) {
+    ws[L.off + L.B] = tot.x; ws[L.poff + L.B] = tot.z; ws[L.moff + L.B] = tot.w;
+  }
+  // tiles: exclusive scan of the kept counts; the last kept index overall
+  int base = 0, last = -1;
+  for (long long t0 = 0; t0 < L.NT; t0 += kSpScanThreads) {
+    const long long t = t0 + threadIdx.x;
+    const int k = t < L.NT ? ws[L.tkept + t] : 0;
+    if (t < L.NT && ws[L.tlast + t] > last) last = ws[L.tlast + t];
+    const SpScan sc = sp_block_scan(make_int4(k, 0, 0, 0));
+    if (t < L.NT) ws[L.tbase + t] = base + sc.excl.x;
+    base += sc.tot.x;
+  }
+  last = (int)__reduce_max_sync(0xffffffffu, (unsigned)(last + 1)) - 1;
+  __shared__ int s_last;
+  if (threadIdx.x == 0) s_last = -1;
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) atomicMax(&s_last, last);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    // the last filled entry is row B-1's: its fill id 0 when empty, else the last kept id of the input
+    const long long id = cnt[L.B - 1] == 0 ? 0 : (long long)vals[s_last];
+    *reinterpret_cast<long long*>(ws + L.last) = id;
+  }
+}
+
+// Pass 3: scatter the kept ids to their filled positions (tile-local rank in entry order), the fill id 0 of each
+// empty row, the row of every piece, and the tail copies of the last filled id.
+template <typename V>
+__global__ void __launch_bounds__(256) k_sparse_scatter(const long long* rows, const V* vals, SparseLayout L, int* ws,
+                                                        long long* ids_f) {
+  __shared__ int s_w[8];
+  const int* cnt = ws + L.cnt;
+  int* rowf = ws + L.rowf;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long t = blockIdx.x; t < L.NT; t += gridDim.x) {
+    int base = ws[L.tbase + t];
+    for (int q = 0; q < kSpTile / 256; ++q) {
+      const long long i = t * kSpTile + q * 256 + threadIdx.x;
+      long long r = -1;
+      long long v = -1;
+      if (i < L.nnz) {
+        r = rows[i];
+        v = (long long)vals[i];
+      }
+      const bool keep = r >= 0 && r < L.B && v >= 0;
+      const unsigned km = __ballot_sync(0xffffffffu, keep);
+      if (lane == 0) s_w[warp] = __popc(km);
+      __syncthreads();
+      int wb = 0, tot = 0;
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        wb += u < warp ? s_w[u] : 0;
+        tot += s_w[u];
+      }
+      if (keep) {
+        const long long pos = base + wb + __popc(km & ((1u << lane) - 1)) + ws[L.ebef + r];
+        ids_f[pos] = v;
+        rowf[pos] = (int)r;
+      }
+      base += tot;
+      __syncthreads();
+    }
+  }
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  for (long long b = g; b < L.B; b += stride) {
+    const int c = cnt[b], o = ws[L.off + b], po = ws[L.poff + b], np = sp_pieces(c);
+    if (c == 0) {
+      ids_f[o] = 0;
+      rowf[o] = -1;
+    }
+    for (int p = 0; p < np; ++p) ws[L.prow + po + p] = (int)b;
+  }
+  const long long kf = ws[L.off + L.B];
+  const long long last = *reinterpret_cast<const long long*>(ws + L.last);
+  for (long long j = kf + g; j < L.K; j += stride) {
+    ids_f[j] = last;
+    rowf[j] = -1;
+  }
+}
+
+template <int VPT>
+__device__ __forceinline__ void sp_scale_store(float* o, const float* x, int cnt, int combiner) {
+  constexpr int W = VPT == 0 ? 1 : 4 * VPT;
+  float y[W];
+  const float d = combiner == kSpMean ? (float)cnt : fsqrt((float)cnt);
+#pragma unroll
+  for (int e = 0; e < W; ++e) y[e] = cnt == 0 ? 0.f : combiner == kSpSum ? x[e] : fdiv(x[e], d);
+  if (VPT == 0) o[0] = y[0];
+  else {
+#pragma unroll
+    for (int v = 0; v < VPT; ++v) st_f4(o + 4 * v, *reinterpret_cast<float4*>(&y[4 * v]));
+  }
+}
+
+// Combine forward: one warp per piece (<= kSpPiece filled entries of one row).  Lanes split as (entry slot, column
+// chunk): CL lanes cover CL chunks of W floats, E = 32 / CL entries are read at once; each lane sums its entries in
+// entry order, then the lanes of one chunk add through a fixed xor butterfly.  A row of one piece is scaled and
+// stored; the pieces of a longer row store partials and the last piece to finish adds them in piece order and resets
+// the row's arrival counter, so the combine can run again on the same workspace.  Every order is fixed, so two calls
+// give the same bits; it is not strict entry order (see b200ps_sparse_combine).
+template <int VPT>
+__global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict__ bet, const int* __restrict__ inv,
+                                                        SparseLayout L, int* ws, int dim, int combiner, float* out) {
+  constexpr int W = VPT == 0 ? 1 : 4 * VPT;
+  const int chunks = dim / W;
+  int CL = 1;
+  while (CL < chunks && CL < 32) CL <<= 1;
+  const int E = 32 / CL;
+  const int lane = threadIdx.x & 31;
+  const int* off = ws + L.off;
+  float* part = reinterpret_cast<float*>(ws + L.part);
+  const long long npieces = ws[L.poff + L.B];
+  const long long nwarps = (long long)gridDim.x * blockDim.x / 32;
+  for (long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < npieces; w += nwarps) {
+    const int row = ws[L.prow + w];
+    const int po = ws[L.poff + row], np = ws[L.poff + row + 1] - po, p = (int)(w - po);
+    const int cnt = ws[L.cnt + row];
+    const int s = off[row] + p * kSpPiece, e_end = min(s + kSpPiece, off[row + 1]);
+    for (int cb = 0; cb < chunks; cb += CL) {
+      const int c = cb + (lane & (CL - 1));
+      const bool cok = c < chunks;
+      float acc[W];
+#pragma unroll
+      for (int e = 0; e < W; ++e) acc[e] = 0.f;
+      if (cok) {
+        for (int j = s + lane / CL; j < e_end; j += E) {
+          const float* src = bet + (long long)inv[j] * dim + c * W;
+          if (VPT == 0) acc[0] = add(acc[0], __ldg(src));
+          else {
+#pragma unroll
+            for (int v = 0; v < VPT; ++v) {
+              const float4 x = __ldg(reinterpret_cast<const float4*>(src + 4 * v));
+              acc[4 * v] = add(acc[4 * v], x.x); acc[4 * v + 1] = add(acc[4 * v + 1], x.y);
+              acc[4 * v + 2] = add(acc[4 * v + 2], x.z); acc[4 * v + 3] = add(acc[4 * v + 3], x.w);
+            }
+          }
+        }
+      }
+      for (int o = CL; o < 32; o <<= 1) {
+#pragma unroll
+        for (int e = 0; e < W; ++e) acc[e] = add(acc[e], __shfl_xor_sync(0xffffffffu, acc[e], o));
+      }
+      if (cok && lane < CL) {
+        if (np == 1) sp_scale_store<VPT>(out + (long long)row * dim + c * W, acc, cnt, combiner);
+        else {
+          float* dst = part + ((long long)ws[L.moff + row] + p) * dim + c * W;
+#pragma unroll
+          for (int e = 0; e < W; ++e) dst[e] = acc[e];
+        }
+      }
+    }
+    if (np > 1) {
+      __threadfence();
+      __syncwarp();
+      int done = 0;
+      if (lane == 0) done = atomicAdd(ws + L.arrive + row, 1) == np - 1;
+      done = __shfl_sync(0xffffffffu, done, 0);
+      if (done) {
+        __threadfence();
+        if (lane == 0) ws[L.arrive + row] = 0;  // all np pieces have arrived: nothing else touches the counter
+        const float* P = part + (long long)ws[L.moff + row] * dim;
+        for (int c = lane; c < chunks; c += 32) {
+          float acc[W];
+#pragma unroll
+          for (int e = 0; e < W; ++e) acc[e] = 0.f;
+          for (int q = 0; q < np; ++q) {
+#pragma unroll
+            for (int e = 0; e < W; ++e) acc[e] = add(acc[e], __ldcg(P + (long long)q * dim + c * W + e));
+          }
+          sp_scale_store<VPT>(out + (long long)row * dim + c * W, acc, cnt, combiner);
+        }
+      }
+    }
+  }
+}
+
+// Combine backward load: entry j of the filled stream contributes s_row * gout[row, :] when it belongs to a non-empty
+// row (rowf >= 0); the division is the one torch's autograd of out / counts (out / counts.sqrt()) performs.
+template <int VPT>
+struct SparseGradLoad {
+  const float* G;
+  const int* rowf;
+  const int* cnt;
+  int dim, combiner;
+  __device__ __forceinline__ bool live(long long j) const { return rowf[j] >= 0; }
+  __device__ __forceinline__ void load(long long j, int c, float* x) const {
+    const int r = rowf[j];
+    RowsLoad<VPT>{G, dim}.load(r, c, x);
+    if (combiner != kSpSum) {
+      constexpr int W = VPT == 0 ? 1 : 4 * VPT;
+      const int n = cnt[r];
+      const float d = combiner == kSpMean ? (float)n : fsqrt((float)n);
+#pragma unroll
+      for (int e = 0; e < W; ++e) x[e] = fdiv(x[e], d);
+    }
+  }
+};
+
+template <int VPT>
+__global__ void __launch_bounds__(256) k_sparse_combine_grad(const float* gout, const int* inv, SparseLayout L,
+                                                             const int* ws, int dim, int combiner, float* gbet) {
+  const SparseGradLoad<VPT> ld{gout, ws + L.rowf, ws + L.cnt, dim, combiner};
+  segment_sum_loop<VPT>(ld, inv, L.K, dim, gbet);
 }
 
 }  // namespace b200ps_impl

@@ -117,9 +117,12 @@ class Embedding(torch.nn.Module):
             bet = torch.as_tensor(bet, dtype=torch.float32, device=unique_ids.device)
         return bet
 
-    def _unique_and_pull(self, flat_ids):
+    def _unique_and_pull(self, flat_ids, dropped=None):
         uniq, inv, n = ops.unique(flat_ids, 1)
         u = int(n.item())  # exact BET shape, as the reference exposes it
+        if dropped is not None and int(dropped.item()):  # the stream is idle after n.item(): a 4-byte copy
+            raise ValueError("sparse input has %d entries whose row index is outside [0, batch_size)"
+                             % int(dropped.item()))
         unique_ids = uniq[:u]
         bet = self._gather_embedding_vectors(unique_ids)
         if self.tape:
@@ -154,29 +157,11 @@ class Embedding(torch.nn.Module):
 
     def safe_embedding_lookup_sparse(self, sparse_ids, combiner="mean"):
         """embedding_delegate.py:108-230 without weights: prune ids < 0, give empty rows
-        id 0, combine per row, then zero the rows that were empty."""
+        id 0, combine per row, then zero the rows that were empty (ops.sparse_prep and
+        ops.SparseCombine: CUDA kernels from the coalesced COO to the [batch, dim] output)."""
         sp = sparse_ids.coalesce()
-        rows = sp.indices()[0]
-        vals = sp.values().to(torch.int64)
         batch = sp.shape[0]
-        keep = vals >= 0  # _prune_invalid_ids
-        rows, vals = rows[keep], vals[keep]
-        counts = torch.bincount(rows, minlength=batch)
-        is_row_empty = counts == 0
-        empty_rows = torch.nonzero(is_row_empty).reshape(-1)
-        if empty_rows.numel():  # sparse_fill_empty_rows(sparse_ids, 0)
-            rows = torch.cat([rows, empty_rows])
-            vals = torch.cat([vals, torch.zeros_like(empty_rows)])
-            order = torch.argsort(rows, stable=True)
-            rows, vals = rows[order], vals[order]
-            counts = torch.bincount(rows, minlength=batch)
-        k = vals.numel()
-        bet, inv = self._unique_and_pull(vals)
-        per_id = ops.GatherRows.apply(bet, inv, 1, k, self.output_dim)
-        out = torch.zeros((batch, self.output_dim), dtype=torch.float32, device=per_id.device)
-        out = out.index_add(0, rows, per_id)  # segment_sum
-        if combiner == "mean":
-            out = out / counts.clamp(min=1).to(out.dtype).unsqueeze(1)
-        elif combiner == "sqrtn":
-            out = out / counts.clamp(min=1).to(out.dtype).sqrt().unsqueeze(1)
-        return torch.where(is_row_empty.unsqueeze(1), torch.zeros_like(out), out)
+        nnz = sp.values().numel()
+        ids, ws = ops.sparse_prep(sp.indices()[0], sp.values(), batch, self.output_dim)
+        bet, inv = self._unique_and_pull(ids, dropped=ws[:4].view(torch.int32))
+        return ops.SparseCombine.apply(bet, inv, ws, batch, nnz, combiner, self.output_dim)

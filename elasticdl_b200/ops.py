@@ -1,6 +1,7 @@
 """Device primitives of the client side of the exchange, as torch-level calls
 into libb200ps.so: first-occurrence unique (tf.unique), row gather and its
-backward (segment sum with warp-level id dedup).  CUDA only -- no fallback."""
+backward (segment sum with warp-level id dedup), and the pooled lookup of sparse
+input (prep, combine and its backward).  CUDA only -- no fallback."""
 import ctypes
 
 import torch
@@ -73,6 +74,62 @@ def segment_sum(values, inv, T, k, dim):
         check(_lib.lib().b200ps_segment_sum(None, values.data_ptr(), inv.data_ptr(), T, k, dim, out.data_ptr(),
                                             _stream(values.device)))
     return out
+
+
+COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
+
+
+def sparse_prep(rows, vals, batch, dim):
+    """_prune_invalid_ids + sparse_fill_empty_rows(ids, 0) (embedding_delegate.py:155-170) of a coalesced
+    [batch, L] COO (rows int64 [nnz] row-major, vals int64 | int32 [nnz]), in three launches with no host read.
+    Returns (ids int64 [nnz + batch]: the filled id stream, then copies of its last id; ws: the workspace the
+    combine reads, whose first int32 counts the entries dropped for a row outside [0, batch))."""
+    _need_cuda(vals, "vals")
+    nnz = vals.numel()
+    rows = rows.contiguous().view(-1)
+    vals = vals.contiguous().view(-1)
+    if vals.dtype not in (torch.int32, torch.int64):
+        vals = vals.to(torch.int64)
+    lib = _lib.lib()
+    need = lib.b200ps_sparse_workspace(batch, nnz, dim)
+    ws = torch.empty(need, dtype=torch.uint8, device=vals.device)
+    ids = torch.empty(nnz + batch, dtype=torch.int64, device=vals.device)
+    with torch.cuda.device(vals.device):
+        check(lib.b200ps_sparse_prep(None, rows.data_ptr() if nnz else None, vals.data_ptr() if nnz else None,
+                                     int(vals.dtype == torch.int32), batch, nnz, dim, ids.data_ptr(), ws.data_ptr(),
+                                     need, _stream(vals.device)))
+    return ids, ws
+
+
+class SparseCombine(torch.autograd.Function):
+    """BET [U, dim] -> [batch, dim]: each row's BET rows summed, scaled by the combiner, 0 for the rows that were
+    empty (sparse_segment_{sum,mean,sqrt_n}); backward = the scaled segment sum into [U, dim].  dim is the one
+    sparse_prep sized `ws` for."""
+
+    @staticmethod
+    def forward(ctx, bet, inv, ws, batch, nnz, combiner, dim):
+        bet = bet.contiguous()
+        if bet.dim() != 2 or bet.shape[1] != dim:
+            raise ValueError("the lookup returned rows of shape %s, the layer needs [n_unique, %d]"
+                             % (tuple(bet.shape), dim))
+        ctx.save_for_backward(inv, ws)
+        ctx.shape = (batch, nnz, dim, COMBINERS[combiner], bet.shape[0])
+        out = torch.empty((batch, dim), dtype=torch.float32, device=bet.device)
+        with torch.cuda.device(bet.device):
+            check(_lib.lib().b200ps_sparse_combine(None, bet.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(), batch,
+                                                   nnz, dim, COMBINERS[combiner], out.data_ptr(), _stream(bet.device)))
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        inv, ws = ctx.saved_tensors
+        batch, nnz, dim, comb, u = ctx.shape
+        g = grad_out.contiguous()
+        gbet = torch.empty((u, dim), dtype=torch.float32, device=g.device)
+        with torch.cuda.device(g.device):
+            check(_lib.lib().b200ps_sparse_combine_grad(None, g.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                        batch, nnz, dim, comb, u, gbet.data_ptr(), _stream(g.device)))
+        return gbet, None, None, None, None, None, None
 
 
 class GatherRows(torch.autograd.Function):

@@ -308,6 +308,38 @@ int b200ps_segment_sum(b200ps_t* ps, const float* values_dev, const int32_t* inv
 int b200ps_gather_rows(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, int T, int64_t k,
                        int dim, float* out_dev, void* stream);
 
+/* ---- pooled lookup of a sparse [B, L] input (safe_embedding_lookup_sparse without weights,
+ * embedding_delegate.py:108-230): prune ids < 0, give each empty row the id 0, sum each row's BET rows, scale
+ * (combiner 0 = sum, 1 = mean: / cnt, 2 = sqrtn: / sqrtf(cnt)), write 0 for the rows that were empty.
+ * The input is a coalesced COO: rows_dev int64 [nnz] in row-major order, vals_dev int64 or int32 [nnz].  All three
+ * take the same (B, nnz, dim) and one workspace of b200ps_sparse_workspace(B, nnz, dim) bytes (16 B aligned), which
+ * prep fills and combine / combine_grad use; either may run any number of times after one prep.  Each refuses a
+ * workspace_bytes smaller than b200ps_sparse_workspace(B, nnz, dim), nnz + B above INT32_MAX.  ps may be NULL, as for
+ * b200ps_unique. */
+size_t b200ps_sparse_workspace(int64_t B, int64_t nnz, int dim);
+/* Three launches, no host read.  ids_dev int64 [nnz + B] receives the filled id stream: row-major, the kept ids in
+ * input order and one id 0 in the slot of each empty row, then copies of the last filled id up to nnz + B (a repeat
+ * changes neither tf.unique's set nor its first-occurrence order, so b200ps_unique can take all nnz + B entries).
+ * An entry whose row lies outside [0, B) is dropped and counted in the workspace's first int32 word. */
+int b200ps_sparse_prep(b200ps_t* ps, const int64_t* rows_dev, const void* vals_dev, int vals_are_int32, int64_t B,
+                       int64_t nnz, int dim, int64_t* ids_dev, void* workspace_dev, size_t workspace_bytes,
+                       void* stream);
+/* out_dev[b, :] = s_b * sum of bet_dev[inv_dev[j], :] over row b's filled entries j; bet_dev is [U, dim] (the
+ * unique rows), inv_dev is b200ps_unique's inverse of ids_dev.  One launch.  Rows of any length are split into
+ * pieces of 256 entries across warps.  The sum is NOT in strict entry order: within a piece each lane sums a
+ * lane-strided subset of the entries in order, the lanes are added through a fixed xor butterfly, and the pieces of a
+ * row in piece order.  Every order is fixed, so two calls give the same bits, and the result lies within
+ * (m - 1) 2^-24 sum|x| of the exact sum of m entries, as any order does. */
+int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, void* workspace_dev,
+                          size_t workspace_bytes, int64_t B, int64_t nnz, int dim, int combiner, float* out_dev,
+                          void* stream);
+/* Its backward: gbet_dev [n_unique, dim] = 0, then gbet[inv[j], :] += s_row(j) * gout[row(j), :] for every entry j of
+ * a non-empty row (b200ps_segment_sum's warp-dedup reduction, with its INT32_MAX work-item refusal: (nnz + B) *
+ * (dim / W)). */
+int b200ps_sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev, const void* workspace_dev,
+                               size_t workspace_bytes, int64_t B, int64_t nnz, int dim, int combiner, int64_t n_unique,
+                               float* gbet_dev, void* stream);
+
 /* ---- state queries (synchronous on the client device) ---------------- */
 int b200ps_shard_state(b200ps_t* ps, int shard, int32_t* version, int64_t* step, int32_t* initialized);
 int b200ps_set_shard_state(b200ps_t* ps, int shard, int32_t version, int64_t step, int32_t initialized);
