@@ -178,6 +178,12 @@ SYMBOLS = {
     "b200feat_hash_strings": (_i, [_vp, _i, _i64, _i64, _vp, _vp]),
     "b200feat_hash_ints": (_i, [_vp, _i64, _i64, _vp, _vp]),
     "b200feat_bucketize": (_i, [_vp, _i64, _vp, _i, _vp, _vp]),
+    "b200feat_transform_ext": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _i, _i, _i64, _vp, _i, _vp, _vp]),
+    "b200feat_vocab_slots": (_i64, [_i64]),
+    "b200feat_vocab_build": (_i, [_vp, _i64, _i, _i64, _vp, ctypes.POINTER(_i64)]),
+    "b200feat_index_lookup": (_i, [_vp, _i, _i64, _vp, _vp, _i64, ctypes.c_int32, ctypes.c_int32, _i64, _vp, _vp]),
+    "b200feat_log_round": (_i, [_vp, _i, _i64, _i64, _i64, _i, ctypes.c_double, _vp, _vp]),
+    "b200feat_round_identity": (_i, [_vp, _i, _i64, _i64, _i64, _vp, _vp]),
     "b200feat_fingerprint64": (_i, [_vp, _i, _i64, _vp, _vp]),
     "b200feat_launch_count": (_i64, []),
 }

@@ -1,13 +1,19 @@
-// Feature-id generation on the GPU (include/b200_features.h): Hashing / Discretization /
-// ConcatenateWithOffset / Normalizer of elasticdl_preprocessing/layers, fused into one launch that
-// writes the [G][B] id matrix b200ps_unique consumes -- the worker's feature transform
-// (model_zoo/dac_ctr/feature_transform.py:36-118) no longer runs on the host.
+// Feature-id generation on the GPU (include/b200_features.h): Hashing / Discretization / IndexLookup /
+// LogRound / RoundIdentity / ConcatenateWithOffset / Normalizer of elasticdl_preprocessing/layers, fused
+// into one launch that writes the [G][B] id matrix b200ps_unique consumes -- the worker's feature transform
+// (model_zoo/dac_ctr/feature_transform.py:36-118, census_wide_deep_model/wide_deep_functional_api.py:120-161)
+// no longer runs on the host.
 //
 // HBM-bound integer / byte work: one thread per (group, sample); inputs are feature-major so a warp
-// reads 32 consecutive values of one feature (coalesced), ids are written coalesced.
+// reads 32 consecutive values of one feature (coalesced), ids are written coalesced.  IndexLookup probes a
+// vocabulary table built on the host (b200feat_vocab_build) straight from global memory through the
+// read-only cache: one 16-byte slot load per probe step, the term bytes only on a fingerprint match.
 #include <cuda_runtime.h>
 
+#include <cmath>
+#include <cstddef>
 #include <cstdint>
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <type_traits>
@@ -136,21 +142,108 @@ __device__ inline int bucketize(float x, const float* b, int n) {
   return lo;
 }
 
+static_assert(sizeof(b200feat_vocab_slot_t) == 16 && offsetof(b200feat_vocab_slot_t, index) == 8 &&
+                  offsetof(b200feat_vocab_slot_t, length) == 12,
+              "b200feat_vocab_slot_t is one 16-byte load: {fingerprint, index | length << 32}");
+
+// The launch's copy of b200feat_group_ext_t: the table's probe mask, and log(base) taken once on the host.
+struct GroupExt {
+  const ulonglong2* slots;
+  const uint8_t* terms;
+  unsigned long long mask;  // n_slots - 1
+  int V, Wv;
+  long long dflt;
+  double log_base;
+  int has_base;
+};
+
 struct Plan {  // passed by value (< 4 KB): the launch is self-contained and capturable in a CUDA graph
   b200feat_group_t group[kMaxGroups];
   b200feat_dense_t dense[kMaxDense];
   float bnd[kMaxBoundaries];
   int G, n_dense;
 };
+// A transform with LOOKUP / LOG_ROUND / ROUND_IDENTITY groups launches this one (7.4 KB, still by value); one without
+// them launches the Plan instance, whose parameters and code are those of the dac_ctr kinds alone.
+struct PlanExt : Plan {
+  GroupExt ext[kMaxGroups];
+};
+// kernel parameters may take 32,764 bytes on sm_70+ from CUDA 12.1; the other arguments take 48
+static_assert(sizeof(PlanExt) + 64 <= 32764, "PlanExt no longer fits the kernel parameter space");
 
-// T: the numeric columns' type (long long or float)
+// IndexLookup: linear probing from the home slot, at most n_slots steps (a malformed table cannot hang the
+// launch).  An empty slot ends the chain; a slot whose fingerprint and length match is compared byte by byte.
+// Out of vocabulary: V + fp % num_oov (IdTableWithHashBuckets over FastHashSpec), or -1 without OOV buckets.
+__device__ inline long long vocab_lookup(uint64_t fp, const unsigned char* buf, int len, const GroupExt& e,
+                                         long long num_oov) {
+  unsigned long long h = fp & e.mask;
+  for (unsigned long long n = 0; n <= e.mask; ++n) {
+    const ulonglong2 slot = __ldg(e.slots + h);
+    const int index = (int)(unsigned)slot.y, length = (int)(slot.y >> 32);
+    if (index < 0) break;
+    if (slot.x == fp && length == len && index < e.V && len <= e.Wv) {
+      const uint8_t* t = e.terms + (long long)index * e.Wv;
+      int i = 0;
+      while (i < len && __ldg(t + i) == buf[i]) ++i;
+      if (i == len) return index;
+    }
+    h = (h + 1) & e.mask;
+  }
+  return num_oov > 0 ? (long long)e.V + (long long)(fp % (unsigned long long)num_oov) : -1;
+}
+
+// LogRound / RoundIdentity: tf.cast(r, int64) then `r < 0 || r >= num_bins -> default`.  NaN, +-inf and
+// r >= 2^63 go to the default too: TF on x86 casts them to INT64_MIN (cvttsd2si), which is < 0.
+__device__ inline long long rounded_id(double r, long long num_bins, long long dflt) {
+  if (!(r >= 0.0) || r >= 9223372036854775808.0) return dflt;
+  const long long v = (long long)r;
+  return v < num_bins ? v : dflt;
+}
+
+// LOOKUP / LOG_ROUND / ROUND_IDENTITY ids of group g (the kind is uniform over the block row)
 template <typename T>
-__global__ void __launch_bounds__(256) k_feature_transform(Plan p, const T* numeric, const uint8_t* __restrict__ strings,
+__device__ __forceinline__ void ext_group_ids(const b200feat_group_t& gr, const GroupExt& ex, int g, const T* numeric,
+                                              const uint8_t* __restrict__ strings, int W, long long B, void* ids_out,
+                                              int ids32) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += stride) {
+    long long id;
+    if (gr.kind == B200FEAT_LOOKUP) {
+      unsigned char buf[kMaxW];
+      const int len = load_string(strings + ((long long)gr.column * B + b) * W, W, buf);
+      id = vocab_lookup(fingerprint64(buf, len), buf, len, ex, gr.num_bins);
+    } else if (gr.kind == B200FEAT_LOG_ROUND) {
+      // tf.cast(x, float64), then log(x) or log(x) / log(base) in float64, tf.math.round = half to even
+      double q = log((double)numeric[(long long)gr.column * B + b]);
+      if (ex.has_base) q = q / ex.log_base;
+      id = rounded_id(rint(q), gr.num_bins, ex.dflt);
+    } else {  // ROUND_IDENTITY
+      const T x = numeric[(long long)gr.column * B + b];
+      if constexpr (std::is_same<T, long long>::value)  // integers pass through K.round unchanged
+        id = x >= 0 && x < gr.num_bins ? x : ex.dflt;
+      else  // K.round of float32 = rint in float32
+        id = rounded_id((double)rintf(x), gr.num_bins, ex.dflt);
+    }
+    id += gr.offset;
+    if (ids32) reinterpret_cast<int*>(ids_out)[(long long)g * B + b] = (int)id;
+    else reinterpret_cast<long long*>(ids_out)[(long long)g * B + b] = id;
+  }
+}
+
+// T: the numeric columns' type (long long or float); P: Plan, or PlanExt when a group has a kind >= LOOKUP
+template <typename T, typename P>
+__global__ void __launch_bounds__(256) k_feature_transform(P p, const T* numeric, const uint8_t* __restrict__ strings,
                                                            int W, long long B, void* ids_out, int ids32, float* dense_out) {
   __shared__ float s_bnd[kMaxBoundaries];
   const int g = blockIdx.y;
   if (g < p.G) {
     const b200feat_group_t& gr = p.group[g];
+    if constexpr (std::is_same<P, PlanExt>::value) {
+      if (gr.kind > B200FEAT_HASH_INT) {
+        ext_group_ids(gr, p.ext[g], g, numeric, strings, W, B, ids_out, ids32);
+        return;
+      }
+    }
     if (gr.kind == B200FEAT_DISCRETIZE) {
       for (int i = threadIdx.x; i < gr.n_boundaries; i += blockDim.x) s_bnd[i] = p.bnd[gr.boundary_off + i];
       __syncthreads();
@@ -221,6 +314,15 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
                        const b200feat_dense_t* dense, int n_dense, const void* numeric_dev, int n_numeric,
                        int numeric_is_float, const uint8_t* strings_dev, int n_string, int W, int64_t B,
                        void* ids_out_dev, int ids32, float* dense_out_dev, void* stream) {
+  return b200feat_transform_ext(groups, nullptr, G, boundaries, n_boundaries, dense, n_dense, numeric_dev, n_numeric,
+                                numeric_is_float, strings_dev, n_string, W, B, ids_out_dev, ids32, dense_out_dev, stream);
+}
+
+int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_ext_t* ext, int G,
+                           const float* boundaries, int n_boundaries, const b200feat_dense_t* dense, int n_dense,
+                           const void* numeric_dev, int n_numeric, int numeric_is_float, const uint8_t* strings_dev,
+                           int n_string, int W, int64_t B, void* ids_out_dev, int ids32, float* dense_out_dev,
+                           void* stream) {
   if (G < 0 || G > kMaxGroups) return fail(-1, "bad group count (max 64)");
   if (n_dense < 0 || n_dense > kMaxDense) return fail(-1, "bad dense column count (max 32)");
   if (B < 1) return fail(-1, "bad batch size");
@@ -228,13 +330,14 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
   if (G > 0 && (!groups || !ids_out_dev)) return fail(-1, "groups / ids_out is null");
   if (n_dense > 0 && (!dense || !dense_out_dev)) return fail(-1, "dense / dense_out is null");
   if (W < 0 || W > kMaxW) return fail(-1, "strings longer than 64 bytes are not supported (FarmHash restated for lengths 0..64)");
-  Plan p;
+  PlanExt p;
   memset(&p, 0, sizeof(p));
+  bool ext_kinds = false;
   p.G = ids_out_dev ? G : 0;
   p.n_dense = dense_out_dev ? n_dense : 0;
   for (int g = 0; g < p.G; ++g) {
     const b200feat_group_t& gr = groups[g];
-    int64_t span;  // largest id before the offset
+    int64_t lo = 0, hi;  // smallest and largest id before the offset
     if (gr.kind == B200FEAT_DISCRETIZE) {
       if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "discretize: bad numeric column");
       if (gr.n_boundaries < 0 || gr.boundary_off < 0 || gr.boundary_off + gr.n_boundaries > n_boundaries || (gr.n_boundaries && !boundaries))
@@ -243,23 +346,52 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
       for (int i = gr.boundary_off; i < gr.boundary_off + gr.n_boundaries; ++i)
         if (boundaries[i] != boundaries[i] || (i > gr.boundary_off && boundaries[i] < boundaries[i - 1]))
           return fail(-1, "discretize: boundaries are not sorted in ascending order (or hold a NaN)");
-      span = gr.n_boundaries;
+      hi = gr.n_boundaries;
     } else if (gr.kind == B200FEAT_HASH_STRING) {
       if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1) return fail(-1, "hash: bad string column");
       if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");  // hashing.py:53-56
-      span = gr.num_bins - 1;
+      hi = gr.num_bins - 1;
     } else if (gr.kind == B200FEAT_HASH_INT) {
       if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "hash: bad numeric column");
       if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");
       // Hashing converts integer inputs only (hashing.py:63-72); to_hash_bucket_fast refuses float tensors
       if (numeric_is_float) return fail(-1, "hash_int: Hashing takes integer columns, these numeric columns are float32");
-      span = gr.num_bins - 1;
+      hi = gr.num_bins - 1;
+    } else if (ext && gr.kind == B200FEAT_LOOKUP) {
+      const b200feat_group_ext_t& e = ext[g];
+      if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1)
+        return fail(-1, "lookup: bad string column (IndexLookup takes string columns)");
+      if (!e.slots_dev || !e.terms_dev) return fail(-1, "lookup: null table");
+      if (e.V < 1) return fail(-1, "lookup: vocabulary size V must be >= 1");
+      if (e.Wv < 1 || e.Wv > kMaxW) return fail(-1, "lookup: term width Wv must be 1..64");
+      if (e.n_slots < 2 * (int64_t)e.V || (e.n_slots & (e.n_slots - 1)))
+        return fail(-1, "lookup: n_slots must be a power of two >= 2V");
+      if (gr.num_bins < 0) return fail(-1, "lookup: num_oov_tokens must be >= 0");
+      if (gr.num_bins > INT64_MAX - e.V) return fail(-1, "lookup: V + num_oov_tokens overflows int64");
+      if (gr.num_bins == 0) lo = -1;  // the table's default_value
+      hi = gr.num_bins > 0 ? e.V + gr.num_bins - 1 : e.V - 1;
+      p.ext[g].slots = reinterpret_cast<const ulonglong2*>(e.slots_dev);
+      p.ext[g].terms = e.terms_dev;
+      p.ext[g].mask = (unsigned long long)e.n_slots - 1;
+      p.ext[g].V = e.V;
+      p.ext[g].Wv = e.Wv;
+    } else if (ext && (gr.kind == B200FEAT_LOG_ROUND || gr.kind == B200FEAT_ROUND_IDENTITY)) {
+      const b200feat_group_ext_t& e = ext[g];
+      if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev)
+        return fail(-1, gr.kind == B200FEAT_LOG_ROUND ? "log_round: bad numeric column" : "round_identity: bad numeric column");
+      // ids: [0, num_bins) u {default_value}; num_bins <= 0 is accepted (log_round.py:53-57): every id is the default
+      lo = gr.num_bins > 0 ? std::min<int64_t>(0, e.default_value) : e.default_value;
+      hi = gr.num_bins > 0 ? std::max<int64_t>(gr.num_bins - 1, e.default_value) : e.default_value;
+      p.ext[g].dflt = e.default_value;
+      p.ext[g].has_base = gr.kind == B200FEAT_LOG_ROUND && e.has_base;
+      p.ext[g].log_base = std::log(e.base);  // base = 0: -inf, and log(x) / -inf = -+0 (not refused, like the reference)
     } else {
       return fail(-1, "unknown group kind");
     }
-    if (ids32 && (gr.offset < INT32_MIN || gr.offset > (int64_t)INT32_MAX - span))
+    if (ids32 && ((__int128)gr.offset + lo < INT32_MIN || (__int128)gr.offset + hi > INT32_MAX))
       return fail(-1, "int32 ids: offset + id range of a group does not fit int32");
     p.group[g] = gr;
+    ext_kinds |= gr.kind > B200FEAT_HASH_INT;
   }
   for (int j = 0; j < p.n_dense; ++j) {
     if (dense[j].column < 0 || dense[j].column >= n_numeric || !numeric_dev) return fail(-1, "normalizer: bad numeric column");
@@ -273,15 +405,57 @@ int b200feat_transform(const b200feat_group_t* groups, int G, const float* bound
   const int per = (max_blocks() + p.G + p.n_dense - 1) / (p.G + p.n_dense);
   if (gx > per) gx = per < 1 ? 1 : per;
   dim3 grid(gx, p.G + p.n_dense);
-  if (numeric_is_float)
+  const Plan& base = p;
+  if (numeric_is_float && ext_kinds)
     k_feature_transform<<<grid, 256, 0, st>>>(p, (const float*)numeric_dev, strings_dev, W, (long long)B, ids_out_dev,
                                               ids32, dense_out_dev);
-  else
-    k_feature_transform<<<grid, 256, 0, st>>>(p, (const long long*)numeric_dev, strings_dev, W, (long long)B, ids_out_dev,
+  else if (numeric_is_float)
+    k_feature_transform<<<grid, 256, 0, st>>>(base, (const float*)numeric_dev, strings_dev, W, (long long)B, ids_out_dev,
                                               ids32, dense_out_dev);
+  else if (ext_kinds)
+    k_feature_transform<<<grid, 256, 0, st>>>(p, (const long long*)numeric_dev, strings_dev, W, (long long)B,
+                                              ids_out_dev, ids32, dense_out_dev);
+  else
+    k_feature_transform<<<grid, 256, 0, st>>>(base, (const long long*)numeric_dev, strings_dev, W, (long long)B,
+                                              ids_out_dev, ids32, dense_out_dev);
   g_launches++;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(-2, cudaGetErrorString(e));
+  return 0;
+}
+
+int64_t b200feat_vocab_slots(int64_t V) {
+  if (V < 1 || V >= (1LL << 31)) return -1;
+  int64_t n = 2;
+  while (n < 2 * V) n <<= 1;
+  return n;
+}
+
+int b200feat_vocab_build(const uint8_t* terms, int64_t V, int Wv, int64_t n_slots, b200feat_vocab_slot_t* slots,
+                         int64_t* dup_pos) {
+  if (V < 1 || V >= (1LL << 31)) return fail(-1, "vocab build: V must be 1 .. 2^31 - 1");
+  if (Wv < 1 || Wv > kMaxW) return fail(-1, "vocab build: term width Wv must be 1..64");
+  if (n_slots < 2 * V || (n_slots & (n_slots - 1))) return fail(-1, "vocab build: n_slots must be a power of two >= 2V");
+  if (!terms || !slots) return fail(-1, "vocab build: terms / slots is null");
+  for (int64_t i = 0; i < n_slots; ++i) slots[i] = b200feat_vocab_slot_t{0, -1, 0};
+  const uint64_t mask = (uint64_t)n_slots - 1;
+  for (int64_t v = 0; v < V; ++v) {
+    const uint8_t* t = terms + v * Wv;
+    int len = 0;
+    while (len < Wv && t[len]) ++len;
+    for (int i = len; i < Wv; ++i)
+      if (t[i]) return fail(-1, "vocab build: term " + std::to_string(v) + " holds a NUL byte (rows are zero padded)");
+    const uint64_t fp = fingerprint64(t, len);
+    uint64_t h = fp & mask;
+    for (; slots[h].index >= 0; h = (h + 1) & mask) {  // load <= 1/2: an empty slot is always reached
+      const b200feat_vocab_slot_t& s = slots[h];
+      if (s.fingerprint == fp && s.length == len && memcmp(terms + (int64_t)s.index * Wv, t, len) == 0) {
+        if (dup_pos) *dup_pos = v;
+        return fail(-1, "vocab build: term " + std::to_string(v) + " repeats term " + std::to_string(s.index));
+      }
+    }
+    slots[h] = b200feat_vocab_slot_t{fp, (int32_t)v, len};
+  }
   return 0;
 }
 
@@ -304,6 +478,46 @@ int b200feat_bucketize(const float* x_dev, int64_t n, const float* boundaries, i
   g.kind = B200FEAT_DISCRETIZE;
   g.n_boundaries = n_boundaries;
   return b200feat_transform(&g, 1, boundaries, n_boundaries, nullptr, 0, x_dev, 1, 1, nullptr, 0, 0, n, out_dev, 0, nullptr, stream);
+}
+
+int b200feat_index_lookup(const uint8_t* strings_dev, int W, int64_t n, const b200feat_vocab_slot_t* slots_dev,
+                          const uint8_t* terms_dev, int64_t n_slots, int32_t V, int32_t Wv, int64_t num_oov_tokens,
+                          int64_t* out_dev, void* stream) {
+  b200feat_group_t g{};
+  g.kind = B200FEAT_LOOKUP;
+  g.num_bins = num_oov_tokens;
+  b200feat_group_ext_t e{};
+  e.slots_dev = slots_dev;
+  e.terms_dev = terms_dev;
+  e.n_slots = n_slots;
+  e.V = V;
+  e.Wv = Wv;
+  return b200feat_transform_ext(&g, &e, 1, nullptr, 0, nullptr, 0, nullptr, 0, 0, strings_dev, 1, W, n, out_dev, 0,
+                                nullptr, stream);
+}
+
+int b200feat_log_round(const void* x_dev, int x_is_float, int64_t n, int64_t num_bins, int64_t default_value,
+                       int has_base, double base, int64_t* out_dev, void* stream) {
+  b200feat_group_t g{};
+  g.kind = B200FEAT_LOG_ROUND;
+  g.num_bins = num_bins;
+  b200feat_group_ext_t e{};
+  e.default_value = default_value;
+  e.has_base = has_base;
+  e.base = base;
+  return b200feat_transform_ext(&g, &e, 1, nullptr, 0, nullptr, 0, x_dev, 1, x_is_float, nullptr, 0, 0, n, out_dev, 0,
+                                nullptr, stream);
+}
+
+int b200feat_round_identity(const void* x_dev, int x_is_float, int64_t n, int64_t num_buckets, int64_t default_value,
+                            int64_t* out_dev, void* stream) {
+  b200feat_group_t g{};
+  g.kind = B200FEAT_ROUND_IDENTITY;
+  g.num_bins = num_buckets;
+  b200feat_group_ext_t e{};
+  e.default_value = default_value;
+  return b200feat_transform_ext(&g, &e, 1, nullptr, 0, nullptr, 0, x_dev, 1, x_is_float, nullptr, 0, 0, n, out_dev, 0,
+                                nullptr, stream);
 }
 
 int b200feat_fingerprint64(const uint8_t* strings_dev, int W, int64_t n, uint64_t* out_dev, void* stream) {
