@@ -55,6 +55,16 @@ class DeepFMArgs(ctypes.Structure):  # b200_deepfm_args_t (include/b200_deepfm.h
     ]
 
 
+class CensusArgs(ctypes.Structure):  # b200_census_args_t (include/b200_census.h)
+    _fields_ = [
+        ("B", ctypes.c_int32), ("reference_reshape", ctypes.c_int32),
+        ("ids", ctypes.c_void_p), ("labels", ctypes.c_void_p), ("params", ctypes.c_void_p),
+        ("loss", ctypes.c_void_p), ("logits", ctypes.c_void_p), ("grads", ctypes.c_void_p),
+        ("uniq", ctypes.c_void_p), ("n_unique", ctypes.c_void_p), ("gsum", ctypes.c_void_p),
+        ("error", ctypes.c_void_p), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 class PSError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("b200ps error %d: %s" % (code, msg))
@@ -187,6 +197,13 @@ SYMBOLS = {
     "b200feat_fingerprint64": (_i, [_vp, _i, _i64, _vp, _vp]),
     "b200feat_launch_count": (_i64, []),
 }
+# include/b200_census.h
+CENSUS_SYMBOLS = {
+    "b200_census_workspace_bytes": (_sz, [_i64]),
+    "b200_census_tower": (_i, [ctypes.POINTER(CensusArgs), _vp]),
+    "b200_census_last_error": (ctypes.c_char_p, []),
+    "b200_census_launch_count": (_i64, []),
+}
 
 _lib = None
 
@@ -199,7 +216,7 @@ def lib():
         if not os.path.exists(path) or _build._stale():
             path = _build.build()
         handle = ctypes.CDLL(path)
-        for name, (res, args) in SYMBOLS.items():
+        for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args
