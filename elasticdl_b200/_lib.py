@@ -65,6 +65,17 @@ class CensusArgs(ctypes.Structure):  # b200_census_args_t (include/b200_census.h
     ]
 
 
+class FrappeArgs(ctypes.Structure):  # b200_frappe_args_t (include/b200_frappe.h)
+    _fields_ = [
+        ("B", ctypes.c_int32), ("pad_", ctypes.c_int32),
+        ("ids", ctypes.c_void_p), ("inv", ctypes.c_void_p), ("n_unique", ctypes.c_void_p),
+        ("bet_deep", ctypes.c_void_p), ("bet_wide", ctypes.c_void_p), ("labels", ctypes.c_void_p),
+        ("params", ctypes.c_void_p), ("loss", ctypes.c_void_p), ("logits", ctypes.c_void_p),
+        ("grads", ctypes.c_void_p), ("gsum_deep", ctypes.c_void_p), ("gsum_wide", ctypes.c_void_p),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 class PSError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("b200ps error %d: %s" % (code, msg))
@@ -204,6 +215,14 @@ CENSUS_SYMBOLS = {
     "b200_census_last_error": (ctypes.c_char_p, []),
     "b200_census_launch_count": (_i64, []),
 }
+# include/b200_frappe.h
+FRAPPE_SYMBOLS = {
+    "b200_frappe_workspace_bytes": (_sz, [_i64]),
+    "b200_frappe_tower": (_i, [ctypes.POINTER(FrappeArgs), _vp]),
+    "b200_frappe_forward": (_i, [ctypes.POINTER(FrappeArgs), _vp]),
+    "b200_frappe_last_error": (ctypes.c_char_p, []),
+    "b200_frappe_launch_count": (_i64, []),
+}
 
 _lib = None
 
@@ -216,7 +235,7 @@ def lib():
         if not os.path.exists(path) or _build._stale():
             path = _build.build()
         handle = ctypes.CDLL(path)
-        for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()):
+        for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args
