@@ -18,6 +18,8 @@ import math
 
 import torch
 
+from oracle import tf32 as _tf32
+
 ND, D, H1, H2 = 13, 8, 16, 4
 WD_PAD = 16
 EPS32 = 2.0 ** -24
@@ -133,10 +135,17 @@ def _scatter_rows(occ, inv, n_rows):
     return out.view(G, n_rows, k)
 
 
-def tower_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, weight=None):
+def tower_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, weight=None, contraction=None,
+                    dnn_masks=None):
     """Float64 forward + backward of one batch.  weight [B] (optional): a multiplicity per sample in every
     reduction (loss, parameter gradients, per-id sums) -- 1 everywhere is the real tower; the comparator
     tests use 0 / 32 to model a dropped / replayed sample.
+
+    contraction (oracle/tf32.py modes): the first layer's three contractions evaluated with the TF32 products of
+    a mode, with the operands the mma tower (csrc/deepfm_tower_mma.cu) splits: "forward" H = [x | 1] [W1 | b1]^T,
+    "data" dX = dH1 W1[:, deep columns], "weight" [dW1 | db1] = dH1^T [x | 1].  dnn_masks (m1 [B, 16], m2 [B, 4]
+    bool): the ReLU masks to use instead of h > 0 (an emulated run takes the exact run's, so that its error does
+    not flip a unit).  The magnitudes are those of the exact run's operands either way.
 
     Returns a dict of float64 tensors on the inputs' device:
       logits [B], loss [], grads [P] (flat layout, padding 0), gsum_wide [G, B], gsum_deep [G, B, 8]
@@ -152,14 +161,19 @@ def tower_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, we
     y = labels.to(f64)
     wd, W1, b1, W2, b2, w3 = (t.to(f64) for t in unflatten(params, G))
     w = torch.ones(B, dtype=f64, device=dev) if weight is None else weight.to(f64)
+    cm = _tf32.modes(contraction)
+    one = torch.ones((B, 1), dtype=f64, device=dev)
 
     # forward (workloads.deepfm.DeepFMTower): x = [dense | deep of group 0 | ... | deep of group G-1]
     x = torch.cat([dense, deep.permute(1, 0, 2).reshape(B, G * D)], 1)
-    h1 = x @ W1.t() + b1
-    m1 = (h1 > 0).to(f64)
+    if cm["forward"] == "fp32":
+        h1 = x @ W1.t() + b1
+    else:  # the bias is the tile's constant column
+        h1 = _tf32.contract(torch.cat([x, one], 1), torch.cat([W1, b1.unsqueeze(1)], 1).t(), cm["forward"])
+    m1 = (h1 > 0 if dnn_masks is None else dnn_masks[0]).to(f64)
     a1 = h1 * m1
     h2 = a1 @ W2.t() + b2
-    m2 = (h2 > 0).to(f64)
+    m2 = (h2 > 0 if dnn_masks is None else dnn_masks[1]).to(f64)
     a2 = h2 * m2
     dnn = a2 @ w3
     s = deep.sum(0)  # [B, 8]
@@ -178,10 +192,14 @@ def tower_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, we
     dW2 = dh2.t() @ a1
     db2 = dh2.sum(0)
     dh1 = (dh2 @ W2) * m1
-    dW1 = dh1.t() @ x
-    db1 = dh1.sum(0)
+    if cm["weight"] == "fp32":
+        dW1 = dh1.t() @ x
+        db1 = dh1.sum(0)
+    else:
+        dW1b = _tf32.contract(dh1.t(), torch.cat([x, one], 1), cm["weight"])
+        dW1, db1 = dW1b[:, :-1], dW1b[:, -1]
     dwd = dense.t() @ dz
-    dx = dh1 @ W1
+    dx = dh1 @ W1 if cm["data"] == "fp32" else _tf32.contract(dh1, W1, cm["data"])
     ddeep = dx[:, ND:].reshape(B, G, D).permute(1, 0, 2) + dz.view(1, B, 1) * (s.unsqueeze(0) - deep)
     dwide = dz.unsqueeze(0).expand(G, B)
     gsum_deep = _scatter_rows(ddeep, inv, B)
@@ -221,6 +239,20 @@ def tower_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, we
     occ = _scatter_rows(torch.ones((G, B, 1), dtype=f64, device=dev), inv, B).squeeze(2)
     return {"logits": z, "loss": loss, "grads": grads, "gsum_wide": gsum_wide, "gsum_deep": gsum_deep,
             "h1": h1, "h2": h2, "M": M, "n_unique": n_unique.to(device=dev, dtype=torch.int64), "occ": occ}
+
+
+PRECISION_CHECKS = ("forward", "data", "weight")
+
+
+def precision_selection(ref, check):
+    """(family, selection) for tf32.ratio: the elements the mma tower's first-layer contraction `check` feeds --
+    the logits, the live rows of gsum_deep, dW1 and db1."""
+    if check == "forward":
+        return "logits", None
+    if check == "data":
+        return "gsum_deep", _tf32.live_rows(ref, "gsum_deep")
+    o = layout(ref["gsum_wide"].shape[0])
+    return "grads", slice(o["w1"], o["b1"] + H1)
 
 
 def near_relu_kink(ref, tau=1e-4):

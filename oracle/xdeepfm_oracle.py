@@ -25,6 +25,7 @@ import torch
 from oracle.tower_oracle import (  # noqa: F401  (re-exported: the tests use this module as the tower's oracle)
     C_TOL, D, EPS32, FAMILIES, FLT_MIN, H1, H2, ND, P_FLOOR, WD_PAD, _scatter_rows, first_occurrence_inverse,
     near_relu_kink)
+from oracle import tf32 as _tf32
 from oracle import tower_oracle as _T
 
 CIN_H, HALF, NP = 128, 64, 192
@@ -97,9 +98,11 @@ def _split_back(dz, n, H0, Hk, k_order):
     return dz.reshape(n, D, Hk, H0).transpose(2, 3)
 
 
-def _cin_forward(x0, W, mask_override, k_order, swap_halves, magnitudes):
+def _cin_forward(x0, W, mask_override, k_order, swap_halves, magnitudes, cm=None):
     """One chunk: x0 [n, G, D] -> dict with p [n, 192], pre0 / pre1 [n, 128, D], masks, x1 and (magnitudes) their
-    magnitudes."""
+    magnitudes.  cm: tf32.modes; the forward contraction's operands are k_cin_fwd's, A = W_k and B = Z_k formed
+    as the fp32 product X0 X_k."""
+    fwd = _tf32.modes(cm)["forward"]
     W0, b0, W1, b1 = W
     n, G, _ = x0.shape
     out = {}
@@ -107,7 +110,10 @@ def _cin_forward(x0, W, mask_override, k_order, swap_halves, magnitudes):
     direct, mdirect = [], []
     for k, (w, b) in enumerate(((W0, b0), (W1, b1))):
         z = _outer(x0, xk, k_order)
-        pre = (z @ w.t() + b).transpose(1, 2)  # [n, 128, D]
+        if fwd == "fp32":
+            pre = (z @ w.t() + b).transpose(1, 2)  # [n, 128, D]
+        else:
+            pre = _tf32.contract(w, z, fwd, eq="hk,bdk->bhd") + b.view(1, -1, 1)
         mpre = None
         if magnitudes or mask_override is not None:
             mpre = (_outer(x0.abs(), mxk, k_order) @ w.abs().t() + b.abs()).transpose(1, 2)
@@ -137,17 +143,30 @@ def _cin_forward(x0, W, mask_override, k_order, swap_halves, magnitudes):
     return out
 
 
-def _cin_backward(x0, f, dz, W, wex, k_order, swap_halves):
-    """One chunk: d loss / d (x0, W_0, b_0, W_1, b_1) from the forward record f and dz [n] (already weighted)."""
+def _cin_backward(x0, f, dz, W, wex, k_order, swap_halves, cm=None):
+    """One chunk: d loss / d (x0, W_0, b_0, W_1, b_1) from the forward record f and dz [n] (already weighted).
+    cm: tf32.modes, with the operands of csrc/xdeepfm_cin.cu.  Data pass (k_cin_data): A = W_k^T with the direct
+    channels' rows scaled by their w_ex, B = mask ? dz : 0 (direct channels) or dC_0 (X_1's channels).  Weight
+    pass (k_cin_weights): A = dC_0 and B = Z_0 for X_1's channels; else A = the 0/1 mask (exact) and B = dz Z_k,
+    the output scaled by w_ex."""
+    data, wgt = (_tf32.modes(cm)[k] for k in ("data", "weight"))
+    f32 = _tf32.fp32
     W0, b0, W1, b1 = W
     n, G, _ = x0.shape
     x1 = f["x1"]
     lo, hi = (slice(HALF, None), slice(None, HALF)) if swap_halves else (slice(None, HALF), slice(HALF, None))
     dc1 = dz.view(n, 1, 1) * wex[HALF:].view(1, CIN_H, 1) * f["m1"]
     z1 = _outer(x0, f.get("x1_batch", x1), k_order)
-    dW1 = torch.einsum("bhd,bdk->hk", dc1, z1)
+    if wgt == "fp32":
+        dW1 = torch.einsum("bhd,bdk->hk", dc1, z1)
+    else:
+        dW1 = _tf32.contract(f["m1"], f32(dz.view(n, 1, 1) * f32(z1)), wgt, eq="bhd,bdk->hk") * wex[HALF:].view(-1, 1)
     db1 = dc1.sum((0, 2))
-    dZ1 = _split_back(torch.einsum("bhd,hk->bdk", dc1, W1), n, G, HALF, k_order)  # [n, D, G, 64]
+    if data == "fp32":
+        dZ1 = torch.einsum("bhd,hk->bdk", dc1, W1)
+    else:
+        dZ1 = _tf32.contract((W1 * wex[HALF:].view(-1, 1)).t(), dz.view(n, 1, 1) * f["m1"], data, eq="kh,bhd->bdk")
+    dZ1 = _split_back(dZ1, n, G, HALF, k_order)  # [n, D, G, 64]
     dx0 = torch.einsum("bdij,bjd->bid", dZ1, x1)
     dx1 = torch.einsum("bdij,bid->bjd", dZ1, x0)
     dc0 = torch.zeros((n, CIN_H, D), dtype=x0.dtype, device=x0.device)
@@ -155,15 +174,30 @@ def _cin_backward(x0, f, dz, W, wex, k_order, swap_halves):
     dc0[:, hi] = dz.view(n, 1, 1) * wex[:HALF].view(1, HALF, 1)
     dc0 = dc0 * f["m0"]
     z0 = _outer(x0, x0, k_order)
-    dW0 = torch.einsum("bhd,bdk->hk", dc0, z0)
+    if wgt == "fp32":
+        dW0 = torch.einsum("bhd,bdk->hk", dc0, z0)
+    else:
+        dW0 = torch.empty_like(W0)
+        dW0[lo] = _tf32.contract(dc0[:, lo], z0, wgt, eq="bhd,bdk->hk")
+        dW0[hi] = _tf32.contract(f["m0"][:, hi], f32(dz.view(n, 1, 1) * f32(z0)), wgt,
+                                 eq="bhd,bdk->hk") * wex[:HALF].view(-1, 1)
     db0 = dc0.sum((0, 2))
-    dZ0 = _split_back(torch.einsum("bhd,hk->bdk", dc0, W0), n, G, G, k_order)
+    if data == "fp32":
+        dZ0 = torch.einsum("bhd,hk->bdk", dc0, W0)
+    else:
+        scale = torch.ones(CIN_H, dtype=W0.dtype, device=W0.device)
+        scale[hi] = wex[:HALF]
+        b_op = dz.view(n, 1, 1) * f["m0"]
+        b_op[:, lo] = dc0[:, lo]
+        dZ0 = _tf32.contract((W0 * scale.view(-1, 1)).t(), b_op, data, eq="kh,bhd->bdk")
+    dZ0 = _split_back(dZ0, n, G, G, k_order)
     dx0 = dx0 + torch.einsum("bdij,bjd->bid", dZ0, x0) + torch.einsum("bdij,bid->bjd", dZ0, x0)
     return dx0, dW0, db0, dW1, db1
 
 
 def xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, weight=None, mask_override=None,
-                      norm=None, l2=True, magnitudes=True, k_order="ij", swap_halves=False, chunk=1024):
+                      norm=None, l2=True, magnitudes=True, k_order="ij", swap_halves=False, chunk=1024,
+                      contraction=None):
     """Float64 forward + backward of one batch, with the inputs, the optional per-sample weight and the outputs of
     tower_oracle.tower_reference (logits, loss, grads, gsum_wide, gsum_deep, h1, h2, "M", n_unique, occ) plus the
     CIN's pre-activations pre0 / pre1 [B, 128, 8] and their magnitudes (M["pre0"], M["pre1"]), p [B, 192] and the
@@ -171,7 +205,11 @@ def xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, 
     mask_override (m0, m1, tau): bool [B, 128, 8] masks used where |pre| <= tau M_pre.  norm: the batch size the
     loss divides by (default B; a subset of a batch with the full batch's norm gives that subset's share of every
     output, which is how `mutations` models a sample counted differently); l2=False leaves the L2 term out.
-    k_order="ji" and swap_halves are mutations (the K index transposed, the split halves swapped)."""
+    k_order="ji" and swap_halves are mutations (the K index transposed, the split halves swapped).
+    contraction (oracle/tf32.py modes for "forward", "data", "weight"): the CIN's three tensor-core contractions
+    evaluated with the TF32 products of a mode, on the operands the kernels split (_cin_forward, _cin_backward).
+    An emulated run should take the exact run's masks (mask_override with tau = 1), so that its error does not
+    flip a unit.  The magnitude pass is the exact one's."""
     f64 = torch.float64
     G, B = inv.shape
     Bn = B if norm is None else norm
@@ -205,7 +243,7 @@ def xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, 
         mo = None
         if mask_override is not None:
             mo = (mask_override[0][s0:s0 + chunk], mask_override[1][s0:s0 + chunk], mask_override[2])
-        recs.append(_cin_forward(x0_all[s0:s0 + chunk], Wc, mo, k_order, swap_halves, magnitudes))
+        recs.append(_cin_forward(x0_all[s0:s0 + chunk], Wc, mo, k_order, swap_halves, magnitudes, contraction))
     p = torch.cat([r["p"] for r in recs])
     cin = p @ wex + bex[0]
     z = z_wd + cin
@@ -221,7 +259,8 @@ def xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, 
     ddeep = (dh1 @ W1)[:, ND:].reshape(B, G, D)
     grads_cin = [torch.zeros_like(t) for t in Wc]
     for k, s0 in enumerate(range(0, B, chunk)):
-        g = _cin_backward(x0_all[s0:s0 + chunk], recs[k], dz[s0:s0 + chunk], Wc, wex, k_order, swap_halves)
+        g = _cin_backward(x0_all[s0:s0 + chunk], recs[k], dz[s0:s0 + chunk], Wc, wex, k_order, swap_halves,
+                          contraction)
         ddeep[s0:s0 + chunk] += g[0]
         for acc, v in zip(grads_cin, g[1:]):
             acc += v
@@ -277,6 +316,31 @@ def xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, 
         "gsum_wide": _scatter_rows(Mdz.unsqueeze(0).expand(G, B).unsqueeze(2), inv, NR).squeeze(2),
     }
     return out
+
+
+# The elements each CIN contraction feeds, as (family, selection) for tf32.ratio.  The weight pass is two checks:
+# W_0's X_1 channels take A = dC_0 through all three products, every other filter row takes A = the exact 0/1 mask
+# and two products (there a lost lo of A changes nothing, so "2x_no_a_lo" is the kernel itself).
+PRECISION_CHECKS = ("forward", "data", "weight_dc0", "weight_mask")
+CONTRACTION_OF = {"forward": "forward", "data": "data", "weight_dc0": "weight", "weight_mask": "weight"}
+
+
+def precision_selection(ref, check):
+    """(family, selection) of PRECISION_CHECKS' `check` for tf32.ratio."""
+    G = ref["gsum_wide"].shape[0]
+    o = layout(G)
+    if check == "forward":
+        return "logits", None
+    if check == "data":
+        return "gsum_deep", _tf32.live_rows(ref, "gsum_deep")
+    sel = torch.zeros(o["total"], dtype=torch.bool, device=ref["grads"].device)
+    dc0 = slice(o["cin_w0"], o["cin_w0"] + HALF * G * G)
+    if check == "weight_dc0":
+        sel[dc0] = True
+    else:
+        sel[dc0.stop:o["cin_b0"]] = True
+        sel[o["cin_w1"]:o["cin_b1"]] = True
+    return "grads", sel
 
 
 def near_cin_kink(ref, tau=1e-4):

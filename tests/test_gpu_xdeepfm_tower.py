@@ -60,7 +60,15 @@ class XBuffers(Buffers):
                                    device=_dev())
 
 
-def make_inputs(G, B, pattern="zipf", seed=0):
+# Value regimes: Wide & Deep's (test_gpu_wide_deep_tower.py) and the CIN's own.  dead_cin: b_0 = -100 kills every
+# layer-0 channel, so X_1 = 0 and layer 1 sees pre1 = b_1 < 0 (dead too), and b_ex = 0: the CIN adds nothing and
+# the tower is Wide & Deep.  half_dead_cin: b_0[:64] = -100 kills X_1 only, the direct half of layer 0 lives and
+# layer 1's live channels see pre1 = b_1 > 0.  strong_cin: filters 3 times the initializer's and deep rows of
+# scale 1 make the CIN logit dominate, with the Wide & Deep DNN's first layer small (w1_gain 0.1).
+REGIMES = ("base", "large_logit", "dead_l1", "soft", "dead_cin", "half_dead_cin", "strong_cin")
+
+
+def make_inputs(G, B, pattern="zipf", seed=0, regime="base"):
     """Device inputs of one batch in the kernel's layout, conditioned on the DNN's kinks; rows past n_unique[g] and
     the parameters' padding are NaN.  Returns (inputs, float64 reference without a mask override)."""
     dev = _dev()
@@ -68,13 +76,31 @@ def make_inputs(G, B, pattern="zipf", seed=0):
     ids = _ids(pattern, G, B, seed, gen)
     inv, n_unique, _ = X.first_occurrence_inverse(ids)
     sw = 0.5 * (5.0 / max(G, 5)) ** 0.5
+    sd = 1.0 if regime == "strong_cin" else 0.5
     live = torch.arange(B, device=dev).unsqueeze(0) < n_unique.unsqueeze(1).long()
     bet_wide = torch.where(live, torch.randn((G, B), generator=gen, device=dev) * sw, NAN).contiguous()
-    bet_deep = torch.where(live.unsqueeze(2), torch.randn((G, B, X.D), generator=gen, device=dev) * 0.5, NAN)
+    bet_deep = torch.where(live.unsqueeze(2), torch.randn((G, B, X.D), generator=gen, device=dev) * sd, NAN)
     bet_deep = bet_deep.contiguous()
     dense = torch.randn((B, X.ND), generator=gen, device=dev)
-    labels = (torch.rand(B, generator=gen, device=dev) < 0.25).float()
-    params = X.random_params(G, gen, dev, pad=NAN)
+    if regime == "soft":
+        labels = torch.rand(B, generator=gen, device=dev)
+    else:
+        labels = (torch.rand(B, generator=gen, device=dev) < 0.25).float()
+    kw = {}
+    if regime == "large_logit":
+        kw["wd_std"] = 6.0
+    if regime == "dead_l1":
+        kw.update(b1=-100.0, b2=[0.5, -0.5, 0.7, 0.3])
+    if regime == "strong_cin":
+        kw.update(cin_gain=3.0, w1_gain=0.1)
+    params = X.random_params(G, gen, dev, pad=NAN, **kw)
+    o = X.layout(G)
+    if regime == "dead_cin":
+        params[o["cin_b0"]:o["cin_w1"]] = -100.0
+        params[o["cin_b1"]:o["wex"]] = -0.05 - 0.1 * torch.rand(X.CIN_H, generator=gen, device=dev)
+        params[o["bex"]] = 0.0
+    if regime == "half_dead_cin":
+        params[o["cin_b0"]:o["cin_b0"] + X.HALF] = -100.0
     for _ in range(40):
         ref = X.xdeepfm_reference(inv, n_unique, bet_wide, bet_deep, dense, labels, params, chunk=4096)
         near = X.near_relu_kink(ref, TAU)
@@ -83,6 +109,8 @@ def make_inputs(G, B, pattern="zipf", seed=0):
         dense[near] = torch.randn((int(near.sum()), X.ND), generator=gen, device=dev)
     else:
         raise AssertionError("conditioning did not converge")
+    if regime == "large_logit" and B >= 1000:
+        assert float(ref["logits"].abs().max()) > 50
     return (inv, n_unique, bet_wide, bet_deep, dense, labels, params), ref
 
 
@@ -94,7 +122,9 @@ def reference_with_kernel_masks(inputs, ref, scratch, label):
     for k in (0, 1):
         bad = (km[k] != (ref["pre%d" % k] > 0)) & ~near[k]
         assert not bool(bad.any()), "%s: layer %d mask bits wrong at %s" % (label, k, bad.nonzero()[:4].tolist())
-    return X.xdeepfm_reference(*inputs, mask_override=(km[0], km[1], TAU), chunk=4096)
+    ref = X.xdeepfm_reference(*inputs, mask_override=(km[0], km[1], TAU), chunk=4096)
+    ref["kernel_masks"] = km
+    return ref
 
 
 def _call(kind, a):
@@ -114,7 +144,7 @@ def _report():
         print("\nxDeepFM tile tower, largest err / bound per output family (%s, %d SMs):" % (
             torch.cuda.get_device_name(0), _n_sm()))
         for (kind, fam), r in sorted(WORST.items()):
-            print("  %-8s %-10s %.4f" % (kind, fam, r))
+            print("  %-19s %-10s %.4f" % (kind, fam, r))
 
 
 def _outputs(buf):
@@ -122,10 +152,10 @@ def _outputs(buf):
             "gsum_deep": buf.gsum_deep}
 
 
-def run_and_check(kind, G, B, pattern="zipf", seed=0, table_rows=False):
+def run_and_check(kind, G, B, pattern="zipf", seed=0, table_rows=False, regime="base"):
     buf = XBuffers(G, B)
     backward = kind != "forward"
-    inputs, ref = make_inputs(G, B, pattern, seed)
+    inputs, ref = make_inputs(G, B, pattern, seed, regime)
     buf.load(inputs)
     a = buf.args(backward)
     group = None
@@ -146,7 +176,7 @@ def run_and_check(kind, G, B, pattern="zipf", seed=0, table_rows=False):
     finally:
         if group is not None:
             group.close()
-    label = "xdeepfm %s G=%d B=%d %s%s:" % (kind, G, B, pattern, " table" if table_rows else "")
+    label = "xdeepfm %s G=%d B=%d %s/%s%s:" % (kind, G, B, pattern, regime, " table" if table_rows else "")
     if not backward:  # the forward stores no masks: its logits must equal the training call's (the same code)
         return inputs, ref, {f: v.clone() for f, v in _outputs(buf).items()}
     ref = reference_with_kernel_masks(inputs, ref, buf.scratch, label)
@@ -154,7 +184,8 @@ def run_and_check(kind, G, B, pattern="zipf", seed=0, table_rows=False):
     rs = X.check({f: v for f, v in _outputs(buf).items() if f in fams}, ref, families=fams, label=label,
                  n_sm=_n_sm())
     for fam, r in rs.items():
-        WORST[(kind, fam)] = max(WORST.get((kind, fam), 0.0), r)
+        key = kind if regime == "base" else "%s/%s" % (kind, regime)
+        WORST[(key, fam)] = max(WORST.get((key, fam), 0.0), r)
     if backward:
         dead = torch.arange(B, device=_dev()).unsqueeze(0) >= inputs[1].unsqueeze(1).long()
         assert torch.isnan(buf.gsum_wide[dead]).all() and torch.isnan(buf.gsum_deep[dead]).all(), label
@@ -195,6 +226,46 @@ def test_xdeepfm_forward_only(G, B):
     fwd = run_and_check("forward", G, Bn, seed=31)
     one = run_and_check("tile", G, Bn, seed=31)
     assert torch.equal(fwd[2]["logits"], one[2]["logits"])
+
+
+@pytest.mark.parametrize("B", ["1000", "32768"])
+@pytest.mark.parametrize("regime", REGIMES)
+def test_xdeepfm_tower_value_regimes(regime, B):
+    """Every regime within the bound, with the kernel's mask bits equal to pre > 0 outside the tau window; the
+    regimes' exact outputs besides.  dead_l1: Wide & Deep's hidden-layer gradients are 0.  dead_cin: the CIN filter
+    gradients are exactly the prologue's fp32 L2 term 2e-5f W, its bias and w_ex gradients 0, and the logits and
+    row sums are Wide & Deep's within Wide & Deep's (tighter) bound.  half_dead_cin: dW_1 is exactly its L2 term
+    (Z_1 = X0 X_1 = 0).  strong_cin: the CIN logit dominates."""
+    from oracle import wide_deep_oracle as WD
+
+    G, Bn = 38, _batch(B)
+    inputs, ref, got = run_and_check("tile", G, Bn, seed=21, regime=regime)
+    label = "xdeepfm G=%d B=%d %s" % (G, Bn, regime)
+    o = X.layout(G)
+    p, g = inputs[6], got["grads"]
+
+    def l2(a, b):
+        return p[o[a]:o[b]] * torch.tensor(2e-5, dtype=torch.float32, device=p.device)
+
+    if regime == "dead_l1":
+        assert (g[o["w1"]:o["w2"] + X.H2 * X.H1] == 0).all(), label
+    if regime in ("dead_cin", "half_dead_cin"):
+        assert not ref["pre0"][:, :X.HALF].gt(0).any()
+        assert torch.equal(g[o["cin_w1"]:o["cin_b1"]], l2("cin_w1", "cin_b1")), label
+    if regime == "half_dead_cin":
+        assert ref["pre0"][:, X.HALF:].gt(0).any() and ref["pre1"].gt(0).any()
+    if regime == "dead_cin":
+        assert not ref["pre0"].gt(0).any() and not ref["pre1"].gt(0).any()
+        assert torch.equal(g[o["cin_w0"]:o["cin_b0"]], l2("cin_w0", "cin_b0")), label
+        for a, b in (("cin_b0", "cin_w1"), ("cin_b1", "wex"), ("wex", "bex")):
+            assert (g[o[a]:o[b]] == 0).all(), (label, a)
+        wd = WD.wide_deep_reference(*inputs[:6], p[:o["cin_w0"]])
+        fams = ("logits", "gsum_wide", "gsum_deep")
+        rs = WD.check({f: got[f] for f in fams}, wd, families=fams, label=label + " vs Wide & Deep", n_sm=_n_sm())
+        for fam, r in rs.items():
+            WORST[("tile/dead_cin vs W&D", fam)] = max(WORST.get(("tile/dead_cin vs W&D", fam), 0.0), r)
+    if regime == "strong_cin":
+        assert float(ref["cin"].std()) > 3 * float((ref["logits"] - ref["cin"]).std()), label
 
 
 def test_xdeepfm_cin_logit_is_not_hidden():
