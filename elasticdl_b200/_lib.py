@@ -124,6 +124,7 @@ SYMBOLS = {
     "b200ps_push_rows": (_i, [_vp, _segp, _i, _vp]),
     "b200ps_push_dense": (_i, [_vp, _segp, _i, _vp]),
     "b200ps_push_dense_reduce": (_i, [_vp, _i, ctypes.POINTER(_vp), _i, _f, _i, _vp]),
+    "b200ps_push_dense_allreduce": (_i, [_vp, _i, _vp, ctypes.POINTER(_vp), _i, _f, _f, _f, _f, _f, _vp]),
     "b200ps_push_end": (_i, [_vp, _vp, _vp]),
     "b200ps_bump_step": (_i, [_vp, _vp]),
     "b200ps_push_begin_shard": (_i, [_vp, _i, _f, ctypes.POINTER(ctypes.c_int32), _vp]),

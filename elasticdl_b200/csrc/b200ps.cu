@@ -1347,17 +1347,19 @@ int b200ps_push_dense(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* st
   });
 }
 
-int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* grads_dev, int n_replicas, float scale,
-                             int divide, void* stream) {
+static int push_dense_reduce_impl(b200ps_t* ps, int dense_id, const float* const* grads_dev, int n_replicas,
+                                  float scale, int divide, const float* param_dev, const float* adam, void* stream) {
   int rc = ready(ps);
   if (rc) return rc;
   if (dense_id < 0 || dense_id >= (int)ps->tables.size() || !ps->tables[dense_id].is_dense) return fail(B200PS_ENOTFOUND, "not a dense parameter");
   if (n_replicas < 1 || n_replicas > kMaxShards || !grads_dev) return fail(B200PS_EINVAL, "n_replicas out of range");
   if (divide && scale == 0.0f) return fail(B200PS_EINVAL, "divisor is zero");
+  if (param_dev && ps->opt.kind != kSGD && ps->opt.kind != kMomentum && ps->opt.kind != kAdam && ps->opt.kind != kAMSGrad)
+    return fail(B200PS_EINVAL, "the torch allreduce update covers SGD, momentum, Adam and AMSGrad only");
   DeviceGuard g(ps->client_device);
   const Table& t = ps->tables[dense_id];
   ReplicaGrads rg{};
-  bool vec = (t.rows * t.dim) % 4 == 0;
+  bool vec = (t.rows * t.dim) % 4 == 0 && (!param_dev || aligned16(param_dev));
   for (int r = 0; r < n_replicas; ++r) {
     rg.g[r] = grads_dev[r];
     vec = vec && aligned16(grads_dev[r]);
@@ -1365,24 +1367,48 @@ int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* gra
   rg.n = n_replicas;
   rg.scale = scale;
   rg.divide = divide ? 1 : 0;
+  rg.param = param_dev;
+  if (adam) {
+    rg.alpha = adam[0];
+    rg.eps = adam[1];
+    rg.c1 = adam[2];
+    rg.c2 = adam[3];
+  }
   long long numel = t.rows * t.dim;
   GroupView gv = group_view(ps);
   cudaStream_t st = (cudaStream_t)stream;
   OptParams o = ps->opt;
-  const bool twice = (ps->flags & 1u) && o.kind == kAMSGrad;
   int grid = grid_for(ps, vec ? numel / 4 : numel);
-  if (twice) {
-    if (vec) k_push_dense_reduce<kAMSGrad, 4, true><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
-    else k_push_dense_reduce<kAMSGrad, 1, true><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+  if (param_dev) {
+    DISPATCH_OPT(o.kind, {
+      if (vec) k_push_dense_reduce<OPT, 4, false, true><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+      else k_push_dense_reduce<OPT, 1, false, true><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+    });
+  } else if ((ps->flags & 1u) && o.kind == kAMSGrad) {
+    if (vec) k_push_dense_reduce<kAMSGrad, 4, true, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+    else k_push_dense_reduce<kAMSGrad, 1, true, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
   } else {
     DISPATCH_OPT(o.kind, {
-      if (vec) k_push_dense_reduce<OPT, 4, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
-      else k_push_dense_reduce<OPT, 1, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+      if (vec) k_push_dense_reduce<OPT, 4, false, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
+      else k_push_dense_reduce<OPT, 1, false, false><<<grid, 256, 0, st>>>(gv, dense_id, rg, o);
     });
   }
   ps->launches++;
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
+}
+
+int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* grads_dev, int n_replicas, float scale,
+                             int divide, void* stream) {
+  return push_dense_reduce_impl(ps, dense_id, grads_dev, n_replicas, scale, divide, nullptr, nullptr, stream);
+}
+
+int b200ps_push_dense_allreduce(b200ps_t* ps, int dense_id, const float* param_dev, const float* const* grads_dev,
+                                int n_replicas, float scale, float alpha, float epsilon, float one_minus_beta1,
+                                float one_minus_beta2, void* stream) {
+  if (!param_dev) return fail(B200PS_EINVAL, "param_dev is null");
+  const float adam[4] = {alpha, epsilon, one_minus_beta1, one_minus_beta2};
+  return push_dense_reduce_impl(ps, dense_id, grads_dev, n_replicas, scale, 0, param_dev, adam, stream);
 }
 
 static int push_end_impl(b200ps_t* ps, int32_t* versions_out_host, void* stream, int only_shard);

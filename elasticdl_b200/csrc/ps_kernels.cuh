@@ -390,16 +390,30 @@ struct ReplicaGrads {
   int n;
   float scale;
   int divide;  // 1: g = sum / scale (sync-SGD average, servicer.py:207); 0: g = sum * scale (allreduce postscale)
+  // TORCH only: the caller's copy of the parameter (read instead of the PS copy, which is written), and this
+  // step's Adam coefficients from the double hyper-parameters, as torch.optim.Adam has them
+  const float* param;
+  float alpha, eps, c1, c2;
 };
 
-template <int OPT, int VEC, bool TWICE>
+// TORCH (the dense allreduce of a torch optimizer): the parameter is read from rg.param, and Adam's alpha, eps
+// and (1 - beta) come from rg.  Off, the update is kernel_api.cc's: coefficients from k_push_begin and the
+// fp32 betas.
+template <int OPT, int VEC, bool TWICE, bool TORCH = false>
 __device__ __forceinline__ void dense_update_range(const GroupView& gv, const TableView& tv,
-                                                   const ReplicaGrads& rg, const OptParams& o) {
+                                                   const ReplicaGrads& rg, const OptParams& o_in) {
   constexpr int S = opt_slots(OPT);
   const int sh = tv.owner;
-  const float lr = gv.rt->lr[sh], alpha = gv.rt->alpha[sh], l2adj = gv.rt->l2adj[sh];
+  const float lr = gv.rt->lr[sh], alpha = TORCH ? rg.alpha : gv.rt->alpha[sh], l2adj = gv.rt->l2adj[sh];
+  OptParams o = o_in;
+  if (TORCH) {
+    o.epsilon = rg.eps;
+    o.c1 = rg.c1;
+    o.c2 = rg.c2;
+  }
   const long long numel = tv.rows * tv.dim;
   float* P = tv.base[sh];
+  const float* Pin = TORCH ? rg.param : P;
   const long long nvec = numel / VEC;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += stride) {
@@ -411,7 +425,7 @@ __device__ __forceinline__ void dense_update_range(const GroupView& gv, const Ta
         acc.x = add(acc.x, x.x); acc.y = add(acc.y, x.y); acc.z = add(acc.z, x.z); acc.w = add(acc.w, x.w);
       }
       g[0] = acc.x; g[1] = acc.y; g[2] = acc.z; g[3] = acc.w;
-      *reinterpret_cast<float4*>(p) = *reinterpret_cast<const float4*>(P + 4 * i);
+      *reinterpret_cast<float4*>(p) = *reinterpret_cast<const float4*>(Pin + 4 * i);
       if (S > 0) *reinterpret_cast<float4*>(s0) = *reinterpret_cast<const float4*>(P + tv.slot_off[1] + 4 * i);
       if (S > 1) *reinterpret_cast<float4*>(s1) = *reinterpret_cast<const float4*>(P + tv.slot_off[2] + 4 * i);
       if (S > 2) *reinterpret_cast<float4*>(s2) = *reinterpret_cast<const float4*>(P + tv.slot_off[3] + 4 * i);
@@ -419,7 +433,7 @@ __device__ __forceinline__ void dense_update_range(const GroupView& gv, const Ta
       float acc = rg.g[0][i];
       for (int r = 1; r < rg.n; ++r) acc = add(acc, rg.g[r][i]);
       g[0] = acc;
-      p[0] = P[i];
+      p[0] = Pin[i];
       if (S > 0) s0[0] = P[tv.slot_off[1] + i];
       if (S > 1) s1[0] = P[tv.slot_off[2] + i];
       if (S > 2) s2[0] = P[tv.slot_off[3] + i];
@@ -463,9 +477,9 @@ __global__ void __launch_bounds__(256) k_push_dense(GroupView gv, SegBatch sb, O
   else dense_update_range<OPT, 1, TWICE>(gv, tv, rg, o);
 }
 
-template <int OPT, int VEC, bool TWICE>
+template <int OPT, int VEC, bool TWICE, bool TORCH>
 __global__ void __launch_bounds__(256) k_push_dense_reduce(GroupView gv, int table, ReplicaGrads rg, OptParams o) {
-  dense_update_range<OPT, VEC, TWICE>(gv, gv.tables[table], rg, o);
+  dense_update_range<OPT, VEC, TWICE, TORCH>(gv, gv.tables[table], rg, o);
 }
 
 // The reference's own C ABI (go/pkg/kernel/capi/kernel_api.h:10-37) on raw device arrays:

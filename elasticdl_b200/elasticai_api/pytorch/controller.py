@@ -124,9 +124,6 @@ class PyTorchAllReduceController(AllReduceController):
     def broadcast(self):  # controller.py:126-131
         broadcast_parameters(self._model.state_dict(), root_rank=0)
         broadcast_optimizer_state(self._optimizer, root_rank=0)
-        ps = getattr(self._optimizer, "_ps", None)
-        if ps is not None:  # fused mode: the master copy of the parameters lives on the PS shards
-            ps.load_params()
         self.global_completed_batch_num = broadcast_object(self.global_completed_batch_num,
                                                            name="GlobalCompletedBatchNum")
 

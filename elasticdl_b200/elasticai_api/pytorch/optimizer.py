@@ -11,14 +11,29 @@ GPU-first differences from the Horovod original:
     the data path at all.  The flat gradient bucket lives in a peer-mapped RAW buffer of an HBM
     parameter-server group (one shard per rank); the owner of parameter slice s runs ONE kernel that
     reads the N ranks' gradient slices over NVLink, sums, scales and applies the optimizer update in
-    place (b200ps_push_dense_reduce: reduce-scatter + averaging + update fused), then every rank reads
+    place (b200ps_push_dense_allreduce: reduce-scatter + averaging + update fused), then every rank reads
     the updated slices back (b200ps_pull_dense: the all-gather) -- phases ordered by a device-side
-    barrier (b200ps_barrier).  The wrapped optimizer's own step() is not used in this mode; its
-    hyper-parameters (lr incl. schedulers, momentum, nesterov, betas, eps) travel to the kernels.
+    barrier (b200ps_barrier).  The wrapped optimizer's own step() is not used in this mode, but the update
+    is its update within fp32 rounding (tests/test_gpu_fused_allreduce.py checks every step against a float64
+    restatement of torch.optim.SGD / Adam):
+      - Adam / AMSGrad add eps to sqrt(v) / sqrt(1 - beta2^t) and take 1 - beta and the bias corrections from
+        the double hyper-parameters, as torch.optim.Adam does (the PS kernels of kernel_api.cc add eps to sqrt(v)
+        and evaluate 1 - beta from the fp32 betas);
+      - the lr of param_groups[0] travels with every step, so schedulers work, and lr = 0 (a warm-up's first
+        step) applies a zero step while the slots and the Adam step count advance;
+      - momentum, nesterov, dampening, betas, eps, amsgrad, weight_decay and maximize are fixed when the
+        optimizer is built: synchronize() raises ValueError naming the key if one has changed since (e.g.
+        OneCycleLR, which needs cycle_momentum=False here);
+      - the parameters themselves are authoritative: the owner of each slice reads it from its own local
+        parameters, so in-place edits between steps (load_state_dict, clamp_, re-initialisation) are kept.
+        Data-parallel ranks make the same edits, so the owner's copy of each slice stands for every rank's;
+      - the update happens inside synchronize(), so gradients edited between synchronize() and step()
+        (clipping after an explicit synchronize()) are not used.
 Semantics kept: Average / Sum ops, gradient_predivide_factor, backward_passes_per_step,
 fixed_global_batch_size (the averaged gradient is invariant to the world size),
 skip_synchronize(), set_backward_passes_per_step(), the zero_grad()/step() guards.
 """
+import math
 import os
 import warnings
 from contextlib import contextmanager
@@ -54,22 +69,27 @@ class _DevMem(object):
         self._owner = owner
 
 
+# The param-group keys the fused backend is built with; synchronize() refuses a step after one of them changed.
+_FIXED_KEYS = ("momentum", "nesterov", "dampening", "betas", "eps", "amsgrad", "weight_decay", "maximize")
+
+
 def _ps_optimizer_args(opt):
-    """(opt_type, opt_args) of the PS kernels for a torch optimizer, or None if it has no fused form."""
+    """(opt_type, opt_args) of the PS kernels for a torch optimizer, or None if it has no fused form.  The
+    group's learning_rate is 0: the step's lr travels with every call, and a literal lr of 0 must stay 0 (the
+    PS reads lr <= 0 in a call as "use the group's learning_rate")."""
     g = opt.param_groups[0]
     if len(opt.param_groups) != 1 or g.get("weight_decay", 0) != 0:
         return None
     if isinstance(opt, torch.optim.SGD):
         if g.get("dampening", 0) != 0 or g.get("maximize", False):
             return None
-        return "SGD", "learning_rate=%r;momentum=%r;nesterov=%s;" % (float(g["lr"]), float(g["momentum"]),
-                                                                      "true" if g["nesterov"] else "false")
+        return "SGD", "learning_rate=0.0;momentum=%r;nesterov=%s;" % (float(g["momentum"]),
+                                                                       "true" if g["nesterov"] else "false")
     if isinstance(opt, torch.optim.Adam) and not isinstance(opt, torch.optim.AdamW):
         if g.get("maximize", False):
             return None
-        return "Adam", "learning_rate=%r;beta_1=%r;beta_2=%r;epsilon=%r;amsgrad=%s;" % (
-            float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
-            "true" if g.get("amsgrad", False) else "false")
+        return "Adam", "learning_rate=0.0;beta_1=%r;beta_2=%r;epsilon=%r;amsgrad=%s;" % (
+            float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), "true" if g.get("amsgrad", False) else "false")
     return None
 
 
@@ -78,7 +98,7 @@ class _FusedPSBackend(object):
     slice s (and its optimizer slots) on shard s, every rank's flat gradient bucket in a peer-mapped raw
     buffer.  See the module docstring; reference counterpart: optimizer.py:141-168 + the wrapped step."""
 
-    def __init__(self, params, opt_type, opt_args):
+    def __init__(self, params, opt_type, opt_args, betas=(0.0, 0.0), eps=0.0):
         import ctypes
 
         from elasticdl_b200 import _lib
@@ -114,22 +134,14 @@ class _FusedPSBackend(object):
                 off += (k + 3) // 4 * 4
         self.params = params
         self._reduce_ptrs = (ctypes.c_void_p * self.world)(*[q + self.rank * per * 4 for q in self.grad_ptrs])
+        self._own_params = ctypes.c_void_p(self.flat_params[self.rank * per:(self.rank + 1) * per].data_ptr())
+        self._adam = (float(betas[0]), float(betas[1]), float(eps))
+        self.steps = 0  # updates applied: torch.optim.Adam's step count
         self._pull = g.make_segs([(tid, 0, None, None, self.flat_params[s * per:(s + 1) * per])
                                   for s, tid in enumerate(self.slice_ids)])
-        self.load_params()
 
     def _stream(self):
         return self._ct.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
-    def barrier(self):
-        self._check(self._lib.b200ps_barrier(self.group._h, self._stream()))
-
-    def load_params(self):
-        """(Re)initialise the PS master copy of this rank's slice from the local parameters (call after a
-        broadcast; every rank holds the same values then)."""
-        s = self.rank
-        self.group.set_dense([("allreduce/slice_%d" % s, self.flat_params[s * self.per:(s + 1) * self.per])])
-        self.barrier()
 
     def rebind(self):
         off = 0
@@ -146,10 +158,16 @@ class _FusedPSBackend(object):
 
     def reduce_update_gather(self, lr, scale):
         lib, h, st = self._lib, self.group._h, self._stream()
+        # Adam's coefficients of this step in double, as torch.optim.Adam computes them (SGD ignores them)
+        self.steps += 1
+        b1, b2, eps = self._adam
+        bc1, bc2 = 1.0 - b1 ** self.steps, 1.0 - b2 ** self.steps
+        adam = (lr * math.sqrt(bc2) / bc1, eps * math.sqrt(bc2), 1.0 - b1, 1.0 - b2)
         self._check(lib.b200ps_barrier(h, st))                      # every rank's gradients are complete
         self._check(lib.b200ps_push_begin_shard(h, self.rank, float(lr), None, st))
-        self._check(lib.b200ps_push_dense_reduce(h, self.slice_ids[self.rank], self._reduce_ptrs, self.world,
-                                                 float(scale), 0, st))  # reduce + scale + update, one kernel
+        # reduce + scale + update, one kernel; it reads this rank's slice of flat_params and writes the PS copy
+        self._check(lib.b200ps_push_dense_allreduce(h, self.slice_ids[self.rank], self._own_params, self._reduce_ptrs,
+                                                    self.world, float(scale), *adam, st))
         self._check(lib.b200ps_push_end_shard(h, self.rank, st))
         self._check(lib.b200ps_barrier(h, st))                      # every slice is updated
         arr, n = self._pull
@@ -210,7 +228,9 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     raise ValueError("fused=True needs CUDA fp32 parameters on one device, world_size > 1 and an "
                                      "SGD / Adam optimizer without weight decay (one param group)")
             else:
-                self._ps = _FusedPSBackend(ps, *mapped)
+                g = self.param_groups[0]
+                self._ps = _FusedPSBackend(ps, *mapped, betas=g.get("betas", (0.0, 0.0)), eps=g.get("eps", 0.0))
+                self._fixed_hp = {k: g[k] for k in _FIXED_KEYS if k in g}
                 self._buckets[(ps[0].device, torch.float32)] = self._ps.flat_grads
                 return
         groups = {}
@@ -280,6 +300,12 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._rebind_grads()
         scale = self._scale_factor()
         if self._ps is not None:
+            g = self.param_groups[0]
+            for k, v in self._fixed_hp.items():
+                if g.get(k) != v:
+                    raise ValueError("fused=True: param_groups[0][%r] changed from %r to %r after the optimizer was "
+                                     "built; the fused update keeps the value it was built with (only lr may "
+                                     "change: for OneCycleLR pass cycle_momentum=False)" % (k, v, g.get(k)))
             # reduce-scatter + averaging + optimizer update + all-gather on the PS shards: the parameters are
             # already updated when this returns (step() then has nothing left to do)
             self._ps.reduce_update_gather(self.param_groups[0]["lr"], scale)

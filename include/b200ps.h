@@ -221,12 +221,23 @@ int b200ps_push_end_shard(b200ps_t* ps, int shard, void* stream);
 /* ---- the dense allreduce controller's data path (rank-per-GPU groups) ----------------------------
  * Replaces the Horovod collectives of elasticai_api/pytorch/optimizer.py:141-168 + the wrapped optimizer's
  * step: every rank keeps its flat gradient bucket in a RAW buffer that the peers map (CUDA IPC); the owner
- * of parameter slice s runs b200ps_push_dense_reduce with the N peer pointers -- the reduce-scatter, the
+ * of parameter slice s runs b200ps_push_dense_allreduce with the N peer pointers -- the reduce-scatter, the
  * averaging and the in-place optimizer update are ONE kernel that reads the peers' gradients over NVLink --
  * and every rank then reads the updated slices back with b200ps_pull_dense (the all-gather).  b200ps_barrier
  * orders the phases on the device (flags in the peer-mapped shard control blocks; no host round trip, no NCCL).
  * raw_register: a zero-filled allocation of `bytes` on every local shard, exported with the shard; returns its
- * id (shares the table id space).  raw_ptr: its address on `shard` as mapped on the client device. */
+ * id (shares the table id space).  raw_ptr: its address on `shard` as mapped on the client device.
+ * push_dense_allreduce: b200ps_push_dense_reduce with divide = 0 and torch.optim's semantics, for SGD / momentum
+ * / Adam / AMSGrad groups (B200PS_EINVAL otherwise): the parameter is read from param_dev (the caller's copy, so
+ * its edits between steps count) and the updated value written to the PS copy.  Adam takes this step's
+ * coefficients from the caller, evaluated in double from the double hyper-parameters as torch.optim.Adam
+ * does: m = beta1 m + one_minus_beta1 g, v = beta2 v + one_minus_beta2 g^2, p -= alpha m / (sqrt(v) + epsilon)
+ * with alpha = lr sqrt(1 - beta2^t) / (1 - beta1^t) and epsilon = eps sqrt(1 - beta2^t) -- torch adds eps to
+ * sqrt(v) / sqrt(1 - beta2^t).  (kernel_api.cc adds eps to sqrt(v) and evaluates 1 - beta from the fp32
+ * betas, 1.3e-5 off for beta2 = 0.999.)  SGD ignores the four; its lr is b200ps_push_begin_shard's. */
+int b200ps_push_dense_allreduce(b200ps_t* ps, int dense_id, const float* param_dev, const float* const* grads_dev,
+                                int n_replicas, float scale, float alpha, float epsilon, float one_minus_beta1,
+                                float one_minus_beta2, void* stream);
 int b200ps_raw_register(b200ps_t* ps, const char* name, size_t bytes);
 int b200ps_raw_ptr(b200ps_t* ps, int table, int shard, void** ptr, size_t* bytes);
 /* The record slab of a direct-indexed embedding table on `shard`, as mapped on the client device: slot s of
