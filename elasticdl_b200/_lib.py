@@ -224,6 +224,13 @@ FRAPPE_SYMBOLS = {
     "b200_frappe_last_error": (ctypes.c_char_p, []),
     "b200_frappe_launch_count": (_i64, []),
 }
+# include/b200_metrics.h
+METRICS_MAX_THRESHOLDS = 16384  # B200_METRICS_MAX_THRESHOLDS
+METRICS_SYMBOLS = {
+    "b200_metrics_auc_update": (_i, [_vp, _vp, _i64, _vp, ctypes.c_int32, _vp, _vp, _vp]),
+    "b200_metrics_last_error": (ctypes.c_char_p, []),
+    "b200_metrics_launch_count": (_i64, []),
+}
 
 _lib = None
 
@@ -236,7 +243,8 @@ def lib():
         if not os.path.exists(path) or _build._stale():
             path = _build.build()
         handle = ctypes.CDLL(path)
-        for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items()):
+        for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items())\
+                + list(METRICS_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args

@@ -6,13 +6,14 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(CSRC, "libb200ps.so")
 SOURCES = ["b200ps.cu", "deepfm_tower.cu", "deepfm_tower_mma.cu", "deepfm_tower2.cu", "dcn_tower.cu", "xdeepfm_cin.cu",
-           "feature_ids.cu", "census_tower.cu", "frappe_tower.cu"]
+           "feature_ids.cu", "census_tower.cu", "frappe_tower.cu", "eval_metrics.cu"]
 HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "ps_unique.cuh", "deepfm_common.cuh",
            "tile_tower.cuh", "mma_tf32.cuh", "xdeepfm.cuh", os.path.join("..", "..", "include", "b200ps.h"),
            os.path.join("..", "..", "include", "b200_deepfm.h"),
            os.path.join("..", "..", "include", "b200_features.h"),
            os.path.join("..", "..", "include", "b200_census.h"),
-           os.path.join("..", "..", "include", "b200_frappe.h")]
+           os.path.join("..", "..", "include", "b200_frappe.h"),
+           os.path.join("..", "..", "include", "b200_metrics.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",

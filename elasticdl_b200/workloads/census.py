@@ -72,6 +72,14 @@ def initial_params(seed, device):
     return flat
 
 
+def eval_metrics_fn():
+    """The census model's evaluation metrics (model_zoo/census_wide_deep_model/wide_deep_functional_api.py:62-71):
+    accuracy of the LOGITS thresholded at 0.5 (quirk Q12, DESIGN.md section 4) and the AUC of the probabilities."""
+    from elasticdl_b200.common.evaluation_utils import zoo_eval_metrics
+
+    return zoo_eval_metrics(0.5)
+
+
 class CensusTowerCall:
     """The census tower's output buffers and workspace for batch B on `device`, and one launch over them."""
 
@@ -208,6 +216,7 @@ class CensusWideDeepEngine:
         self.push_rows_segs = g.make_segs([(tids[6 + k], GROUP_ROWS[TABLE_GROUP[k]], out["uniq"][k],
                                             t.n_unique[k:k + 1], out["gsum"][k]) for k in range(5)])
         self.zero_versions = [0] * g.n_shards
+        self._eval_tower = None  # evaluate()'s tower buffers (lazy)
         self.graph = None
         self._graph_lr = None
         self.steps = 0
@@ -257,9 +266,30 @@ class CensusWideDeepEngine:
         self.steps += 1
         return out
 
+    def evaluate(self, numeric, strings, labels, metrics):
+        """Forward only from raw rows: pull_dense -> census_transform -> the tower -> metrics.update_evaluation_metrics(
+        {"logits": logits, "probs": sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of eval_metrics_fn()).
+        There is no forward-only census kernel: the tower launch also computes the gradients, which evaluate()
+        discards -- into buffers of its own, so the step's loss and gradients stay as they were -- and pushes
+        nothing.  Returns the logits [B] on the device (overwritten by the next evaluate)."""
+        self._check_batch(numeric, strings, labels)
+        if self._eval_tower is None:
+            self._eval_tower = CensusTowerCall(self.B, self.device)
+        g = self.group
+        with torch.cuda.device(self.device):
+            arr, n = self.pull_segs
+            check(g.lib.b200ps_pull_dense(g._h, arr, n, g._stream()))
+            self.transform(numeric, strings, ids_out=self.ids)
+            self._eval_tower.launch(self.ids, labels, self.flat, self.reference_reshape)
+            logits = self._eval_tower.logits
+            metrics.update_evaluation_metrics({"logits": logits, "probs": torch.sigmoid(logits)}, labels)
+        return logits
+
     def check(self):
-        """Raise PSRangeError (a ValueError) if a step since the last check read an id outside its group (the
-        step used row 0 for it); one device read."""
+        """Raise PSRangeError (a ValueError) if a step or evaluate since the last check read an id outside its
+        group (it used row 0 for it); one device read per tower."""
+        if self._eval_tower is not None:
+            self._eval_tower.check_error()
         self.tower.check_error()
 
     def set_lr(self, lr):

@@ -163,6 +163,14 @@ class XDeepFMTower(WideDeepTower):
 TOWERS = {"deepfm": DeepFMTower, "dcn": DCNTower, "wide_deep": WideDeepTower, "xdeepfm": XDeepFMTower}
 
 
+def eval_metrics_fn():
+    """The dac_ctr models' evaluation metrics (model_zoo/dac_ctr/elasticdl_train.py:51-60): accuracy of the
+    LOGITS thresholded at 0.5 (quirk Q12, DESIGN.md section 4) and the AUC of the probabilities."""
+    from elasticdl_b200.common.evaluation_utils import zoo_eval_metrics
+
+    return zoo_eval_metrics(0.5)
+
+
 def synthetic_batch(batch, seed, device, dist="zipf", zipf_s=1.05, group_rows=GROUP_ROWS):
     """SURVEY.md section 8d config 2: bucket ids uniform, categorical ids Zipf(s) over the
     table's rows (or uniform), dense features N(0,1), labels Bernoulli(0.25).
@@ -982,6 +990,14 @@ class DeepFMPSEngine:
         finally:
             self.__dict__.update(saved)
         return self.logits_buf
+
+    def evaluate(self, ids, dense, labels, metrics):
+        """predict() on one batch, then metrics.update_evaluation_metrics({"logits": logits, "probs":
+        sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of eval_metrics_fn()).  Pushes nothing.  Returns the
+        logits [B] on the device (the buffer predict() returns: the next predict() or step overwrites it)."""
+        logits = self.predict(ids, dense)
+        metrics.update_evaluation_metrics({"logits": logits, "probs": torch.sigmoid(logits)}, labels)
+        return logits
 
     def kernel_report(self, ev, uniq_per_step, opt_slots=2):
         """Average CUDA-event duration and algorithmic GB/s per named PS kernel.

@@ -96,6 +96,15 @@ def synthetic_frappe_batch(B, seed, device, pad_fraction=0.0, zipf_s=1.05):
     return ids.contiguous(), labels
 
 
+def eval_metrics_fn():
+    """The frappe models' evaluation metrics (model_zoo/deepfm_edl_embedding/deepfm_edl_embedding.py:115-124,
+    model_zoo/deepfm_functional_api/deepfm_functional_api.py:128-137): accuracy of logits > 0 and the AUC of the
+    probabilities."""
+    from elasticdl_b200.common.evaluation_utils import zoo_eval_metrics
+
+    return zoo_eval_metrics(0.0)
+
+
 class FrappeTowerCall:
     """The frappe tower's output buffers and workspace for batch B and up to `rows` unique ids on `device`, and
     one launch over them."""
@@ -333,6 +342,18 @@ class FrappeDeepFMEngine:
             self._pull(ids, self.group._stream(), lambda name: None)
             self.tower.launch(ids, self.inv, self.n_unique, self.bet_deep, self.bet_wide, None, self.flat, train=False)
         return self.tower.logits.clone()
+
+    def evaluate(self, ids, labels, metrics):
+        """The forward of predict() on one batch, then metrics.update_evaluation_metrics({"logits": logits,
+        "probs": sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of eval_metrics_fn()).  Pushes nothing.
+        Returns the tower's logits buffer [B] (not a copy: the next step, predict or evaluate overwrites it)."""
+        self._check_batch(ids, labels)
+        with torch.cuda.device(self.device):
+            self._pull(ids, self.group._stream(), lambda name: None)
+            self.tower.launch(ids, self.inv, self.n_unique, self.bet_deep, self.bet_wide, None, self.flat, train=False)
+            logits = self.tower.logits
+            metrics.update_evaluation_metrics({"logits": logits, "probs": torch.sigmoid(logits)}, labels)
+        return logits
 
     def check(self):
         """Raise PSRangeError (a ValueError) if a step since the last check met an id outside [0, input_dim) (the
