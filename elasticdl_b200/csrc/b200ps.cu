@@ -114,6 +114,8 @@ struct b200ps {
   int d_tables_cap = 0;
   bool dirty = true;
   PushRt* d_rt = nullptr;
+  std::vector<float> nadam_sched;  // Nadam: S_t, t = 0..last (nadam_schedule); uploaded to d_nadam
+  float* d_nadam = nullptr;
   unsigned* d_err = nullptr;
   int* d_versions = nullptr;
   unsigned long long* d_count = nullptr;
@@ -158,6 +160,11 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
       {"Adagrad", {"learning_rate", "epsilon"}},
       {"Ftrl", {"learning_rate", "initial_accumulator_value", "l1_regularization_strength",
                 "l2_regularization_strength", "l2_shrinkage_regularization_strength", "beta"}},
+      // the Keras optimizers of the Python PS (optimizer_wrapper.py:116-149), get_config() key names
+      {"RMSprop", {"learning_rate", "rho", "momentum", "epsilon", "centered"}},
+      {"Adadelta", {"learning_rate", "rho", "epsilon"}},
+      {"Adamax", {"learning_rate", "beta_1", "beta_2", "epsilon"}},
+      {"Nadam", {"learning_rate", "beta_1", "beta_2", "epsilon"}},
   };
   auto it = want.find(type);
   if (it == want.end()) return fail(B200PS_EINVAL, "Unknown optimizer type " + type);
@@ -195,6 +202,26 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
   } else if (type == "Adagrad") {
     if (parse_float(kv["epsilon"], &o->epsilon)) return fail(B200PS_EINVAL, "bad Adagrad argument");
     o->kind = kAdagrad;
+  } else if (type == "RMSprop") {
+    bool centered;
+    if (parse_float(kv["rho"], &o->beta1) || parse_float(kv["momentum"], &o->mu) ||
+        parse_float(kv["epsilon"], &o->epsilon) || parse_bool(kv["centered"], &centered))
+      return fail(B200PS_EINVAL, "bad RMSprop argument");
+    const bool mom = o->mu > 0.0f;  // Keras: self._momentum = momentum > 0 (the momentum slot exists only then)
+    o->kind = centered ? (mom ? kRMSpropCenteredMomentum : kRMSpropCentered) : (mom ? kRMSpropMomentum : kRMSprop);
+    o->c1 = (float)(1.0 - (double)o->beta1);  // rho, 1 - rho (OptParams)
+  } else if (type == "Adadelta") {
+    if (parse_float(kv["rho"], &o->beta1) || parse_float(kv["epsilon"], &o->epsilon))
+      return fail(B200PS_EINVAL, "bad Adadelta argument");
+    o->kind = kAdadelta;
+    o->c1 = (float)(1.0 - (double)o->beta1);  // rho, 1 - rho (OptParams)
+  } else if (type == "Adamax" || type == "Nadam") {
+    if (parse_float(kv["beta_1"], &o->beta1) || parse_float(kv["beta_2"], &o->beta2) ||
+        parse_float(kv["epsilon"], &o->epsilon))
+      return fail(B200PS_EINVAL, "bad " + type + " argument");
+    o->kind = type == "Adamax" ? kAdamax : kNadam;
+    o->c1 = (float)(1.0 - (double)o->beta1);
+    o->c2 = (float)(1.0 - (double)o->beta2);
   } else {
     if (parse_float(kv["initial_accumulator_value"], &o->init_accum) ||
         parse_float(kv["l1_regularization_strength"], &o->l1) ||
@@ -204,6 +231,30 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
     o->kind = kFTRL;
   }
   return B200PS_OK;
+}
+
+// Nadam's schedule S_0 = 1, S_t = S_{t-1} * u_t, multiplied in float32 in Keras' order, up to the first t
+// where it stops changing (ps_types.cuh, kNadamMaxSteps).  From there on it never changes again: once 0 it
+// stays 0, and for 0 <= beta_1 <= 1 the factors u_t grow with t and stay below 1, so S * u keeps rounding to S.
+int nadam_schedule(float beta1, std::vector<float>* s) {
+  s->assign(1, 1.0f);
+  for (long long t = 1; t <= kNadamMaxSteps; ++t) {
+    const float prev = s->back(), cur = prev * nadam_u(beta1, t);
+    s->push_back(cur);
+    if (cur == prev && (cur == 0.0f || (beta1 >= 0.0f && beta1 <= 1.0f))) return B200PS_OK;
+  }
+  s->clear();
+  return fail(B200PS_EINVAL, "Nadam: the momentum schedule of beta_1 = " + std::to_string(beta1) +
+                                 " does not settle within " + std::to_string(kNadamMaxSteps) + " steps");
+}
+
+// Copies the host schedule to the client device, where k_push_begin reads it.
+cudaError_t upload_nadam(b200ps_t* ps) {
+  if (ps->opt.kind != kNadam) return cudaSuccess;
+  const size_t bytes = ps->nadam_sched.size() * sizeof(float);
+  cudaError_t e = cudaMalloc(&ps->d_nadam, bytes);
+  if (e == cudaSuccess) e = cudaMemcpy(ps->d_nadam, ps->nadam_sched.data(), bytes, cudaMemcpyHostToDevice);
+  return e;
 }
 
 GroupView group_view(b200ps_t* ps) {
@@ -248,6 +299,8 @@ int ready(b200ps_t* ps) {
   for (int s = 0; s < ps->n_shards; ++s)
     if (!ps->shard[s].attached) return fail(B200PS_ESTATE, "shard " + std::to_string(s) + " is not attached");
   if (ps->dirty) return fail(B200PS_ESTATE, "b200ps_commit() not called after the last registration/import");
+  if (ps->opt.kind < 0 || ps->opt.kind >= kNumOptKinds)  // parse_optimizer sets every kind; DISPATCH_OPT relies on it
+    return fail(B200PS_EINVAL, "unknown optimizer kind " + std::to_string(ps->opt.kind));
   return B200PS_OK;
 }
 
@@ -490,6 +543,8 @@ int b200ps_create(int n_shards, int client_device, const char* opt_type, const c
   OptParams o;
   int rc = parse_optimizer(opt_type, opt_args, &o);
   if (rc) return rc;
+  std::vector<float> sched;
+  if (o.kind == kNadam && (rc = nadam_schedule(o.beta1, &sched))) return rc;
   int ndev = 0;
   CUDA_OK(cudaGetDeviceCount(&ndev));
   if (client_device < 0 || client_device >= ndev) return fail(B200PS_ECUDA, "client device " + std::to_string(client_device) + " not present");
@@ -497,6 +552,7 @@ int b200ps_create(int n_shards, int client_device, const char* opt_type, const c
   ps->n_shards = n_shards;
   ps->client_device = client_device;
   ps->opt = o;
+  ps->nadam_sched = std::move(sched);
   ps->staleness = lr_staleness_modulation;
   ps->flags = flags;
   DeviceGuard g(client_device);
@@ -512,6 +568,7 @@ int b200ps_create(int n_shards, int client_device, const char* opt_type, const c
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_versions, sizeof(int) * kMaxShards);
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_count, 64);
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_state, sizeof(long long) * 3 * kMaxShards);
+  if (e == cudaSuccess) e = upload_nadam(ps);
   if (e != cudaSuccess) {
     delete ps;
     return fail(B200PS_ECUDA, std::string("b200ps_create: ") + cudaGetErrorString(e));
@@ -538,6 +595,7 @@ int b200ps_destroy(b200ps_t* ps) {
   }
   cudaFree(ps->d_tables);
   cudaFree(ps->d_rt);
+  cudaFree(ps->d_nadam);
   cudaFree(ps->d_err);
   cudaFree(ps->d_versions);
   cudaFree(ps->d_count);
@@ -558,6 +616,7 @@ int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
   ps->n_shards = src->n_shards;
   ps->client_device = client_device;
   ps->opt = src->opt;
+  ps->nadam_sched = src->nadam_sched;
   ps->staleness = src->staleness;
   ps->flags = src->flags;
   ps->n_sm = src->n_sm;
@@ -586,6 +645,7 @@ int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_versions, sizeof(int) * kMaxShards);
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_count, 64);
   if (e == cudaSuccess) e = cudaMalloc(&ps->d_state, sizeof(long long) * 3 * kMaxShards);
+  if (e == cudaSuccess) e = upload_nadam(ps);
   if (e != cudaSuccess) {
     delete ps;
     return fail(B200PS_ECUDA, std::string("b200ps_clone_view: ") + cudaGetErrorString(e));
@@ -971,7 +1031,8 @@ static int push_begin_impl(b200ps_t* ps, float lr, const int32_t* mv, void* stre
   DeviceGuard g(ps->client_device);
   VersionsIn v{};
   for (int s = 0; s < ps->n_shards; ++s) v.v[s] = mv ? mv[s] : 0;
-  k_push_begin<<<1, 32, 0, (cudaStream_t)stream>>>(group_view(ps), ps->opt, lr, v, ps->staleness, bump_only, only_shard);
+  k_push_begin<<<1, 32, 0, (cudaStream_t)stream>>>(group_view(ps), ps->opt, lr, v, ps->staleness, bump_only, only_shard,
+                                                    ps->d_nadam, (long long)ps->nadam_sched.size() - 1);
   ps->launches++;
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
@@ -993,8 +1054,17 @@ int b200ps_push_begin_shard(b200ps_t* ps, int shard, float learning_rate, const 
     case kAdam: { constexpr int OPT = kAdam; __VA_ARGS__; } break;         \
     case kAMSGrad: { constexpr int OPT = kAMSGrad; __VA_ARGS__; } break;   \
     case kAdagrad: { constexpr int OPT = kAdagrad; __VA_ARGS__; } break;   \
-    default: { constexpr int OPT = kFTRL; __VA_ARGS__; } break;            \
+    case kFTRL: { constexpr int OPT = kFTRL; __VA_ARGS__; } break;         \
+    case kRMSprop: { constexpr int OPT = kRMSprop; __VA_ARGS__; } break;   \
+    case kRMSpropMomentum: { constexpr int OPT = kRMSpropMomentum; __VA_ARGS__; } break;                 \
+    case kRMSpropCentered: { constexpr int OPT = kRMSpropCentered; __VA_ARGS__; } break;                 \
+    case kRMSpropCenteredMomentum: { constexpr int OPT = kRMSpropCenteredMomentum; __VA_ARGS__; } break; \
+    case kAdadelta: { constexpr int OPT = kAdadelta; __VA_ARGS__; } break; \
+    case kAdamax: { constexpr int OPT = kAdamax; __VA_ARGS__; } break;     \
+    case kNadam: { constexpr int OPT = kNadam; __VA_ARGS__; } break;       \
+    default: break;  /* unreachable: ready() refuses any other kind before a push dispatches */         \
   }
+static_assert(kNumOptKinds == 13, "DISPATCH_OPT has one case per OptKind");
 
 int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream) {
   int rc = ready(ps);

@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(256) k_x_send_upd(const __grid_constant__ XVie
   char* upd = xupd(x, owner, x.me);  // remote, contiguous
   const int lane = threadIdx.x & 31, lane4 = threadIdx.x & 3;
   const unsigned gm = 0xfu << (lane & 28);
-  if (blockIdx.x == 0 && threadIdx.x == 0)  // this push's lr / Adam alpha / l2 for that shard (k_push_begin)
+  if (blockIdx.x == 0 && threadIdx.x == 0)  // this push's lr / Adam alpha / l2 for that shard (k_push_begin; Nadam: nadam_coefs)
     st_word16(&xhdr(x, owner)->updh[x.me], __float_as_int(rt->lr[owner]), __float_as_int(rt->alpha[owner]),
               __float_as_int(rt->l2adj[owner]), epoch);
   const long long stride = (long long)gridDim.x * blockDim.x / 4;

@@ -21,6 +21,7 @@ __device__ __forceinline__ float fsqrt(float a) { return __fsqrt_rn(a); }
 template <int OPT>
 __device__ __forceinline__ void opt_update(float g, float& p, float& s0, float& s1, float& s2,
                                            float lr, float alpha, float l2adj, const OptParams& o) {
+  static_assert(OPT >= 0 && OPT < kNumOptKinds, "opt_update: unknown optimizer kind");
   if (OPT == kSGD) {  // kernel_api.cc:6-14
     p = sub(p, mul(lr, g));
   } else if (OPT == kMomentum) {  // kernel_api.cc:16-38
@@ -46,6 +47,46 @@ __device__ __forceinline__ void opt_update(float g, float& p, float& s0, float& 
     float a = add(s0, mul(g, g));
     s0 = a;
     p = sub(p, fdiv(mul(lr, g), add(fsqrt(a), o.epsilon)));
+  } else if (OPT == kRMSprop || OPT == kRMSpropMomentum || OPT == kRMSpropCentered ||
+             OPT == kRMSpropCenteredMomentum) {
+    // Keras RMSprop, sparse form; slots rms[, momentum][, mg].  momentum = 0: eps outside the square
+    // root (Keras' python ops); momentum > 0: TF SparseApply[Centered]RMSProp, eps inside it (Q13).
+    constexpr bool MOM = OPT == kRMSpropMomentum || OPT == kRMSpropCenteredMomentum;
+    constexpr bool CEN = OPT == kRMSpropCentered || OPT == kRMSpropCenteredMomentum;
+    float rms = add(mul(o.beta1, s0), mul(o.c1, mul(g, g)));
+    s0 = rms;
+    float den = rms;
+    if (CEN) {
+      float& mg_slot = MOM ? s2 : s1;
+      float mg = add(mul(o.beta1, mg_slot), mul(o.c1, g));
+      mg_slot = mg;
+      den = sub(rms, mul(mg, mg));
+    }
+    if (MOM) {
+      float mom = add(mul(o.mu, s1), fdiv(mul(lr, g), fsqrt(add(den, o.epsilon))));
+      s1 = mom;
+      p = sub(p, mom);
+    } else {
+      p = sub(p, fdiv(mul(lr, g), add(fsqrt(den), o.epsilon)));
+    }
+  } else if (OPT == kAdadelta) {  // TF SparseApplyAdadelta; slots accum_grad, accum_var
+    float ag = add(mul(o.beta1, s0), mul(o.c1, mul(g, g)));
+    s0 = ag;
+    float u = mul(fdiv(fsqrt(add(s1, o.epsilon)), fsqrt(add(ag, o.epsilon))), g);
+    p = sub(p, mul(lr, u));
+    s1 = add(mul(o.beta1, s1), mul(o.c1, mul(u, u)));
+  } else if (OPT == kAdamax) {  // Keras Adamax._resource_apply_sparse; alpha = lr/(1-b1^t)
+    float m = add(mul(o.beta1, s0), mul(o.c1, g));
+    float v = fmaxf(mul(o.beta2, s1), fabsf(g));
+    s0 = m;
+    s1 = v;
+    p = sub(p, fdiv(mul(alpha, m), add(v, o.epsilon)));
+  } else if (OPT == kNadam) {  // Keras Nadam with its per-push scalars folded (nadam_coefs)
+    float m = add(mul(o.beta1, s0), mul(o.c1, g));
+    float v = add(mul(o.beta2, s1), mul(o.c2, mul(g, g)));
+    s0 = m;
+    s1 = v;
+    p = sub(p, fdiv(add(mul(lr, g), mul(alpha, m)), add(fsqrt(v), l2adj)));
   } else {  // FTRL: TF ApplyFtrl, lr_power = -0.5 (restated in DESIGN.md; parity unpinned)
     float gs = add(g, mul(mul(2.0f, o.l2s), p));
     float a_new = add(s0, mul(g, g));
@@ -544,12 +585,37 @@ __global__ void __launch_bounds__(256) k_dense_copy(GroupView gv, SegBatch sb, i
 // ---------------------------------------------------------------------------
 // Push control (server.go:176-206, optimizer.go:43-44): one thread per shard.
 // ---------------------------------------------------------------------------
+// Keras Nadam's momentum cache u_t = beta_1 * (1 - 0.5 * 0.96^(0.004 t)), in double, rounded to float32
+// (the float32 value Keras multiplies into its schedule).
+__host__ __device__ __forceinline__ float nadam_u(float beta1, long long t) {
+  return (float)((double)beta1 * (1.0 - 0.5 * pow(0.96, 0.004 * (double)t)));
+}
+
+// Nadam's per-push scalars at step t, folded into the three words every row kernel takes:
+//   p -= lr * mbar / (sqrt(v / (1 - b2^t)) + eps),  mbar = (1 - u_t) g / (1 - S_t) + u_{t+1} m / (1 - S_{t+1})
+// is, multiplied through by sqrt(1 - b2^t),
+//   p -= (cg * g + cm * m) / (sqrt(v) + ce),  cg = lr (1 - u_t) sqrt(1 - b2^t) / (1 - S_t),
+//                                            cm = lr u_{t+1} sqrt(1 - b2^t) / (1 - S_{t+1}),  ce = eps sqrt(1 - b2^t).
+// S_{t+1} = S_t * u_{t+1} is Keras' m_schedule_next.  Each scalar is formed in double and rounded once.
+// sched: S_t for t = 0..last (b200ps.cu nadam_schedule); S_t = sched[min(t, last)].
+__device__ __forceinline__ void nadam_coefs(const OptParams& o, const float* sched, long long last, float lr, long long t,
+                                            float* cg, float* cm, float* ce) {
+  const double ut = nadam_u(o.beta1, t), ut1 = nadam_u(o.beta1, t + 1);
+  const double st = sched[t < last ? t : last];
+  const double st1 = sched[t + 1 < last ? t + 1 : last];
+  const double sb = sqrt(1.0 - pow((double)o.beta2, (double)t));
+  *cg = (float)((double)lr * (1.0 - ut) * sb / (1.0 - st));
+  *cm = (float)((double)lr * ut1 * sb / (1.0 - st1));
+  *ce = (float)((double)o.epsilon * sb);
+}
+
 struct VersionsIn {
   int v[kMaxShards];
 };
 
 __global__ void k_push_begin(GroupView gv, OptParams o, float learning_rate, VersionsIn mv,
-                             int staleness_modulation, int bump_only, int only_shard) {
+                             int staleness_modulation, int bump_only, int only_shard, const float* nadam_sched,
+                             long long nadam_last) {
   int s = threadIdx.x;
   if (s >= gv.n_shards) return;
   if (only_shard >= 0 && s != only_shard) return;  // an ApplyGradients that reaches one shard only
@@ -563,9 +629,17 @@ __global__ void k_push_begin(GroupView gv, OptParams o, float learning_rate, Ver
   PushRt* rt = gv.rt;
   rt->lr[s] = lr;
   rt->step[s] = step;
-  // kernel_api.cc:67: lr *= sqrt(1 - pow(beta2, step)) / (1 - pow(beta1, step)) in double
-  double corr = sqrt(1.0 - pow((double)o.beta2, (double)step)) / (1.0 - pow((double)o.beta1, (double)step));
-  rt->alpha[s] = (float)((double)lr * corr);
+  if (o.kind == kNadam) {
+    nadam_coefs(o, nadam_sched, nadam_last, lr, step, &rt->lr[s], &rt->alpha[s], &rt->l2adj[s]);
+    return;
+  }
+  if (o.kind == kAdamax) {  // Keras Adamax: lr_t = lr / (1 - beta_1^t), power in double, rounded once
+    rt->alpha[s] = (float)((double)lr / (1.0 - pow((double)o.beta1, (double)step)));
+  } else {
+    // kernel_api.cc:67: lr *= sqrt(1 - pow(beta2, step)) / (1 - pow(beta1, step)) in double
+    double corr = sqrt(1.0 - pow((double)o.beta2, (double)step)) / (1.0 - pow((double)o.beta1, (double)step));
+    rt->alpha[s] = (float)((double)lr * corr);
+  }
   rt->l2adj[s] = o.beta != 0.0f ? add(o.l2, fdiv(o.beta, mul(2.0f, lr))) : o.l2;
 }
 

@@ -54,6 +54,18 @@ class PSGroup:
     opt_type / opt_args: exactly what the reference hands the Go PS
     (``-opt_type=Adam -opt_args="learning_rate=0.001;beta_1=0.9;..."``,
     python/common/model_utils.py:227-254, go/pkg/ps/optimizer.go:304-390).
+    Accepted types and keys (every key required, no other key allowed):
+      SGD       learning_rate, momentum, nesterov
+      Adam      learning_rate, beta_1, beta_2, epsilon, amsgrad
+      Adagrad   learning_rate, epsilon
+      Ftrl      learning_rate, initial_accumulator_value, l1_regularization_strength,
+                l2_regularization_strength, l2_shrinkage_regularization_strength, beta
+      RMSprop   learning_rate, rho, momentum, epsilon, centered
+      Adadelta  learning_rate, rho, epsilon
+      Adamax    learning_rate, beta_1, beta_2, epsilon
+      Nadam     learning_rate, beta_1, beta_2, epsilon
+    The last four are the Python PS's Keras optimizers with get_config() key names, applied
+    to the pushed rows only (DESIGN.md section 4).
 
     local_shards: shard ids whose memory this process owns (default: all, the
     single-process layout the reference's own tests use,
