@@ -268,3 +268,11 @@ def check(rc):
     if rc in (EINVAL, EWIDTH):
         raise ValueError("b200ps error %d: %s" % (rc, msg))
     raise PSError(rc, msg)
+
+
+def check_call(rc, name, last_error):
+    """Raise for a non-zero return code of the tower or metrics entry point `name`: ValueError for EINVAL (an
+    argument it refused), RuntimeError otherwise, with the message of its own last_error()."""
+    if rc:
+        msg = last_error().decode("utf-8", "replace")
+        raise (ValueError if rc == EINVAL else RuntimeError)("%s failed (%d): %s" % (name, rc, msg))

@@ -107,10 +107,7 @@ class AUC(Metric):
             rc = self.lib.b200_metrics_auc_update(preds.data_ptr(), labels.data_ptr(), preds.numel(),
                                                   self.thresholds.data_ptr(), T, self.state.data_ptr(),
                                                   self.state[2 * (T + 1):].data_ptr(), ctypes.c_void_p(st))
-        if rc:
-            msg = self.lib.b200_metrics_last_error().decode("utf-8", "replace")
-            raise (ValueError if rc == _lib.EINVAL else RuntimeError)("b200_metrics_auc_update failed (%d): %s"
-                                                                      % (rc, msg))
+        _lib.check_call(rc, "b200_metrics_auc_update", self.lib.b200_metrics_last_error)
 
     def confusion(self):
         """(tp, fp, tn, fn) uint64 [T] and the number of invalid predictions, from one read of the state."""

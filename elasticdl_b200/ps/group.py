@@ -444,6 +444,17 @@ class PSGroup:
     def finish_init(self, shard, version):
         check(self.lib.b200ps_finish_init(self._h, shard, int(version), self._stream()))
 
+    def init_dense(self, named_values):
+        """First writer wins (PushModel, server.go:209-221): for each local shard, in shard order, that no client
+        has initialised yet, set the values of [(name, value)] whose dense parameter it owns, then mark it
+        initialised at version 0 (also when it owns none of them)."""
+        for s in range(self.n_shards):
+            if s in self.local_shards and self.try_init(s):
+                mine = [(n, v) for n, v in named_values if self.dense_owner[n] == s]
+                if mine:
+                    self.set_dense(mine)
+                self.finish_init(s, 0)
+
     def table_size(self, name, shard=None):
         tid = self.lookup(name)[0]
         total = 0

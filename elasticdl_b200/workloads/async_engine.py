@@ -1,0 +1,90 @@
+"""What the fixed-model engines (census, frappe) share: one async worker of a model whose step is a fixed set of
+launches over a flat dense buffer, pushed to the parameter server without model versions, and replayable as one
+CUDA graph over static inputs."""
+import torch
+
+from elasticdl_b200._lib import check
+
+
+def check_tensor(t, name, dtype, shape, device):
+    """ValueError unless `t` is a contiguous `dtype` tensor of `shape` on `device`."""
+    if not (isinstance(t, torch.Tensor) and t.device == device and t.dtype == dtype and tuple(t.shape) == shape
+            and t.is_contiguous()):
+        got = (tuple(t.shape), t.dtype, t.device) if isinstance(t, torch.Tensor) else type(t)
+        raise ValueError("%s must be a contiguous %s tensor of shape %s on %s, not %s"
+                         % (name, dtype, shape, device, got))
+
+
+class AsyncEngine:
+    """The part of one async worker on the parameter-server step that the census and frappe engines share.
+
+    group: an async PSGroup without lr staleness modulation (ValueError otherwise: the captured step carries no
+    pulled versions; the drop-in ParameterServerTrainer covers those modes).  register=False attaches to a
+    group.clone_view(), for another worker thread.
+
+    A subclass sets `inputs`, its step's inputs as [(name, dtype, shape)], `tower` (whose `loss` the step leaves),
+    `push_dense_segs` and `push_rows_segs`, and defines _step(*inputs), which ends in _push()."""
+
+    def __init__(self, group, batch, lr, register):
+        name = type(self).__name__
+        if not getattr(group, "use_async", True):
+            raise ValueError("%s trains async only: a sync-SGD group needs the drop-in trainer" % name)
+        if getattr(group, "lr_staleness_modulation", False):
+            raise ValueError("%s pushes without model versions: a group with lr_staleness_modulation needs the "
+                             "drop-in trainer" % name)
+        self.B = int(batch)
+        if self.B < 1:
+            raise ValueError("batch size must be >= 1, not %d" % self.B)
+        self.group = group if register else group.clone_view()
+        self.device = self.group.device
+        self.lr = float(lr)
+        self.zero_versions = [0] * self.group.n_shards
+        self.graph = None
+        self._graph_lr = None
+        self.steps = 0
+
+    def _check_batch(self, *tensors):
+        """Check a batch, one tensor per declared input, against the declaration."""
+        if len(tensors) != len(self.inputs):
+            raise TypeError("a batch is %d tensors (%s), not %d"
+                            % (len(self.inputs), ", ".join(n for n, _, _ in self.inputs), len(tensors)))
+        for t, (name, dtype, shape) in zip(tensors, self.inputs):
+            check_tensor(t, name, dtype, shape, self.device)
+
+    def _push(self, st):
+        """push_begin -> push_dense -> push_rows -> push_end on stream `st`, with no host read."""
+        g, lib = self.group, self.group.lib
+        g.push_begin(self.lr, self.zero_versions)
+        arr, n = self.push_dense_segs
+        check(lib.b200ps_push_dense(g._h, arr, n, st))
+        arr, n = self.push_rows_segs
+        check(lib.b200ps_push_rows(g._h, arr, n, st))
+        g.push_end(sync=False)
+
+    def set_lr(self, lr):
+        """The learning rate the next pushes carry (the reference's schedule callback sets it per version);
+        the captured graph is re-captured on the next replay."""
+        self.lr = float(lr)
+
+    def capture(self):
+        """Capture one step over static inputs (self.statics, one per declared input) into a CUDA graph on the
+        current stream's device; the learning rate is baked in."""
+        if self.graph is None:
+            self.statics = [torch.zeros(shape, dtype=dtype, device=self.device) for _, dtype, shape in self.inputs]
+        torch.cuda.current_stream(self.device).synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            self._step(*self.statics)
+        self.graph, self._graph_lr = graph, self.lr
+        return graph
+
+    def replay(self, *inputs):
+        """step() through the captured graph (captured now if there is none or the learning rate changed)."""
+        self._check_batch(*inputs)
+        if self.graph is None or self._graph_lr != self.lr:
+            self.capture()
+        for s, t in zip(self.statics, inputs):
+            s.copy_(t)
+        self.graph.replay()
+        self.steps += 1
+        return self.tower.loss.reshape(())

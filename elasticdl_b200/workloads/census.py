@@ -20,6 +20,7 @@ import torch
 from elasticdl_b200 import _lib
 from elasticdl_b200._lib import CensusArgs, check
 from elasticdl_b200.common.hash_utils import string_to_id
+from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor
 from elasticdl_b200.workloads.census_features import ID_GROUP_DIMS, STRING_WIDTH, census_transform
 
 GROUP_ROWS = tuple(ID_GROUP_DIMS[g] for g in ("group1", "group2", "group3"))  # 28, 75, 115
@@ -108,18 +109,9 @@ class CensusTowerCall:
         self.args = a
 
     def check_inputs(self, ids, labels, flat):
-        B, dev = self.B, self.device
-
-        def need(t, name, dtype, shape):
-            if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == dtype
-                    and tuple(t.shape) == shape and t.is_contiguous()):
-                got = (tuple(t.shape), t.dtype, t.device) if isinstance(t, torch.Tensor) else type(t)
-                raise ValueError("%s must be a contiguous %s tensor of shape %s on %s, not %s"
-                                 % (name, dtype, shape, dev, got))
-
-        need(ids, "ids", torch.int32, (12, B))
-        need(labels, "labels", torch.float32, (B,))
-        need(flat, "params", torch.float32, (N_PARAMS,))
+        check_tensor(ids, "ids", torch.int32, (12, self.B), self.device)
+        check_tensor(labels, "labels", torch.float32, (self.B,), self.device)
+        check_tensor(flat, "params", torch.float32, (N_PARAMS,), self.device)
 
     def launch(self, ids, labels, flat, reference_reshape):
         """One tower launch on the current stream (no checks, no host read)."""
@@ -128,9 +120,7 @@ class CensusTowerCall:
         a.reference_reshape = 1 if reference_reshape else 0
         with torch.cuda.device(self.device):
             rc = self.lib.b200_census_tower(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        if rc:
-            msg = self.lib.b200_census_last_error().decode("utf-8", "replace")
-            raise (ValueError if rc == _lib.EINVAL else RuntimeError)("b200_census_tower failed (%d): %s" % (rc, msg))
+        _lib.check_call(rc, "b200_census_tower", self.lib.b200_census_last_error)
 
     def check_error(self):
         """Raise PSRangeError (a ValueError) if a launch since the last check read an id outside its group, and
@@ -164,50 +154,35 @@ def census_tower(ids, labels, flat, reference_reshape=False):
     return call.outputs()
 
 
-class CensusWideDeepEngine:
+class CensusWideDeepEngine(AsyncEngine):
     """One async worker of the census wide & deep model on the parameter-server step.
 
-    group: an async PSGroup without lr staleness modulation (ValueError otherwise: the captured step carries no
-    pulled versions; the drop-in ParameterServerTrainer covers those modes).  register=True registers the eleven
-    parameters and sets their initial values first-writer-wins (as PushModel does); register=False attaches to a
-    group.clone_view() of a group where another engine registered them, for another worker thread.
+    group: an async PSGroup, as AsyncEngine takes it.  register=True registers the eleven parameters and sets their
+    initial values first-writer-wins (as PushModel does); register=False attaches to a group.clone_view() of a
+    group where another engine registered them, for another worker thread.
     step(numeric float32 [4, B], strings uint8 [8, B, 32], labels float32 [B]) runs pull_dense (into the flat
     buffer) -> census_transform -> the tower -> push_begin -> push_dense (MLP) -> push_rows (the five tables'
     touched rows, counts on the device) -> push_end, with no host read, and returns the loss on the device.
     capture() / replay() run the same step as one CUDA graph over static inputs; a new learning rate re-captures."""
 
     def __init__(self, group, batch, lr, reference_reshape=False, seed=0, register=True):
-        if not getattr(group, "use_async", True):
-            raise ValueError("CensusWideDeepEngine trains async only: a sync-SGD group needs the drop-in trainer")
-        if getattr(group, "lr_staleness_modulation", False):
-            raise ValueError("CensusWideDeepEngine pushes without model versions: a group with "
-                             "lr_staleness_modulation needs the drop-in trainer")
-        self.B = int(batch)
-        if self.B < 1:
-            raise ValueError("batch size must be >= 1, not %d" % self.B)
-        self.group = group if register else group.clone_view()
-        g = self.group
-        self.device = g.device
-        self.lr = float(lr)
+        super().__init__(group, batch, lr, register)
+        g, B = self.group, self.B
+        self.inputs = [("numeric", torch.float32, (4, B)), ("strings", torch.uint8, (8, B, STRING_WIDTH)),
+                       ("labels", torch.float32, (B,))]
         self.reference_reshape = bool(reference_reshape)
         self.owner = {n: string_to_id(n, g.n_shards) for n, _ in PARAMS}
         if register:
             for n, s in PARAMS:
                 g.register_dense(n, s, self.owner[n])
             g.commit()
-            init = flat_views(initial_params(seed, self.device))
-            for s in range(g.n_shards):  # first writer wins (PushModel, server.go:209-221)
-                if s in g.local_shards and g.try_init(s):
-                    mine = [(n, init[n]) for n, _ in PARAMS if self.owner[n] == s]
-                    if mine:
-                        g.set_dense(mine)
-                    g.finish_init(s, 0)
+            g.init_dense(flat_views(initial_params(seed, self.device)).items())
         tids = [g.lookup(n)[0] for n, _ in PARAMS]  # PSNotFound when no engine registered them
         self.flat = torch.zeros(N_PARAMS, dtype=torch.float32, device=self.device)
         self.views = flat_views(self.flat)
-        self.ids = torch.zeros((12, self.B), dtype=torch.int32, device=self.device)
+        self.ids = torch.zeros((12, B), dtype=torch.int32, device=self.device)
         self.transform = census_transform(torch.int32, device=self.device)
-        self.tower = CensusTowerCall(self.B, self.device)
+        self.tower = CensusTowerCall(B, self.device)
         t = self.tower
         self.pull_segs = g.make_segs([(tid, 0, None, None, self.views[n]) for tid, (n, _) in zip(tids, PARAMS)])
         self.push_dense_segs = g.make_segs([(tids[i], 0, None, None, t.grads[OFFSETS[n]:OFFSETS[n] + int(np.prod(s))])
@@ -215,26 +190,10 @@ class CensusWideDeepEngine:
         out = t.outputs()
         self.push_rows_segs = g.make_segs([(tids[6 + k], GROUP_ROWS[TABLE_GROUP[k]], out["uniq"][k],
                                             t.n_unique[k:k + 1], out["gsum"][k]) for k in range(5)])
-        self.zero_versions = [0] * g.n_shards
         self._eval_tower = None  # evaluate()'s tower buffers (lazy)
-        self.graph = None
-        self._graph_lr = None
-        self.steps = 0
-
-    # ------------------------------------------------------------------ inputs
-    def _check_batch(self, numeric, strings, labels):
-        B, dev = self.B, self.device
-        for t, name, dtype, shape in ((numeric, "numeric", torch.float32, (4, B)),
-                                      (strings, "strings", torch.uint8, (8, B, STRING_WIDTH)),
-                                      (labels, "labels", torch.float32, (B,))):
-            if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == dtype and tuple(t.shape) == shape
-                    and t.is_contiguous()):
-                got = (tuple(t.shape), t.dtype, t.device) if isinstance(t, torch.Tensor) else type(t)
-                raise ValueError("%s must be a contiguous %s tensor of shape %s on %s, not %s"
-                                 % (name, dtype, shape, dev, got))
 
     # ------------------------------------------------------------------ the step
-    def _step(self, numeric, strings, ids, labels):
+    def _step(self, numeric, strings, labels, ids=None):
         g, lib = self.group, self.group.lib
         with torch.cuda.device(self.device):
             st = g._stream()
@@ -244,25 +203,20 @@ class CensusWideDeepEngine:
                 self.transform(numeric, strings, ids_out=self.ids)
                 ids = self.ids
             self.tower.launch(ids, labels, self.flat, self.reference_reshape)
-            g.push_begin(self.lr, self.zero_versions)
-            arr, n = self.push_dense_segs
-            check(lib.b200ps_push_dense(g._h, arr, n, st))
-            arr, n = self.push_rows_segs
-            check(lib.b200ps_push_rows(g._h, arr, n, st))
-            g.push_end(sync=False)
+            self._push(st)
         return self.tower.loss.reshape(())
 
     def step(self, numeric, strings, labels):
         """One training step from raw rows; returns the loss (device scalar, not synchronised)."""
         self._check_batch(numeric, strings, labels)
-        out = self._step(numeric, strings, None, labels)
+        out = self._step(numeric, strings, labels)
         self.steps += 1
         return out
 
     def step_ids(self, ids, labels):
         """One training step from the ids census_transform(torch.int32) gives: int32 [12, B]."""
         self.tower.check_inputs(ids, labels, self.flat)
-        out = self._step(None, None, ids, labels)
+        out = self._step(None, None, labels, ids)
         self.steps += 1
         return out
 
@@ -291,39 +245,6 @@ class CensusWideDeepEngine:
         if self._eval_tower is not None:
             self._eval_tower.check_error()
         self.tower.check_error()
-
-    def set_lr(self, lr):
-        """The learning rate the next pushes carry (the reference's schedule callback sets it per version);
-        the captured graph is re-captured on the next replay."""
-        self.lr = float(lr)
-
-    # ------------------------------------------------------------------ CUDA graph
-    def capture(self):
-        """Capture one step over static inputs (self.s_numeric, self.s_strings, self.s_labels) into a CUDA graph
-        on the current stream's device; the learning rate is baked in."""
-        dev, B = self.device, self.B
-        if self.graph is None:
-            self.s_numeric = torch.zeros((4, B), dtype=torch.float32, device=dev)
-            self.s_strings = torch.zeros((8, B, STRING_WIDTH), dtype=torch.uint8, device=dev)
-            self.s_labels = torch.zeros(B, dtype=torch.float32, device=dev)
-        torch.cuda.current_stream(dev).synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            self._step(self.s_numeric, self.s_strings, None, self.s_labels)
-        self.graph, self._graph_lr = graph, self.lr
-        return graph
-
-    def replay(self, numeric, strings, labels):
-        """step() through the captured graph (captured now if there is none or the learning rate changed)."""
-        self._check_batch(numeric, strings, labels)
-        if self.graph is None or self._graph_lr != self.lr:
-            self.capture()
-        self.s_numeric.copy_(numeric)
-        self.s_strings.copy_(strings)
-        self.s_labels.copy_(labels)
-        self.graph.replay()
-        self.steps += 1
-        return self.tower.loss.reshape(())
 
 
 class CensusWideDeep(torch.nn.Module):

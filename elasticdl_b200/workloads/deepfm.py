@@ -512,13 +512,7 @@ class DeepFMPSEngine:
                         vals = torch.randn((r, dim), generator=gen, device=dev) * init_std
                     if ids.numel():
                         group.set_rows([(n, ids, vals)])
-        # first-writer-wins dense init (PushModel)
-        for s in range(group.n_shards):
-            if s in group.local_shards and group.try_init(s):
-                mine = [(n, p.detach()) for (n, p) in self.params if string_to_id(n, group.n_shards) == s]
-                if mine:
-                    group.set_dense(mine)
-                group.finish_init(s, 0)
+        group.init_dense([(n, p.detach()) for n, p in self.params])
         # persistent buffers
         f32 = dict(dtype=torch.float32, device=dev)
         import ctypes as _ctb

@@ -22,6 +22,7 @@ import torch
 from elasticdl_b200 import _lib
 from elasticdl_b200._lib import FrappeArgs, check
 from elasticdl_b200.common.hash_utils import string_to_id
+from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor
 
 FIELDS = 10
 DIM = 64
@@ -133,24 +134,16 @@ class FrappeTowerCall:
 
     def check_inputs(self, ids, inv, n_unique, bet_deep, bet_wide, labels, flat):
         B, dev = self.B, self.device
-
-        def need(t, name, dtype, shape):
-            if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == dtype
-                    and tuple(t.shape) == shape and t.is_contiguous()):
-                got = (tuple(t.shape), t.dtype, t.device) if isinstance(t, torch.Tensor) else type(t)
-                raise ValueError("%s must be a contiguous %s tensor of shape %s on %s, not %s"
-                                 % (name, dtype, shape, dev, got))
-
-        need(ids, "ids", torch.int64, (B, FIELDS))
-        need(inv, "inv", torch.int32, (FIELDS * B,))
-        need(n_unique, "n_unique", torch.int32, (1,))
+        check_tensor(ids, "ids", torch.int64, (B, FIELDS), dev)
+        check_tensor(inv, "inv", torch.int32, (FIELDS * B,), dev)
+        check_tensor(n_unique, "n_unique", torch.int32, (1,), dev)
         if not (isinstance(bet_deep, torch.Tensor) and bet_deep.dim() == 2 and bet_deep.shape[0] <= self.rows):
             raise ValueError("bet_deep must be [rows <= %d, 64]" % self.rows)
-        need(bet_deep, "bet_deep", torch.float32, (bet_deep.shape[0], DIM))
-        need(bet_wide, "bet_wide", torch.float32, (bet_deep.shape[0], 1))
+        check_tensor(bet_deep, "bet_deep", torch.float32, (bet_deep.shape[0], DIM), dev)
+        check_tensor(bet_wide, "bet_wide", torch.float32, (bet_deep.shape[0], 1), dev)
         if labels is not None:
-            need(labels, "labels", torch.float32, (B,))
-        need(flat, "params", torch.float32, (N_PARAMS,))
+            check_tensor(labels, "labels", torch.float32, (B,), dev)
+        check_tensor(flat, "params", torch.float32, (N_PARAMS,), dev)
 
     def launch(self, ids, inv, n_unique, bet_deep, bet_wide, labels, flat, train=True):
         """One tower call (two kernels) on the current stream: no checks, no host read."""
@@ -161,9 +154,7 @@ class FrappeTowerCall:
         fn = self.lib.b200_frappe_tower if train else self.lib.b200_frappe_forward
         with torch.cuda.device(self.device):
             rc = fn(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        if rc:
-            msg = self.lib.b200_frappe_last_error().decode("utf-8", "replace")
-            raise (ValueError if rc == _lib.EINVAL else RuntimeError)("%s failed (%d): %s" % (fn.__name__, rc, msg))
+        _lib.check_call(rc, fn.__name__, self.lib.b200_frappe_last_error)
 
     def outputs(self, n):
         """{loss, logits, grads, gsum_deep [n, 64], gsum_wide [n, 1]} (views of the buffers)."""
@@ -183,13 +174,12 @@ def frappe_tower(ids, inv, n_unique, bet_deep, bet_wide, labels, flat, train=Tru
     return call.outputs(rows)
 
 
-class FrappeDeepFMEngine:
+class FrappeDeepFMEngine(AsyncEngine):
     """One async worker of the frappe DeepFM model on the parameter-server step.
 
-    group: an async PSGroup without lr staleness modulation (ValueError otherwise: the captured step carries no
-    pulled versions; the drop-in ParameterServerTrainer covers those modes).  input_dim=None: hashed tables sized
-    for `expected_rows` distinct ids (the group's default when None); input_dim=5383: bounded ids, tables as dense
-    PS parameters.  register=True registers the six parameters and sets the initial values of the dense ones
+    group: an async PSGroup, as AsyncEngine takes it.  input_dim=None: hashed tables sized for `expected_rows`
+    distinct ids (the group's default when None); input_dim=5383: bounded ids, tables as dense PS parameters.
+    register=True registers the six parameters and sets the initial values of the dense ones
     first-writer-wins (as PushModel does); register=False attaches to a group.clone_view() of a group where
     another engine registered them, for another worker thread.
     step(ids int64 [B, 10], labels float32 [B]) runs pull_dense (into the flat buffer) -> dedup of the 10 B ids
@@ -198,21 +188,12 @@ class FrappeDeepFMEngine:
     the same step as one CUDA graph over static inputs; a new learning rate re-captures."""
 
     def __init__(self, group, batch, lr, input_dim=None, seed=0, register=True, expected_rows=None):
-        if not getattr(group, "use_async", True):
-            raise ValueError("FrappeDeepFMEngine trains async only: a sync-SGD group needs the drop-in trainer")
-        if getattr(group, "lr_staleness_modulation", False):
-            raise ValueError("FrappeDeepFMEngine pushes without model versions: a group with "
-                             "lr_staleness_modulation needs the drop-in trainer")
-        self.B = int(batch)
-        if self.B < 1:
-            raise ValueError("batch size must be >= 1, not %d" % self.B)
+        super().__init__(group, batch, lr, register)
         if input_dim is not None and int(input_dim) < 1:
             raise ValueError("input_dim must be None (hashed tables) or >= 1, not %r" % (input_dim,))
+        g, dev, B = self.group, self.device, self.B
+        self.inputs = [("ids", torch.int64, (B, FIELDS)), ("labels", torch.float32, (B,))]
         self.input_dim = None if input_dim is None else int(input_dim)
-        self.group = group if register else group.clone_view()
-        g = self.group
-        self.device = g.device
-        self.lr = float(lr)
         tables = [(DEEP_NAME, DIM), (WIDE_NAME, 1)]
         self.owner = {n: string_to_id(n, g.n_shards) for n, _ in DENSE_PARAMS}
         if self.input_dim is not None:
@@ -230,14 +211,8 @@ class FrappeDeepFMEngine:
             if self.input_dim is not None:
                 for n, dim in tables:
                     init[n] = initial_table(seed, dim, self.device, self.input_dim)
-            for s in range(g.n_shards):  # first writer wins (PushModel, server.go:209-221)
-                if s in g.local_shards and g.try_init(s):
-                    mine = [(n, v) for n, v in init.items() if self.owner[n] == s]
-                    if mine:
-                        g.set_dense(mine)
-                    g.finish_init(s, 0)
+            g.init_dense(init.items())
         self.tids = {n: g.lookup(n)[0] for n in [DEEP_NAME, WIDE_NAME] + DENSE_NAMES}  # PSNotFound if unregistered
-        dev, B = self.device, self.B
         self.rows = FIELDS * B if self.input_dim is None else min(FIELDS * B, self.input_dim)
         self.flat = torch.zeros(N_PARAMS, dtype=torch.float32, device=dev)
         self.views = flat_views(self.flat)
@@ -264,23 +239,6 @@ class FrappeDeepFMEngine:
         self.push_rows_segs = g.make_segs([
             (self.tids[DEEP_NAME], self.rows, self.uniq, self.n_unique, t.gsum_deep),
             (self.tids[WIDE_NAME], self.rows, self.uniq, self.n_unique, t.gsum_wide)])
-        self.zero_versions = [0] * g.n_shards
-        self.graph = None
-        self._graph_lr = None
-        self.steps = 0
-
-    # ------------------------------------------------------------------ inputs
-    def _check_batch(self, ids, labels):
-        B, dev = self.B, self.device
-        checks = [(ids, "ids", torch.int64, (B, FIELDS))]
-        if labels is not None:
-            checks.append((labels, "labels", torch.float32, (B,)))
-        for t, name, dtype, shape in checks:
-            if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == dtype and tuple(t.shape) == shape
-                    and t.is_contiguous()):
-                got = (tuple(t.shape), t.dtype, t.device) if isinstance(t, torch.Tensor) else type(t)
-                raise ValueError("%s must be a contiguous %s tensor of shape %s on %s, not %s"
-                                 % (name, dtype, shape, dev, got))
 
     # ------------------------------------------------------------------ the step
     def _pull(self, ids, st, mark):
@@ -303,8 +261,6 @@ class FrappeDeepFMEngine:
         mark("pull")
 
     def _step(self, ids, labels, ev=None):
-        g, lib = self.group, self.group.lib
-
         def mark(name):  # an event after each part of the step
             if ev is not None:
                 e = torch.cuda.Event(enable_timing=True)
@@ -312,17 +268,12 @@ class FrappeDeepFMEngine:
                 ev.setdefault(name, []).append(e)
 
         with torch.cuda.device(self.device):
-            st = g._stream()
+            st = self.group._stream()
             mark("start")
             self._pull(ids, st, mark)
             self.tower.launch(ids, self.inv, self.n_unique, self.bet_deep, self.bet_wide, labels, self.flat)
             mark("tower")
-            g.push_begin(self.lr, self.zero_versions)
-            arr, n = self.push_dense_segs
-            check(lib.b200ps_push_dense(g._h, arr, n, st))
-            arr, n = self.push_rows_segs
-            check(lib.b200ps_push_rows(g._h, arr, n, st))
-            g.push_end(sync=False)
+            self._push(st)
             mark("push")
         return self.tower.loss.reshape(())
 
@@ -337,7 +288,7 @@ class FrappeDeepFMEngine:
     def predict(self, ids):
         """Logits [B] of the current parameters (pull_dense -> dedup -> pull -> the tower's forward-only
         instance); the pulled rows are not pushed.  Returns a fresh tensor, not synchronised."""
-        self._check_batch(ids, None)
+        check_tensor(ids, *self.inputs[0], self.device)
         with torch.cuda.device(self.device):
             self._pull(ids, self.group._stream(), lambda name: None)
             self.tower.launch(ids, self.inv, self.n_unique, self.bet_deep, self.bet_wide, None, self.flat, train=False)
@@ -359,36 +310,6 @@ class FrappeDeepFMEngine:
         """Raise PSRangeError (a ValueError) if a step since the last check met an id outside [0, input_dim) (the
         step used row 0 for it) or a hashed table ran out of slots; synchronises the device."""
         self.group.check()
-
-    def set_lr(self, lr):
-        """The learning rate the next pushes carry; the captured graph is re-captured on the next replay."""
-        self.lr = float(lr)
-
-    # ------------------------------------------------------------------ CUDA graph
-    def capture(self):
-        """Capture one step over static inputs (self.s_ids, self.s_labels) into a CUDA graph on the current
-        stream's device; the learning rate is baked in."""
-        dev, B = self.device, self.B
-        if self.graph is None:
-            self.s_ids = torch.zeros((B, FIELDS), dtype=torch.int64, device=dev)
-            self.s_labels = torch.zeros(B, dtype=torch.float32, device=dev)
-        torch.cuda.current_stream(dev).synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            self._step(self.s_ids, self.s_labels)
-        self.graph, self._graph_lr = graph, self.lr
-        return graph
-
-    def replay(self, ids, labels):
-        """step() through the captured graph (captured now if there is none or the learning rate changed)."""
-        self._check_batch(ids, labels)
-        if self.graph is None or self._graph_lr != self.lr:
-            self.capture()
-        self.s_ids.copy_(ids)
-        self.s_labels.copy_(labels)
-        self.graph.replay()
-        self.steps += 1
-        return self.tower.loss.reshape(())
 
 
 class FrappeDeepFM(torch.nn.Module):
