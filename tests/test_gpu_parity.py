@@ -872,12 +872,13 @@ def test_unique_many_tiles_lookback_int32_and_negative_ids(k, hi, T, bounded):
     group.close()
 
 
-def _flat_launch_case(opt, n_shards, large):
+def _flat_launch_case(opt, n_shards, large, make_pair=make_pair):
     """ONE b200ps_pull_rows / b200ps_push_rows call over segments of mixed dims, a dense parameter addressed by rows
     (Indexed* kernels, kernel.go:48-55) and device-side live counts (n_dev < n), pushed twice so that the second
     push reads nonzero slots: the flat kernels (csrc/ps_flat.cuh) must equal the oracle bit for bit -- params and
     every slot -- and must not touch rows beyond the live counts.  large: the host-side item bound reaches
-    8 x 6 x 256 x #SM, which selects the instances with two rows in flight per thread (U = 2)."""
+    8 x 6 x 256 x #SM, which selects the instances with two rows in flight per thread (U = 2).  make_pair: the
+    (group, client, oracle client) maker of the optimizer family `opt` belongs to."""
     from elasticdl_b200 import _lib
     from elasticdl_b200.common.hash_utils import string_to_id
 
