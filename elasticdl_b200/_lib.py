@@ -155,6 +155,9 @@ SYMBOLS = {
     "b200ps_bag_prep": (_i, [_vp, _vp, _i, _vp, _i64, _i, _i64, _i64, _i64, _i, _vp, _vp, _sz, _vp]),
     "b200ps_sparse_combine": (_i, [_vp, _vp, _vp, _vp, _sz, _i64, _i64, _i, _i, _vp, _vp]),
     "b200ps_sparse_combine_grad": (_i, [_vp, _vp, _vp, _vp, _sz, _i64, _i64, _i, _i, _i64, _vp, _vp]),
+    "b200ps_sparse_combine_weighted": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i64, _i64, _i, _i, _vp, _vp]),
+    "b200ps_sparse_combine_weighted_grad": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _sz, _i64, _i64, _i, _i, _i64, _vp, _vp,
+                                                 _vp]),
     "b200ps_shard_state": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(_i64), ctypes.POINTER(ctypes.c_int32)]),
     "b200ps_set_shard_state": (_i, [_vp, _i, ctypes.c_int32, _i64, ctypes.c_int32]),
     "b200ps_snapshot_state": (_i, [_vp, _vp, _vp]),

@@ -1924,21 +1924,100 @@ int b200ps_bag_prep(b200ps_t* ps, const void* ids_dev, int ids_are_int32, const 
   return B200PS_OK;
 }
 
-int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, void* ws, size_t ws_bytes,
-                          int64_t B, int64_t nnz, int dim, int combiner, float* out_dev, void* stream) {
+}  // extern "C"
+
+template <bool WT>
+static void launch_combine(int c, int grid, cudaStream_t st, const float* bet, const int32_t* inv, const SparseLayout& L,
+                           int* w, int dim, int combiner, float* out, const float* wt) {
+  if (c == 2) k_sparse_combine<2, WT><<<grid, 256, 0, st>>>(bet, inv, L, w, dim, combiner, out, wt);
+  else if (c == 1) k_sparse_combine<1, WT><<<grid, 256, 0, st>>>(bet, inv, L, w, dim, combiner, out, wt);
+  else k_sparse_combine<0, WT><<<grid, 256, 0, st>>>(bet, inv, L, w, dim, combiner, out, wt);
+}
+
+extern "C" {
+
+static int sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, const float* weights_dev,
+                          bool weighted, void* ws, size_t ws_bytes, int64_t B, int64_t nnz, int dim, int combiner,
+                          float* out_dev, void* stream) {
+  const char* fn = weighted ? "sparse_combine_weighted" : "sparse_combine";
   if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
-  if (combiner < kSpSum || combiner > kSpSqrtn) return fail(B200PS_EINVAL, "sparse_combine: combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
-  if (!bet_dev || !inv_dev || !out_dev) return fail(B200PS_EINVAL, "sparse_combine: null pointer");
+  if (combiner < kSpSum || combiner > kSpSqrtn)
+    return fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+  if (!bet_dev || !inv_dev || !out_dev || (weighted && nnz > 0 && !weights_dev))
+    return fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   const SparseLayout L(B, nnz, dim);
   const int c = dim_class(dim, bet_dev, out_dev);
   const int grid = grid_for(ps, L.PB * 32);
   int* w = (int*)ws;
-  if (c == 2) k_sparse_combine<2><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
-  else if (c == 1) k_sparse_combine<1><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
-  else k_sparse_combine<0><<<grid, 256, 0, st>>>(bet_dev, inv_dev, L, w, dim, combiner, out_dev);
+  if (weighted) launch_combine<true>(c, grid, st, bet_dev, inv_dev, L, w, dim, combiner, out_dev, weights_dev);
+  else launch_combine<false>(c, grid, st, bet_dev, inv_dev, L, w, dim, combiner, out_dev, nullptr);
   count_launch(ps, 1);
+  CUDA_OK(cudaGetLastError());
+  return B200PS_OK;
+}
+
+int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, void* ws, size_t ws_bytes,
+                          int64_t B, int64_t nnz, int dim, int combiner, float* out_dev, void* stream) {
+  return sparse_combine(ps, bet_dev, inv_dev, nullptr, false, ws, ws_bytes, B, nnz, dim, combiner, out_dev, stream);
+}
+
+int b200ps_sparse_combine_weighted(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev,
+                                   const float* weights_dev, void* ws, size_t ws_bytes, int64_t B, int64_t nnz, int dim,
+                                   int combiner, float* out_dev, void* stream) {
+  return sparse_combine(ps, bet_dev, inv_dev, weights_dev, true, ws, ws_bytes, B, nnz, dim, combiner, out_dev, stream);
+}
+
+}  // extern "C"
+
+template <bool WT>
+static void launch_combine_grad(int c, int grid, cudaStream_t st, const float* gout, const int32_t* inv,
+                                const SparseLayout& L, const int* w, int dim, int combiner, float* gbet,
+                                const float* wt) {
+  if (c == 2) k_sparse_combine_grad<2, WT><<<grid, 256, 0, st>>>(gout, inv, L, w, dim, combiner, gbet, wt);
+  else if (c == 1) k_sparse_combine_grad<1, WT><<<grid, 256, 0, st>>>(gout, inv, L, w, dim, combiner, gbet, wt);
+  else k_sparse_combine_grad<0, WT><<<grid, 256, 0, st>>>(gout, inv, L, w, dim, combiner, gbet, wt);
+}
+
+extern "C" {
+
+static int sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev, const float* weights_dev,
+                               bool weighted, const float* bet_dev, const void* ws, size_t ws_bytes, int64_t B,
+                               int64_t nnz, int dim, int combiner, int64_t n_unique, float* gbet_dev,
+                               float* gweights_dev, void* stream) {
+  const char* fn = weighted ? "sparse_combine_weighted_grad" : "sparse_combine_grad";
+  if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
+  if (combiner < kSpSum || combiner > kSpSqrtn)
+    return fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+  if (n_unique < 1 || n_unique > nnz + B)
+    return fail(B200PS_EINVAL, std::string(fn) + ": n_unique outside [1, nnz + B]");
+  if (!gout_dev || !inv_dev || !gbet_dev || (weighted && nnz > 0 && !weights_dev))
+    return fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
+  if (gweights_dev && combiner != kSpSum)
+    return fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient is defined for the sum combiner only");
+  if (gweights_dev && !bet_dev) return fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient needs bet_dev");
+  const SparseLayout L(B, nnz, dim);
+  const int c = dim_class(dim, gout_dev, gbet_dev);
+  const int W = c == 0 ? 1 : 4 * c;
+  if (L.K * (dim / W) > INT32_MAX)  // segment_sum_loop's 32-bit warp key, as in b200ps_segment_sum
+    return fail(B200PS_EINVAL, std::string(fn) + ": (nnz + B) * (dim / " + std::to_string(W) + ") = " +
+                                   std::to_string(L.K * (dim / W)) + " work items, more than INT32_MAX (2147483647)");
+  DeviceGuard g(client_dev(ps));
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_OK(cudaMemsetAsync(gbet_dev, 0, (size_t)n_unique * dim * sizeof(float), st));
+  const int grid = grid_for(ps, L.K * (dim / W));
+  const int* w = (const int*)ws;
+  if (weighted) launch_combine_grad<true>(c, grid, st, gout_dev, inv_dev, L, w, dim, combiner, gbet_dev, weights_dev);
+  else launch_combine_grad<false>(c, grid, st, gout_dev, inv_dev, L, w, dim, combiner, gbet_dev, nullptr);
+  count_launch(ps, 1);
+  if (gweights_dev && nnz > 0) {
+    CUDA_OK(cudaMemsetAsync(gweights_dev, 0, (size_t)nnz * sizeof(float), st));
+    int cl = 1;  // lanes per entry, as the kernel picks them
+    while (cl < dim && cl < 32) cl <<= 1;
+    k_sparse_weight_grad<<<grid_for(ps, L.K * cl), 256, 0, st>>>(bet_dev, inv_dev, gout_dev, L, w, dim, gweights_dev);
+    count_launch(ps, 1);
+  }
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
 }
@@ -1946,28 +2025,16 @@ int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv
 int b200ps_sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev, const void* ws,
                                size_t ws_bytes, int64_t B, int64_t nnz, int dim, int combiner, int64_t n_unique,
                                float* gbet_dev, void* stream) {
-  if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
-  if (combiner < kSpSum || combiner > kSpSqrtn)
-    return fail(B200PS_EINVAL, "sparse_combine_grad: combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
-  if (n_unique < 1 || n_unique > nnz + B) return fail(B200PS_EINVAL, "sparse_combine_grad: n_unique outside [1, nnz + B]");
-  if (!gout_dev || !inv_dev || !gbet_dev) return fail(B200PS_EINVAL, "sparse_combine_grad: null pointer");
-  const SparseLayout L(B, nnz, dim);
-  const int c = dim_class(dim, gout_dev, gbet_dev);
-  const int W = c == 0 ? 1 : 4 * c;
-  if (L.K * (dim / W) > INT32_MAX)  // segment_sum_loop's 32-bit warp key, as in b200ps_segment_sum
-    return fail(B200PS_EINVAL, "sparse_combine_grad: (nnz + B) * (dim / " + std::to_string(W) + ") = " +
-                                   std::to_string(L.K * (dim / W)) + " work items, more than INT32_MAX (2147483647)");
-  DeviceGuard g(client_dev(ps));
-  cudaStream_t st = (cudaStream_t)stream;
-  CUDA_OK(cudaMemsetAsync(gbet_dev, 0, (size_t)n_unique * dim * sizeof(float), st));
-  const int grid = grid_for(ps, L.K * (dim / W));
-  const int* w = (const int*)ws;
-  if (c == 2) k_sparse_combine_grad<2><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
-  else if (c == 1) k_sparse_combine_grad<1><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
-  else k_sparse_combine_grad<0><<<grid, 256, 0, st>>>(gout_dev, inv_dev, L, w, dim, combiner, gbet_dev);
-  count_launch(ps, 1);
-  CUDA_OK(cudaGetLastError());
-  return B200PS_OK;
+  return sparse_combine_grad(ps, gout_dev, inv_dev, nullptr, false, nullptr, ws, ws_bytes, B, nnz, dim, combiner,
+                             n_unique, gbet_dev, nullptr, stream);
+}
+
+int b200ps_sparse_combine_weighted_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev,
+                                        const float* weights_dev, const float* bet_dev, const void* ws, size_t ws_bytes,
+                                        int64_t B, int64_t nnz, int dim, int combiner, int64_t n_unique,
+                                        float* gbet_dev, float* gweights_dev, void* stream) {
+  return sparse_combine_grad(ps, gout_dev, inv_dev, weights_dev, true, bet_dev, ws, ws_bytes, B, nnz, dim, combiner,
+                             n_unique, gbet_dev, gweights_dev, stream);
 }
 
 // ---- state ---------------------------------------------------------------------

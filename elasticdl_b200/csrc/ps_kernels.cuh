@@ -879,7 +879,7 @@ __global__ void __launch_bounds__(256) k_zero(float* p, long long n) {
 }
 
 // ---------------------------------------------------------------------------
-// Pooled lookup of a sparse [B, L] input (safe_embedding_lookup_sparse without weights,
+// Pooled lookup of a sparse [B, L] input (safe_embedding_lookup_sparse, with or without weights,
 // embedding_delegate.py:108-230): prune ids < 0, give each empty row the id 0, combine per row
 // (sum / mean / sqrtn), write 0 for the rows that were empty.
 //
@@ -895,7 +895,14 @@ __global__ void __launch_bounds__(256) k_zero(float* p, long long n) {
 //   tkept[NT], tbase[NT], tlast[NT]   per input tile: kept entries, kept entries before it, last kept index
 //   last[2]     the last filled id (int64), copied into the tail [off[B], K)
 //   rowf[K]     row of each filled entry, -1 for the fill of an empty row and for the tail
+//   srcf[K]     input entry each filled entry came from (coalesced COO order, or the bag input's order), -1 where
+//               rowf is -1: the weighted combine reads weights[srcf[j]], so prep does not depend on the weights
+//   wden[B]     float divisor of each row (sum of weights, or the square root of the sum of their squares), written
+//               by the weighted combine for its backward
+//   wpart[MB]   float partial weight sums of multi-piece rows
 //   part[MB*dim] float partial sums of multi-piece rows
+// srcf, wden and wpart are derived from rowf, K and B rather than stored: the layout is a kernel argument, and a
+// larger one would move the other arguments of every sparse kernel.
 // ---------------------------------------------------------------------------
 constexpr int kSpPiece = 256;  // filled entries one warp sums before a row is split across warps
 constexpr int kSpTile = 1024;  // input entries per block and tile of the prep's count and scatter passes
@@ -924,9 +931,12 @@ struct SparseLayout {
     tlast = up4(tbase + NT);
     last = up4(tlast + NT);
     rowf = up4(last + 2);
-    part = up4(rowf + K);
+    part = up4(wpart() + MB);
     words = up4(part + MB * (long long)dim);
   }
+  __host__ __device__ long long srcf() const { return up4(rowf + K); }
+  __host__ __device__ long long wden() const { return up4(srcf() + K); }
+  __host__ __device__ long long wpart() const { return up4(wden() + B); }
 };
 
 __device__ __forceinline__ int sp_pieces(int cnt) { return ((cnt > 1 ? cnt : 1) + kSpPiece - 1) / kSpPiece; }
@@ -1063,6 +1073,7 @@ __global__ void __launch_bounds__(256) k_sparse_scatter(const long long* rows, c
   __shared__ int s_w[8];
   const int* cnt = ws + L.cnt;
   int* rowf = ws + L.rowf;
+  int* srcf = ws + L.srcf();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (long long t = blockIdx.x; t < L.NT; t += gridDim.x) {
     int base = ws[L.tbase + t];
@@ -1088,6 +1099,7 @@ __global__ void __launch_bounds__(256) k_sparse_scatter(const long long* rows, c
         const long long pos = base + wb + __popc(km & ((1u << lane) - 1)) + ws[L.ebef + r];
         ids_f[pos] = v;
         rowf[pos] = (int)r;
+        srcf[pos] = (int)i;
       }
       base += tot;
       __syncthreads();
@@ -1100,6 +1112,7 @@ __global__ void __launch_bounds__(256) k_sparse_scatter(const long long* rows, c
     if (c == 0) {
       ids_f[o] = 0;
       rowf[o] = -1;
+      srcf[o] = -1;
     }
     for (int p = 0; p < np; ++p) ws[L.prow + po + p] = (int)b;
   }
@@ -1108,6 +1121,7 @@ __global__ void __launch_bounds__(256) k_sparse_scatter(const long long* rows, c
   for (long long j = kf + g; j < L.K; j += stride) {
     ids_f[j] = last;
     rowf[j] = -1;
+    srcf[j] = -1;
   }
 }
 
@@ -1126,6 +1140,7 @@ __global__ void __launch_bounds__(kSpScanThreads) k_bag_prep(const V* __restrict
   const long long B = L.B, nnz = L.nnz;
   int* cnt = ws + L.cnt;
   int* rowf = ws + L.rowf;
+  int* srcf = ws + L.srcf();
   int bad = 0;
   if (offs) {
     const long long n_off = B + include_last;
@@ -1172,12 +1187,14 @@ __global__ void __launch_bounds__(kSpScanThreads) k_bag_prep(const V* __restrict
       if (c == 0) {
         ids_f[o] = 0;
         rowf[o] = -1;
+        srcf[o] = -1;
       } else {
         int q = o;
         for (long long j = s; j < e; ++j) {
           const long long v = (long long)vals[j];
           if (v >= 0 && v != pad) {
             ids_f[q] = v;
+            srcf[q] = (int)j;
             rowf[q++] = (int)b;
             last = v;
           }
@@ -1201,14 +1218,17 @@ __global__ void __launch_bounds__(kSpScanThreads) k_bag_prep(const V* __restrict
   for (long long j = carry.x + threadIdx.x; j < L.K; j += blockDim.x) {
     ids_f[j] = last;
     rowf[j] = -1;
+    srcf[j] = -1;
   }
 }
 
-template <int VPT>
-__device__ __forceinline__ void sp_scale_store(float* o, const float* x, int cnt, int combiner) {
+// Scales a row's sum by its divisor d and stores it; 0 for an empty row.  Unweighted, d is the kept count (mean) or its
+// square root (sqrtn); weighted, the caller passes the weight sum (or the square root of the sum of squares) in wd.
+template <int VPT, bool WT = false>
+__device__ __forceinline__ void sp_scale_store(float* o, const float* x, int cnt, int combiner, float wd = 0.f) {
   constexpr int W = VPT == 0 ? 1 : 4 * VPT;
   float y[W];
-  const float d = combiner == kSpMean ? (float)cnt : fsqrt((float)cnt);
+  const float d = WT ? wd : combiner == kSpMean ? (float)cnt : fsqrt((float)cnt);
 #pragma unroll
   for (int e = 0; e < W; ++e) y[e] = cnt == 0 ? 0.f : combiner == kSpSum ? x[e] : fdiv(x[e], d);
   if (VPT == 0) o[0] = y[0];
@@ -1224,9 +1244,13 @@ __device__ __forceinline__ void sp_scale_store(float* o, const float* x, int cnt
 // stored; the pieces of a longer row store partials and the last piece to finish adds them in piece order and resets
 // the row's arrival counter, so the combine can run again on the same workspace.  Every order is fixed, so two calls
 // give the same bits; it is not strict entry order (see b200ps_sparse_combine).
-template <int VPT>
+// WT (weighted): entry j adds wt[srcf[j]] * bet[inv[j]], and for mean / sqrtn each lane also sums its entries' weights
+// (or their squares) in the same order, through the same butterfly and, for a multi-piece row, the same piece-order
+// partials; the row's divisor goes to wden for the backward.
+template <int VPT, bool WT = false>
 __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict__ bet, const int* __restrict__ inv,
-                                                        SparseLayout L, int* ws, int dim, int combiner, float* out) {
+                                                        SparseLayout L, int* ws, int dim, int combiner, float* out,
+                                                        const float* __restrict__ wt = nullptr) {
   constexpr int W = VPT == 0 ? 1 : 4 * VPT;
   const int chunks = dim / W;
   int CL = 1;
@@ -1235,6 +1259,10 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
   const int lane = threadIdx.x & 31;
   const int* off = ws + L.off;
   float* part = reinterpret_cast<float*>(ws + L.part);
+  const int* srcf = ws + L.srcf();
+  float* wden = reinterpret_cast<float*>(ws + L.wden());
+  float* wpart = reinterpret_cast<float*>(ws + L.wpart());
+  const bool wdiv = WT && combiner != kSpSum;
   const long long npieces = ws[L.poff + L.B];
   const long long nwarps = (long long)gridDim.x * blockDim.x / 32;
   for (long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < npieces; w += nwarps) {
@@ -1242,6 +1270,17 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
     const int po = ws[L.poff + row], np = ws[L.poff + row + 1] - po, p = (int)(w - po);
     const int cnt = ws[L.cnt + row];
     const int s = off[row] + p * kSpPiece, e_end = min(s + kSpPiece, off[row + 1]);
+    float wsum = 0.f;
+    if (wdiv) {
+      for (int j = s + lane / CL; j < e_end; j += E) {
+        const int sf = srcf[j];
+        const float x = sf < 0 ? 0.f : __ldg(wt + sf);
+        wsum = add(wsum, combiner == kSpMean ? x : mul(x, x));
+      }
+      for (int o = CL; o < 32; o <<= 1) wsum = add(wsum, __shfl_xor_sync(0xffffffffu, wsum, o));
+    }
+    const float d1 = combiner == kSpMean ? wsum : fsqrt(wsum);
+    if (wdiv && np == 1 && lane == 0) wden[row] = d1;
     for (int cb = 0; cb < chunks; cb += CL) {
       const int c = cb + (lane & (CL - 1));
       const bool cok = c < chunks;
@@ -1251,7 +1290,19 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
       if (cok) {
         for (int j = s + lane / CL; j < e_end; j += E) {
           const float* src = bet + (long long)inv[j] * dim + c * W;
-          if (VPT == 0) acc[0] = add(acc[0], __ldg(src));
+          if (WT) {
+            const int sf = srcf[j];
+            const float wj = sf < 0 ? 0.f : __ldg(wt + sf);
+            if (VPT == 0) acc[0] = add(acc[0], mul(wj, __ldg(src)));
+            else {
+#pragma unroll
+              for (int v = 0; v < VPT; ++v) {
+                const float4 x = __ldg(reinterpret_cast<const float4*>(src + 4 * v));
+                acc[4 * v] = add(acc[4 * v], mul(wj, x.x)); acc[4 * v + 1] = add(acc[4 * v + 1], mul(wj, x.y));
+                acc[4 * v + 2] = add(acc[4 * v + 2], mul(wj, x.z)); acc[4 * v + 3] = add(acc[4 * v + 3], mul(wj, x.w));
+              }
+            }
+          } else if (VPT == 0) acc[0] = add(acc[0], __ldg(src));
           else {
 #pragma unroll
             for (int v = 0; v < VPT; ++v) {
@@ -1267,7 +1318,7 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
         for (int e = 0; e < W; ++e) acc[e] = add(acc[e], __shfl_xor_sync(0xffffffffu, acc[e], o));
       }
       if (cok && lane < CL) {
-        if (np == 1) sp_scale_store<VPT>(out + (long long)row * dim + c * W, acc, cnt, combiner);
+        if (np == 1) sp_scale_store<VPT, WT>(out + (long long)row * dim + c * W, acc, cnt, combiner, d1);
         else {
           float* dst = part + ((long long)ws[L.moff + row] + p) * dim + c * W;
 #pragma unroll
@@ -1276,6 +1327,7 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
       }
     }
     if (np > 1) {
+      if (wdiv && lane == 0) wpart[ws[L.moff + row] + p] = wsum;
       __threadfence();
       __syncwarp();
       int done = 0;
@@ -1285,6 +1337,13 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
         __threadfence();
         if (lane == 0) ws[L.arrive + row] = 0;  // all np pieces have arrived: nothing else touches the counter
         const float* P = part + (long long)ws[L.moff + row] * dim;
+        float d = 0.f;
+        if (wdiv) {
+          float t = 0.f;
+          for (int q = 0; q < np; ++q) t = add(t, __ldcg(wpart + ws[L.moff + row] + q));
+          d = combiner == kSpMean ? t : fsqrt(t);
+          if (lane == 0) wden[row] = d;
+        }
         for (int c = lane; c < chunks; c += 32) {
           float acc[W];
 #pragma unroll
@@ -1293,7 +1352,7 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
 #pragma unroll
             for (int e = 0; e < W; ++e) acc[e] = add(acc[e], __ldcg(P + (long long)q * dim + c * W + e));
           }
-          sp_scale_store<VPT>(out + (long long)row * dim + c * W, acc, cnt, combiner);
+          sp_scale_store<VPT, WT>(out + (long long)row * dim + c * W, acc, cnt, combiner, d);
         }
       }
     }
@@ -1302,18 +1361,31 @@ __global__ void __launch_bounds__(256) k_sparse_combine(const float* __restrict_
 
 // Combine backward load: entry j of the filled stream contributes s_row * gout[row, :] when it belongs to a non-empty
 // row (rowf >= 0); the division is the one torch's autograd of out / counts (out / counts.sqrt()) performs.
-template <int VPT>
+// WT: (gout[row, :] * w_j) / wden[row] (no division for sum), so unit weights give the unweighted bits.
+template <int VPT, bool WT = false>
 struct SparseGradLoad {
   const float* G;
   const int* rowf;
   const int* cnt;
   int dim, combiner;
+  const float* wt;
+  const int* srcf;
+  const float* wden;
   __device__ __forceinline__ bool live(long long j) const { return rowf[j] >= 0; }
   __device__ __forceinline__ void load(long long j, int c, float* x) const {
+    constexpr int W = VPT == 0 ? 1 : 4 * VPT;
     const int r = rowf[j];
     RowsLoad<VPT>{G, dim}.load(r, c, x);
-    if (combiner != kSpSum) {
-      constexpr int W = VPT == 0 ? 1 : 4 * VPT;
+    if (WT) {
+      const float wj = wt[srcf[j]];
+#pragma unroll
+      for (int e = 0; e < W; ++e) x[e] = mul(x[e], wj);
+      if (combiner != kSpSum) {
+        const float d = wden[r];
+#pragma unroll
+        for (int e = 0; e < W; ++e) x[e] = fdiv(x[e], d);
+      }
+    } else if (combiner != kSpSum) {
       const int n = cnt[r];
       const float d = combiner == kSpMean ? (float)n : fsqrt((float)n);
 #pragma unroll
@@ -1322,11 +1394,42 @@ struct SparseGradLoad {
   }
 };
 
-template <int VPT>
+template <int VPT, bool WT = false>
 __global__ void __launch_bounds__(256) k_sparse_combine_grad(const float* gout, const int* inv, SparseLayout L,
-                                                             const int* ws, int dim, int combiner, float* gbet) {
-  const SparseGradLoad<VPT> ld{gout, ws + L.rowf, ws + L.cnt, dim, combiner};
+                                                             const int* ws, int dim, int combiner, float* gbet,
+                                                             const float* wt = nullptr) {
+  const SparseGradLoad<VPT, WT> ld{gout, ws + L.rowf, ws + L.cnt, dim, combiner, wt, ws + L.srcf(),
+                                   reinterpret_cast<const float*>(ws + L.wden())};
   segment_sum_loop<VPT>(ld, inv, L.K, dim, gbet);
+}
+
+// Weight gradient of the weighted sum: gw[srcf[j]] = dot(bet[inv[j]], gout[row_j]) for every kept entry j.  CL lanes
+// (a power of two >= min(dim, 32)) take one entry, each summing its columns c = lane, lane + CL, ... in order, then
+// adding through a fixed xor butterfly.  An input entry appears at most once in the stream, so there are no atomics;
+// the entries prep dropped keep the zero the caller wrote.
+__global__ void __launch_bounds__(256) k_sparse_weight_grad(const float* __restrict__ bet, const int* __restrict__ inv,
+                                                            const float* __restrict__ gout, SparseLayout L,
+                                                            const int* ws, int dim, float* gw) {
+  int CL = 1;
+  while (CL < dim && CL < 32) CL <<= 1;
+  const int E = 32 / CL;
+  const int lane = threadIdx.x & 31;
+  const int* rowf = ws + L.rowf;
+  const int* srcf = ws + L.srcf();
+  const long long kf = ws[L.off + L.B];  // filled entries; past them the tail, rowf = -1
+  const long long nwarps = (long long)gridDim.x * blockDim.x / 32;
+  for (long long j0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / 32 * E; j0 < kf; j0 += nwarps * E) {
+    const long long j = j0 + lane / CL;
+    const int r = j < kf ? rowf[j] : -1;
+    float acc = 0.f;
+    if (r >= 0) {
+      const float* e = bet + (long long)inv[j] * dim;
+      const float* g = gout + (long long)r * dim;
+      for (int c = lane & (CL - 1); c < dim; c += CL) acc = add(acc, mul(__ldg(e + c), __ldg(g + c)));
+    }
+    for (int o = 1; o < CL; o <<= 1) acc = add(acc, __shfl_xor_sync(0xffffffffu, acc, o));
+    if (r >= 0 && (lane & (CL - 1)) == 0) gw[srcf[j]] = acc;
+  }
 }
 
 }  // namespace b200ps_impl

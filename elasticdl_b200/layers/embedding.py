@@ -4,7 +4,7 @@ Public surface of elasticdl/python/elasticdl/layers/embedding.py:20-162 and the
 EmbeddingDelegate it wraps (embedding_delegate.py:26-310): same constructor
 arguments, `set_lookup_embedding_func`, `set_tape`, `reset`, `embedding_and_ids`,
 `embedding_weight_name`, `set_embedding_weight_name`; dense and sparse (combiner
-sum / mean / sqrtn) inputs.
+sum / mean / sqrtn) inputs, the sparse ones optionally weighted (`sparse_weights`).
 
 Differences that follow from torch (documented in DESIGN.md):
   * there is no GradientTape: `set_tape(x)` with a truthy x makes the layer
@@ -118,11 +118,16 @@ class Embedding(torch.nn.Module):
         return bet
 
     def _unique_and_pull(self, flat_ids, dropped=None):
+        """dropped: int32 device counts checked once n_unique is read -- [0] entries whose row lies outside the batch,
+        [1] (when given) weight indices that differ from the ids' -- in one copy to the host."""
         uniq, inv, n = ops.unique(flat_ids, 1)
         u = int(n.item())  # exact BET shape, as the reference exposes it
-        if dropped is not None and int(dropped.item()):  # the stream is idle after n.item(): a 4-byte copy
-            raise ValueError("sparse input has %d entries whose row index is outside [0, batch_size)"
-                             % int(dropped.item()))
+        if dropped is not None:
+            bad = dropped.tolist()  # the stream is idle after n.item(): one small copy
+            if bad[0]:
+                raise ValueError("sparse input has %d entries whose row index is outside [0, batch_size)" % bad[0])
+            if len(bad) > 1 and bad[1]:
+                raise ValueError("sparse_weights must have the indices of sparse_ids; %d of them differ" % bad[1])
         unique_ids = uniq[:u]
         bet = self._gather_embedding_vectors(unique_ids)
         if self.tape:
@@ -130,14 +135,16 @@ class Embedding(torch.nn.Module):
             self._embedding_and_ids.append(EmbeddingAndIds(bet, unique_ids))
         return bet, inv
 
-    def forward(self, ids):
+    def forward(self, ids, sparse_weights=None):
+        if sparse_weights is not None and not (isinstance(ids, torch.Tensor) and ids.is_sparse):
+            raise ValueError("sparse_weights need sparse ids (a COO tensor with the same indices)")
         self._inputs_seen.append(ids)
         if self._prefetched is not None and self._prefetched[0] is ids:
             rows = self._prefetched[1]  # looked up with every other layer of the model before the forward pass
             self._prefetched = None
             return rows.reshape(tuple(ids.shape) + (self.output_dim,))
         if isinstance(ids, torch.Tensor) and ids.is_sparse:
-            return self._sparse_input_call(ids)
+            return self._sparse_input_call(ids, sparse_weights)
         ids = torch.as_tensor(ids)
         if not ids.is_cuda:
             raise RuntimeError("Embedding input must live on the GPU (no CPU path)")
@@ -150,18 +157,34 @@ class Embedding(torch.nn.Module):
 
     call = forward
 
-    def _sparse_input_call(self, sparse_input):
+    def _sparse_input_call(self, sparse_input, sparse_weights=None):
         if self.combiner not in ["sum", "mean", "sqrtn"]:
             raise ValueError("combiner must set sum, mean or sqrtn for sparse input")
-        return self.safe_embedding_lookup_sparse(sparse_input, combiner=self.combiner)
+        if sparse_weights is None:
+            return self.safe_embedding_lookup_sparse(sparse_input, combiner=self.combiner)
+        return self.safe_embedding_lookup_sparse(sparse_input, sparse_weights, combiner=self.combiner)
 
-    def safe_embedding_lookup_sparse(self, sparse_ids, combiner="mean"):
-        """embedding_delegate.py:108-230 without weights: prune ids < 0, give empty rows
-        id 0, combine per row, then zero the rows that were empty (ops.sparse_prep and
-        ops.SparseCombine: CUDA kernels from the coalesced COO to the [batch, dim] output)."""
+    def safe_embedding_lookup_sparse(self, sparse_ids, sparse_weights=None, combiner="mean"):
+        """embedding_delegate.py:108-230: prune ids < 0, give empty rows id 0, combine per row, then zero the rows
+        that were empty (ops.sparse_prep and ops.SparseCombine: CUDA kernels from the coalesced COO to the [batch, dim]
+        output).  sparse_weights: a COO tensor with the indices of sparse_ids, cast to float32 (:141-142); a weight is
+        pruned with its id, and mean / sqrtn divide by the row's weight sum / the square root of its sum of squares
+        (DESIGN.md §4, Q14)."""
         sp = sparse_ids.coalesce()
         batch = sp.shape[0]
         nnz = sp.values().numel()
         ids, ws = ops.sparse_prep(sp.indices()[0], sp.values(), batch, self.output_dim)
-        bet, inv = self._unique_and_pull(ids, dropped=ws[:4].view(torch.int32))
-        return ops.SparseCombine.apply(bet, inv, ws, batch, nnz, combiner, self.output_dim)
+        checks = ws[:4].view(torch.int32)
+        weights = None
+        if sparse_weights is not None:
+            if not (isinstance(sparse_weights, torch.Tensor) and sparse_weights.is_sparse):
+                raise ValueError("sparse_weights must be a sparse COO tensor with the indices of sparse_ids")
+            sw = sparse_weights.coalesce()
+            if tuple(sw.shape) != tuple(sp.shape) or sw.values().numel() != nnz:
+                raise ValueError("sparse_weights of shape %s with %d entries for sparse_ids of shape %s with %d"
+                                 % (tuple(sw.shape), sw.values().numel(), tuple(sp.shape), nnz))
+            weights = sw.values().to(torch.float32)
+            mismatched = (sw.indices() != sp.indices()).any(0).sum().to(torch.int32).view(1)
+            checks = torch.cat([checks, mismatched])
+        bet, inv = self._unique_and_pull(ids, dropped=checks)
+        return ops.SparseCombine.apply(bet, inv, ws, batch, nnz, combiner, self.output_dim, weights)

@@ -139,32 +139,62 @@ def bag_prep(group, input, offsets, dim, include_last_offset=False, padding_idx=
 class SparseCombine(torch.autograd.Function):
     """BET [U, dim] -> [batch, dim]: each row's BET rows summed, scaled by the combiner, 0 for the rows that were
     empty (sparse_segment_{sum,mean,sqrt_n}); backward = the scaled segment sum into [U, dim].  dim is the one
-    sparse_prep sized `ws` for."""
+    sparse_prep sized `ws` for.
+
+    weights (optional): float32 [nnz] in input-entry order (the coalesced COO's values, or the bag input's): row b is
+    sum w_j e_j, divided by sum w_j (mean) or sqrt(sum w_j^2) (sqrtn).  Weights that require grad get the gradient of
+    the sum combiner (0 for the entries prep dropped); under mean and sqrtn they are data, as in the reference's
+    weighted feature columns, and weights that require grad raise ValueError."""
 
     @staticmethod
-    def forward(ctx, bet, inv, ws, batch, nnz, combiner, dim):
+    def forward(ctx, bet, inv, ws, batch, nnz, combiner, dim, weights=None):
         bet = bet.contiguous()
         if bet.dim() != 2 or bet.shape[1] != dim:
             raise ValueError("the lookup returned rows of shape %s, the layer needs [n_unique, %d]"
                              % (tuple(bet.shape), dim))
-        ctx.save_for_backward(inv, ws)
-        ctx.shape = (batch, nnz, dim, COMBINERS[combiner], bet.shape[0])
+        comb = COMBINERS[combiner]
+        lib = _lib.lib()
         out = torch.empty((batch, dim), dtype=torch.float32, device=bet.device)
+        if weights is None:
+            ctx.save_for_backward(inv, ws)
+        else:
+            if ctx.needs_input_grad[7] and combiner != "sum":
+                raise ValueError("weights that require grad need the sum combiner (under %s they are data)" % combiner)
+            _need_cuda(weights, "weights")
+            if weights.numel() != nnz:
+                raise ValueError("%d weights for %d input entries" % (weights.numel(), nnz))
+            weights = weights.detach().reshape(-1).to(torch.float32).contiguous()
+            ctx.save_for_backward(inv, ws, weights, bet if ctx.needs_input_grad[7] else None)
+        ctx.shape = (batch, nnz, dim, comb, bet.shape[0])
         with torch.cuda.device(bet.device):
-            check(_lib.lib().b200ps_sparse_combine(None, bet.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(), batch,
-                                                   nnz, dim, COMBINERS[combiner], out.data_ptr(), _stream(bet.device)))
+            if weights is None:
+                check(lib.b200ps_sparse_combine(None, bet.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(), batch,
+                                                nnz, dim, comb, out.data_ptr(), _stream(bet.device)))
+            else:
+                check(lib.b200ps_sparse_combine_weighted(None, bet.data_ptr(), inv.data_ptr(), weights.data_ptr(),
+                                                         ws.data_ptr(), ws.numel(), batch, nnz, dim, comb,
+                                                         out.data_ptr(), _stream(bet.device)))
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        inv, ws = ctx.saved_tensors
+        inv, ws, *wsaved = ctx.saved_tensors
         batch, nnz, dim, comb, u = ctx.shape
         g = grad_out.contiguous()
         gbet = torch.empty((u, dim), dtype=torch.float32, device=g.device)
+        lib = _lib.lib()
         with torch.cuda.device(g.device):
-            check(_lib.lib().b200ps_sparse_combine_grad(None, g.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                        batch, nnz, dim, comb, u, gbet.data_ptr(), _stream(g.device)))
-        return gbet, None, None, None, None, None, None
+            if not wsaved:
+                check(lib.b200ps_sparse_combine_grad(None, g.data_ptr(), inv.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                     batch, nnz, dim, comb, u, gbet.data_ptr(), _stream(g.device)))
+                return gbet, None, None, None, None, None, None, None
+            weights, bet = wsaved
+            gw = torch.empty(nnz, dtype=torch.float32, device=g.device) if bet is not None else None
+            check(lib.b200ps_sparse_combine_weighted_grad(
+                None, g.data_ptr(), inv.data_ptr(), weights.data_ptr(), bet.data_ptr() if bet is not None else None,
+                ws.data_ptr(), ws.numel(), batch, nnz, dim, comb, u, gbet.data_ptr(),
+                gw.data_ptr() if gw is not None else None, _stream(g.device)))
+        return gbet, None, None, None, None, None, None, gw
 
 
 class GatherRows(torch.autograd.Function):

@@ -359,6 +359,23 @@ int b200ps_sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv
 int b200ps_sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev, const void* workspace_dev,
                                size_t workspace_bytes, int64_t B, int64_t nnz, int dim, int combiner, int64_t n_unique,
                                float* gbet_dev, void* stream);
+/* The weighted lookup (safe_embedding_lookup_sparse with sparse_weights, nn.EmbeddingBag's per_sample_weights):
+ * weights_dev float32 [nnz] in input-entry order (the coalesced COO's, or the bag input's), read through the entry
+ * order prep records, so one prep serves weighted and unweighted combines.  out[b, :] = sum w_j bet[inv[j], :] over
+ * row b's kept entries, divided by sum w_j (mean) or sqrtf(sum w_j^2) (sqrtn); each divisor is summed in the row's
+ * order, so two calls give the same bits; an empty row gives 0, a non-empty row whose divisor is 0 divides by 0 in IEEE
+ * arithmetic.  Unit weights give the bits of b200ps_sparse_combine.  The combine stores each row's divisor in the
+ * workspace, and the grad of mean / sqrtn reads it: run the grad after the weighted combine of the same weights. */
+int b200ps_sparse_combine_weighted(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev,
+                                   const float* weights_dev, void* workspace_dev, size_t workspace_bytes, int64_t B,
+                                   int64_t nnz, int dim, int combiner, float* out_dev, void* stream);
+/* Its backward: gbet[inv[j], :] += gout[row(j), :] * w_j / d_row (no division for sum).  gweights_dev (nullable,
+ * float32 [nnz], sum combiner only; refused otherwise) receives dot(bet[inv[j], :], gout[row(j), :]) for each kept
+ * input entry and 0 for every dropped one; bet_dev is needed with it. */
+int b200ps_sparse_combine_weighted_grad(b200ps_t* ps, const float* gout_dev, const int32_t* inv_dev,
+                                        const float* weights_dev, const float* bet_dev, const void* workspace_dev,
+                                        size_t workspace_bytes, int64_t B, int64_t nnz, int dim, int combiner,
+                                        int64_t n_unique, float* gbet_dev, float* gweights_dev, void* stream);
 
 /* ---- state queries (synchronous on the client device) ---------------- */
 int b200ps_shard_state(b200ps_t* ps, int shard, int32_t* version, int64_t* step, int32_t* initialized);
