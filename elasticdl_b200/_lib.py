@@ -76,6 +76,20 @@ class FrappeArgs(ctypes.Structure):  # b200_frappe_args_t (include/b200_frappe.h
     ]
 
 
+LR_MAX_BOUNDARIES = 32  # B200PS_LR_MAX_BOUNDARIES
+LR_PIECEWISE, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_POLYNOMIAL = 1, 2, 3, 4
+
+
+class LrSchedule(ctypes.Structure):  # b200ps_lr_schedule_t (include/b200ps.h)
+    _fields_ = [
+        ("kind", ctypes.c_int32), ("n_boundaries", ctypes.c_int32), ("staircase", ctypes.c_int32),
+        ("cycle", ctypes.c_int32),
+        ("initial_learning_rate", ctypes.c_double), ("decay_steps", ctypes.c_double), ("decay_rate", ctypes.c_double),
+        ("end_learning_rate", ctypes.c_double), ("power", ctypes.c_double),
+        ("boundaries", ctypes.c_double * LR_MAX_BOUNDARIES), ("values", ctypes.c_float * (LR_MAX_BOUNDARIES + 1)),
+    ]
+
+
 class PSError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("b200ps error %d: %s" % (code, msg))
@@ -121,6 +135,7 @@ SYMBOLS = {
     "b200ps_slot_rows": (_i, [_vp, _i, _i, _segp, _i, _vp]),
     "b200ps_slot_dense": (_i, [_vp, _i, _i, _segp, _i, _vp]),
     "b200ps_push_begin": (_i, [_vp, _f, ctypes.POINTER(ctypes.c_int32), _vp]),
+    "b200ps_set_lr_schedule": (_i, [_vp, ctypes.POINTER(LrSchedule)]),
     "b200ps_push_rows": (_i, [_vp, _segp, _i, _vp]),
     "b200ps_push_dense": (_i, [_vp, _segp, _i, _vp]),
     "b200ps_push_dense_reduce": (_i, [_vp, _i, ctypes.POINTER(_vp), _i, _f, _i, _vp]),

@@ -116,6 +116,7 @@ struct b200ps {
   PushRt* d_rt = nullptr;
   std::vector<float> nadam_sched;  // Nadam: S_t, t = 0..last (nadam_schedule); uploaded to d_nadam
   float* d_nadam = nullptr;
+  b200ps_lr_schedule_t lr_sched{};  // kind 0: none (b200ps_set_lr_schedule); per view, not copied by clone_view
   unsigned* d_err = nullptr;
   int* d_versions = nullptr;
   unsigned long long* d_count = nullptr;
@@ -1031,8 +1032,10 @@ static int push_begin_impl(b200ps_t* ps, float lr, const int32_t* mv, void* stre
   DeviceGuard g(ps->client_device);
   VersionsIn v{};
   for (int s = 0; s < ps->n_shards; ++s) v.v[s] = mv ? mv[s] : 0;
+  static_assert(kMaxShards <= 32, "k_push_begin runs one warp");
   k_push_begin<<<1, 32, 0, (cudaStream_t)stream>>>(group_view(ps), ps->opt, lr, v, ps->staleness, bump_only, only_shard,
-                                                    ps->d_nadam, (long long)ps->nadam_sched.size() - 1);
+                                                    ps->d_nadam, (long long)ps->nadam_sched.size() - 1,
+                                                    bump_only ? b200ps_lr_schedule_t{} : ps->lr_sched);
   ps->launches++;
   CUDA_OK(cudaGetLastError());
   return B200PS_OK;
@@ -1041,6 +1044,35 @@ static int push_begin_impl(b200ps_t* ps, float lr, const int32_t* mv, void* stre
 int b200ps_push_begin(b200ps_t* ps, float learning_rate, const int32_t* model_versions, void* stream) {
   return push_begin_impl(ps, learning_rate, model_versions, stream, 0);
 }
+int b200ps_set_lr_schedule(b200ps_t* ps, const b200ps_lr_schedule_t* s) {
+  if (!ps) return fail(B200PS_EINVAL, "null group");
+  if (!s) {
+    ps->lr_sched = b200ps_lr_schedule_t{};
+    return B200PS_OK;
+  }
+  if (s->kind < B200PS_LR_PIECEWISE || s->kind > B200PS_LR_POLYNOMIAL)
+    return fail(B200PS_EINVAL, "unknown learning-rate schedule kind " + std::to_string(s->kind));
+  if (s->kind == B200PS_LR_PIECEWISE) {
+    if (s->n_boundaries < 0 || s->n_boundaries > B200PS_LR_MAX_BOUNDARIES)
+      return fail(B200PS_EINVAL, "PiecewiseConstantDecay takes 0 to " + std::to_string(B200PS_LR_MAX_BOUNDARIES) +
+                                     " boundaries, not " + std::to_string(s->n_boundaries));
+    for (int i = 0; i < s->n_boundaries; ++i) {
+      if (!std::isfinite(s->boundaries[i])) return fail(B200PS_EINVAL, "PiecewiseConstantDecay: a boundary is not finite");
+      if (i > 0 && !(s->boundaries[i] > s->boundaries[i - 1]))
+        return fail(B200PS_EINVAL, "PiecewiseConstantDecay: boundaries must be strictly increasing");
+    }
+    for (int i = 0; i <= s->n_boundaries; ++i)
+      if (!std::isfinite(s->values[i])) return fail(B200PS_EINVAL, "PiecewiseConstantDecay: a value is not finite");
+  } else {
+    const double p[] = {s->initial_learning_rate, s->decay_steps, s->decay_rate, s->end_learning_rate, s->power};
+    for (double x : p)
+      if (!std::isfinite(x)) return fail(B200PS_EINVAL, "learning-rate schedule: a parameter is not finite");
+    if (!(s->decay_steps > 0)) return fail(B200PS_EINVAL, "learning-rate schedule: decay_steps must be > 0");
+  }
+  ps->lr_sched = *s;
+  return B200PS_OK;
+}
+
 int b200ps_bump_step(b200ps_t* ps, void* stream) { return push_begin_impl(ps, 0.f, nullptr, stream, 1); }
 int b200ps_push_begin_shard(b200ps_t* ps, int shard, float learning_rate, const int32_t* model_versions, void* stream) {
   if (shard < 0) return fail(B200PS_EINVAL, "bad shard id");

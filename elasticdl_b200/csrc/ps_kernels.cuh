@@ -613,10 +613,35 @@ struct VersionsIn {
   int v[kMaxShards];
 };
 
+// The learning-rate schedule of b200ps_lr_schedule_t at x, in double (include/b200ps.h gives the formulas).
+__device__ __forceinline__ double lr_schedule_at(const b200ps_lr_schedule_t& sc, double x) {
+  if (sc.kind == B200PS_LR_PIECEWISE) {
+    int i = 0;
+    while (i < sc.n_boundaries && x > sc.boundaries[i]) ++i;
+    return sc.values[i];
+  }
+  if (sc.kind == B200PS_LR_POLYNOMIAL) {
+    double s = fmin(x, sc.decay_steps), d = sc.decay_steps;
+    if (sc.cycle) s = x, d = sc.decay_steps * fmax(1.0, ceil(x / sc.decay_steps));
+    return (sc.initial_learning_rate - sc.end_learning_rate) * pow(1.0 - s / d, sc.power) + sc.end_learning_rate;
+  }
+  double p = x / sc.decay_steps;
+  if (sc.staircase) p = floor(p);
+  return sc.kind == B200PS_LR_EXPONENTIAL ? sc.initial_learning_rate * pow(sc.decay_rate, p)
+                                          : sc.initial_learning_rate / (1.0 + sc.decay_rate * p);
+}
+
+// sched.kind == 0: no schedule, the lr is `learning_rate` (the request's).  Otherwise the schedule's value at
+// max_s(version_s) - 1 (clamped at 0) replaces it; every lane reads every shard's version before any returns.
 __global__ void k_push_begin(GroupView gv, OptParams o, float learning_rate, VersionsIn mv,
                              int staleness_modulation, int bump_only, int only_shard, const float* nadam_sched,
-                             long long nadam_last) {
+                             long long nadam_last, b200ps_lr_schedule_t sched) {
   int s = threadIdx.x;
+  if (sched.kind != 0) {  // block-uniform; the launch is one warp (kMaxShards <= 32)
+    int v = s < gv.n_shards ? *(volatile int*)&gv.ctl[s]->version : 0;
+    int vmax = __reduce_max_sync(0xffffffffu, v);
+    learning_rate = (float)lr_schedule_at(sched, (double)(vmax > 0 ? vmax - 1 : 0));
+  }
   if (s >= gv.n_shards) return;
   if (only_shard >= 0 && s != only_shard) return;  // an ApplyGradients that reaches one shard only
   ShardCtl* ctl = gv.ctl[s];

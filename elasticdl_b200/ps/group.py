@@ -113,6 +113,7 @@ class PSGroup:
         self._pinned_state = torch.empty(3 * _lib.MAX_SHARDS, dtype=torch.int64).pin_memory()
         self._pinned_versions = torch.empty(_lib.MAX_SHARDS, dtype=torch.int32).pin_memory()
         self._ws = None
+        self.lr_schedule = None  # set_lr_schedule
         if len(self.local_shards) == self.n_shards:
             check(self.lib.b200ps_commit(self._h))
 
@@ -143,6 +144,7 @@ class PSGroup:
         view._h = h
         view.device = dev
         view.local_shards = []  # owns no memory
+        view.lr_schedule = None
         view.tables = dict(self.tables)
         view._owner = self  # keep the owner alive
         view._pinned_state = torch.empty(3 * _lib.MAX_SHARDS, dtype=torch.int64).pin_memory()
@@ -346,6 +348,17 @@ class PSGroup:
     def push_begin(self, learning_rate, model_versions):
         mv = (ctypes.c_int32 * _lib.MAX_SHARDS)(*[int(v) for v in model_versions])
         check(self.lib.b200ps_push_begin(self._h, float(learning_rate), mv, self._stream()))
+
+    def set_lr_schedule(self, schedule):
+        """Evaluate `schedule` (an elasticdl_b200.callbacks.LearningRateSchedule) on the device at every push of
+        this view from now on, in place of the learning rate the push carries; None removes it.  The schedule
+        belongs to this view (one worker): clone_view() starts without one.  A CUDA graph captured before keeps
+        the schedule it captured.  ValueError on a sync-SGD group."""
+        if schedule is not None and not self.use_async:
+            raise ValueError("a device learning-rate schedule needs an async group: sync-SGD applies buffered "
+                             "gradients with the pushes' own learning rate")
+        check(self.lib.b200ps_set_lr_schedule(self._h, None if schedule is None else ctypes.byref(schedule.struct())))
+        self.lr_schedule = schedule
 
     def bump_step(self):
         check(self.lib.b200ps_bump_step(self._h, self._stream()))

@@ -317,7 +317,10 @@ class ParameterServerTrainer(object):
             if not (isinstance(v, torch.Tensor) and v.is_cuda and not v.is_sparse):
                 return None
             sig.append((k, tuple(v.shape), v.dtype, v.device.index))
-        return (type(features).__name__, tuple(sig), float(self._optimizer.param_groups[0]["lr"]))
+        # a schedule the push evaluates on the device is part of the captured launch; the host's lr is not used
+        sched = getattr(self._ps_client.group, "lr_schedule", None)
+        lr = float(self._optimizer.param_groups[0]["lr"]) if sched is None else ("lr_schedule", sched.key())
+        return (type(features).__name__, tuple(sig), lr)
 
     @staticmethod
     def _as_one(tensors):
@@ -516,14 +519,29 @@ class ParameterServerTrainer(object):
         self._non_embed_grads = None
 
     # ------------------------------------------------------------------ the worker's training loop
-    def train_loop(self, batches, max_minibatch_retry_num=64, on_step=None):
+    def train_loop(self, batches, max_minibatch_retry_num=64, on_step=None, callbacks=None):
         """The training loop of elasticdl/python/worker/worker.py:338-370 around train_minibatch, with its
         `get_model_steps` logic (SSP, docs/designs/async_sgd.md:129-157): the dense model is pulled from the
         PS only every `get_model_steps` minibatches (and after a failed one); in between the worker trains
         with its LOCAL model, which `_update_local_model` advances with the gradients it just pushed
         (dense variables only -- embedding rows are always pulled fresh).  A minibatch whose push is not
         accepted is retried up to `max_minibatch_retry_num` times (worker.py:181-234: "Worker got stuck").
-        batches: iterable of (features, labels).  Returns [(version, loss)] per minibatch."""
+        batches: iterable of (features, labels).  Returns [(version, loss)] per minibatch.
+        callbacks (elasticdl_b200.callbacks): each is given the model, and its on_train_batch_begin is called with
+        the model version before every minibatch (worker.py:198).  On an async group a LearningRateScheduler over a
+        declarative schedule is also installed on the PS group, whose pushes then evaluate it on the device, so that
+        the graphed step needs no re-capture for it; on a sync-SGD group the schedule is evaluated on the host only,
+        as the reference does.  Passing callbacks replaces the group's schedule (callbacks without a declarative
+        scheduler remove one set by hand), and the schedule stays installed after train_loop returns; without
+        callbacks the group's schedule is left as it is."""
+        if callbacks is not None:
+            from elasticdl_b200.callbacks import device_schedule
+
+            callbacks = list(callbacks)
+            for cb in callbacks:
+                cb.set_model(self._model)
+            group = self._ps_client.group
+            group.set_lr_schedule(device_schedule(callbacks) if group.use_async else None)
         local_update_count = self._get_model_steps
         last_training_minibatch_failed = False
         out = []
@@ -536,6 +554,8 @@ class ParameterServerTrainer(object):
             err_msg = ""
             try:  # _safe_process_minibatch (worker.py:274-300)
                 for _ in range(max_minibatch_retry_num):
+                    for cb in callbacks or ():
+                        cb.on_train_batch_begin(self.get_model_version())
                     accepted, version, loss = self.train_minibatch(features, labels, train_with_local_model)
                     if accepted:
                         break

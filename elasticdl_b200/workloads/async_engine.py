@@ -25,7 +25,7 @@ class AsyncEngine:
     A subclass sets `inputs`, its step's inputs as [(name, dtype, shape)], `tower` (whose `loss` the step leaves),
     `push_dense_segs` and `push_rows_segs`, and defines _step(*inputs), which ends in _push()."""
 
-    def __init__(self, group, batch, lr, register):
+    def __init__(self, group, batch, lr, register, lr_schedule=None):
         name = type(self).__name__
         if not getattr(group, "use_async", True):
             raise ValueError("%s trains async only: a sync-SGD group needs the drop-in trainer" % name)
@@ -42,6 +42,9 @@ class AsyncEngine:
         self.graph = None
         self._graph_lr = None
         self.steps = 0
+        self.lr_schedule = None
+        if lr_schedule is not None:
+            self.set_lr_schedule(lr_schedule)
 
     def _check_batch(self, *tensors):
         """Check a batch, one tensor per declared input, against the declaration."""
@@ -63,25 +66,38 @@ class AsyncEngine:
 
     def set_lr(self, lr):
         """The learning rate the next pushes carry (the reference's schedule callback sets it per version);
-        the captured graph is re-captured on the next replay."""
+        the captured graph is re-captured on the next replay.  ValueError while a schedule is installed."""
+        if self.lr_schedule is not None:
+            raise ValueError("the learning rate comes from the installed schedule: set_lr_schedule(None) first")
         self.lr = float(lr)
+
+    def set_lr_schedule(self, schedule):
+        """Evaluate `schedule` (an elasticdl_b200.callbacks.LearningRateSchedule) on the device at every push, in
+        place of `lr`, from the shard versions the push begins on; None goes back to `lr`.  The captured graph is
+        re-captured on the next replay, and then replays the schedule with no re-capture."""
+        self.group.set_lr_schedule(schedule)
+        self.lr_schedule = schedule
+
+    def _graph_key(self):
+        return self.lr if self.lr_schedule is None else self.lr_schedule.key()
 
     def capture(self):
         """Capture one step over static inputs (self.statics, one per declared input) into a CUDA graph on the
-        current stream's device; the learning rate is baked in."""
+        current stream's device; the learning rate, or the schedule, is baked in."""
         if self.graph is None:
             self.statics = [torch.zeros(shape, dtype=dtype, device=self.device) for _, dtype, shape in self.inputs]
         torch.cuda.current_stream(self.device).synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             self._step(*self.statics)
-        self.graph, self._graph_lr = graph, self.lr
+        self.graph, self._graph_lr = graph, self._graph_key()
         return graph
 
     def replay(self, *inputs):
-        """step() through the captured graph (captured now if there is none or the learning rate changed)."""
+        """step() through the captured graph (captured now if there is none or the learning rate or the schedule
+        changed)."""
         self._check_batch(*inputs)
-        if self.graph is None or self._graph_lr != self.lr:
+        if self.graph is None or self._graph_lr != self._graph_key():
             self.capture()
         for s, t in zip(self.statics, inputs):
             s.copy_(t)

@@ -81,6 +81,15 @@ def eval_metrics_fn():
     return zoo_eval_metrics(0.5)
 
 
+def callbacks():
+    """The census model's learning-rate schedule (model_zoo/census_wide_deep_model/wide_deep_functional_api.py:74-83:
+    3e-4 below version 5000, 2e-4 below 12000, then 1e-4) as a declarative schedule the push evaluates on the
+    device; versions are integers, so `< 5000` is `<= 4999`."""
+    from elasticdl_b200.callbacks import LearningRateScheduler, PiecewiseConstantDecay
+
+    return [LearningRateScheduler(PiecewiseConstantDecay([4999, 11999], [3e-4, 2e-4, 1e-4]))]
+
+
 class CensusTowerCall:
     """The census tower's output buffers and workspace for batch B on `device`, and one launch over them."""
 
@@ -163,10 +172,11 @@ class CensusWideDeepEngine(AsyncEngine):
     step(numeric float32 [4, B], strings uint8 [8, B, 32], labels float32 [B]) runs pull_dense (into the flat
     buffer) -> census_transform -> the tower -> push_begin -> push_dense (MLP) -> push_rows (the five tables'
     touched rows, counts on the device) -> push_end, with no host read, and returns the loss on the device.
-    capture() / replay() run the same step as one CUDA graph over static inputs; a new learning rate re-captures."""
+    capture() / replay() run the same step as one CUDA graph over static inputs; a new learning rate re-captures.
+    lr_schedule: a schedule to install, as AsyncEngine.set_lr_schedule does."""
 
-    def __init__(self, group, batch, lr, reference_reshape=False, seed=0, register=True):
-        super().__init__(group, batch, lr, register)
+    def __init__(self, group, batch, lr, reference_reshape=False, seed=0, register=True, lr_schedule=None):
+        super().__init__(group, batch, lr, register, lr_schedule)
         g, B = self.group, self.B
         self.inputs = [("numeric", torch.float32, (4, B)), ("strings", torch.uint8, (8, B, STRING_WIDTH)),
                        ("labels", torch.float32, (B,))]

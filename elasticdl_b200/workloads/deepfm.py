@@ -414,7 +414,7 @@ def resolve_row_source(row_source, tower, n_shards, exchange, paired):
 class DeepFMPSEngine:
     def __init__(self, group, batch, lr=1e-3, init_std=0.01, seed=7, group_rows=GROUP_ROWS, deep_dim=DEEP_DIM,
                  init_rows=True, tower="tile", paired=None, exchange=None, id_transport="int32", row_source="auto",
-                 model="deepfm"):
+                 model="deepfm", lr_schedule=None):
         """tower="tile": rows of 32 samples gathered once into shared memory, forward / backward / parameter
         gradients from the tile (csrc/deepfm_tower2.cu);
         tower="fused": round 1's hand-written CUDA tower (csrc/deepfm_tower.cu, three row gathers);
@@ -429,7 +429,8 @@ class DeepFMPSEngine:
         kernel without it) or "xdeepfm" (XDeepFMTower, the model the dac_ctr training script runs: Wide & Deep plus
         a CIN, csrc/xdeepfm_cin.cu); the dedup, the rows, the push and the pipelines are the same for all four.
         The models other than "deepfm" run on tower="tile" or "torch" and at most 38 id groups, "xdeepfm" on at
-        least 2, and raise ValueError otherwise (the fused and mma towers compute DeepFM only)."""
+        least 2, and raise ValueError otherwise (the fused and mma towers compute DeepFM only).
+        lr_schedule: a schedule to install, as set_lr_schedule does."""
         assert tower in ("tile", "fused", "mma", "torch")
         if model not in TOWERS:
             raise ValueError("model must be one of %s, not %r" % (sorted(TOWERS), model))
@@ -554,6 +555,21 @@ class DeepFMPSEngine:
         if self.exchange == "owner":
             group.xchg_create(G, B, self.deep_ids, self.wide_ids)
         self.steps = 0
+        self.lr_schedule = None
+        if lr_schedule is not None:
+            self.set_lr_schedule(lr_schedule)
+
+    def set_lr_schedule(self, schedule):
+        """Evaluate `schedule` (an elasticdl_b200.callbacks.LearningRateSchedule) on the device at every push, in
+        place of `lr`, from the shard versions the push begins on; None goes back to `lr`.  The graphs captured
+        so far are captured again (a lookahead pipeline keeps its loaded batch); they then replay the schedule
+        with no host read."""
+        self.group.set_lr_schedule(schedule)
+        self.lr_schedule = schedule
+        if self.graph is not None:
+            self.capture()
+        if self.graphs_ahead is not None:
+            self.capture_ahead()
 
     _PLAN_ATTRS = ("uniq", "inv", "n_unique", "pull_segs", "push_segs", "pull_pair", "push_pair", "tower_args",
                    "tower_rows", "pull_names", "push_names")
@@ -849,7 +865,9 @@ class DeepFMPSEngine:
             raise RuntimeError("graph capture needs the fused tower (torch autograd allocates)")
         dev, G, B = self.device, self.G, self.B
         self._ensure_plans()
-        self.s_packed = [torch.zeros(packed_nbytes(G, B, self.widths), dtype=torch.uint8, device=dev) for _ in range(2)]
+        if getattr(self, "s_packed", None) is None:  # a second capture keeps the batch loaded into them
+            self.s_packed = [torch.zeros(packed_nbytes(G, B, self.widths), dtype=torch.uint8, device=dev)
+                             for _ in range(2)]
         views = [packed_views(b, G, B, self.widths) for b in self.s_packed]
         torch.cuda.synchronize(dev)
         start, steps = self.cur, self.steps
@@ -900,8 +918,8 @@ class DeepFMPSEngine:
     # ------------------------------------------------------------------ CUDA graph
     def capture(self):
         """Capture one whole step into a CUDA graph.  Every buffer the step touches is persistent, so
-        the graph replays on new inputs copied into the static packed input buffer.  lr is baked in:
-        re-capture to change it."""
+        the graph replays on new inputs copied into the static packed input buffer.  lr, or the schedule, is
+        baked in: re-capture to change it."""
         if self.tower_kind == "torch":
             raise RuntimeError("graph capture needs the fused tower (torch autograd allocates)")
         dev, G, B = self.device, self.G, self.B

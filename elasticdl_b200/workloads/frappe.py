@@ -106,6 +106,15 @@ def eval_metrics_fn():
     return zoo_eval_metrics(0.0)
 
 
+def callbacks():
+    """The frappe DeepFM model's learning-rate schedule (model_zoo/deepfm_functional_api/deepfm_functional_api.py:
+    140-145: 0.5 below version 100, then 0.2) as a declarative schedule the push evaluates on the device; versions
+    are integers, so `< 100` is `<= 99`."""
+    from elasticdl_b200.callbacks import LearningRateScheduler, PiecewiseConstantDecay
+
+    return [LearningRateScheduler(PiecewiseConstantDecay([99], [0.5, 0.2]))]
+
+
 class FrappeTowerCall:
     """The frappe tower's output buffers and workspace for batch B and up to `rows` unique ids on `device`, and
     one launch over them."""
@@ -185,10 +194,11 @@ class FrappeDeepFMEngine(AsyncEngine):
     step(ids int64 [B, 10], labels float32 [B]) runs pull_dense (into the flat buffer) -> dedup of the 10 B ids
     -> one pull_rows for both tables -> the tower -> push_begin -> push_dense -> push_rows (two segments, counts
     on the device) -> push_end, with no host read, and returns the loss on the device.  capture() / replay() run
-    the same step as one CUDA graph over static inputs; a new learning rate re-captures."""
+    the same step as one CUDA graph over static inputs; a new learning rate re-captures.
+    lr_schedule: a schedule to install, as AsyncEngine.set_lr_schedule does."""
 
-    def __init__(self, group, batch, lr, input_dim=None, seed=0, register=True, expected_rows=None):
-        super().__init__(group, batch, lr, register)
+    def __init__(self, group, batch, lr, input_dim=None, seed=0, register=True, expected_rows=None, lr_schedule=None):
+        super().__init__(group, batch, lr, register, lr_schedule)
         if input_dim is not None and int(input_dim) < 1:
             raise ValueError("input_dim must be None (hashed tables) or >= 1, not %r" % (input_dim,))
         g, dev, B = self.group, self.device, self.B

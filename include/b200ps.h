@@ -199,6 +199,40 @@ int b200ps_slot_dense(b200ps_t* ps, int slot, int write, const b200ps_seg_t* seg
  * push_rows expects ids unique within a segment (PSClient dedups first,
  * ps_client.py:255-257) -- use b200ps_unique + b200ps_segment_sum. */
 int b200ps_push_begin(b200ps_t* ps, float learning_rate, const int32_t* model_versions, void* stream);
+
+/* A learning-rate schedule of tf.keras.optimizers.schedules (TF 2.5), evaluated by push_begin on the device
+ * (elasticdl/python/elasticdl/callbacks.py:69-109 runs it on the worker; server.go:178-187 applies its lr).
+ * Argument x = max(max_s version_s - 1, 0), the shard versions push_begin reads; in double, rounded once to
+ * float:
+ *   PIECEWISE     values[0] for x <= boundaries[0], values[i] for boundaries[i-1] < x <= boundaries[i],
+ *                 values[n_boundaries] past the last (boundaries strictly increasing, at most 32);
+ *   EXPONENTIAL   initial * decay_rate^p, p = x / decay_steps (floored if staircase);
+ *   INVERSE_TIME  initial / (1 + decay_rate * p), p as EXPONENTIAL;
+ *   POLYNOMIAL    (initial - end) * (1 - s / D)^power + end; s = min(x, decay_steps), D = decay_steps, or with
+ *                 cycle s = x, D = decay_steps * max(1, ceil(x / decay_steps)).
+ * The value takes the place of push_begin's learning_rate, which is ignored while a schedule is installed;
+ * staleness modulation still divides it and a value <= 0 falls back to the optimizer's lr. */
+#define B200PS_LR_MAX_BOUNDARIES 32
+enum {
+  B200PS_LR_PIECEWISE = 1,
+  B200PS_LR_EXPONENTIAL = 2,
+  B200PS_LR_INVERSE_TIME = 3,
+  B200PS_LR_POLYNOMIAL = 4
+};
+typedef struct {
+  int32_t kind;         /* B200PS_LR_* */
+  int32_t n_boundaries; /* PIECEWISE */
+  int32_t staircase;    /* EXPONENTIAL, INVERSE_TIME */
+  int32_t cycle;        /* POLYNOMIAL */
+  double initial_learning_rate, decay_steps, decay_rate, end_learning_rate, power;
+  double boundaries[B200PS_LR_MAX_BOUNDARIES];
+  float values[B200PS_LR_MAX_BOUNDARIES + 1];
+} b200ps_lr_schedule_t;
+/* Install `s` on this client view (copied; NULL clears it).  Other views of the group, b200ps_clone_view's
+ * included, keep their own.  B200PS_EINVAL, changing nothing, for an unknown kind, decay_steps <= 0 (the
+ * decaying kinds), a non-finite parameter, or n_boundaries outside [0, 32] or boundaries not strictly
+ * increasing (PIECEWISE). */
+int b200ps_set_lr_schedule(b200ps_t* ps, const b200ps_lr_schedule_t* s);
 int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream);
 /* Dense gradients: rows_dev = gradient [numel]. */
 int b200ps_push_dense(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream);
