@@ -76,6 +76,35 @@ class FrappeArgs(ctypes.Structure):  # b200_frappe_args_t (include/b200_frappe.h
     ]
 
 
+FC_MAX_TABLES, FC_MAX_BLOCKS = 8, 16  # B200_FC_DNN_MAX_TABLES, B200_FC_DNN_MAX_BLOCKS
+
+
+class FcBlock(ctypes.Structure):  # b200_fc_block_t (include/b200_fc_dnn.h)
+    _fields_ = [("kind", ctypes.c_int32), ("src", ctypes.c_int32), ("width", ctypes.c_int32),
+                ("offset", ctypes.c_int32)]
+
+
+class FcLayout(ctypes.Structure):  # b200_fc_layout_t
+    _fields_ = [
+        ("F", ctypes.c_int32), ("n_blocks", ctypes.c_int32), ("n_tables", ctypes.c_int32),
+        ("loss_mean", ctypes.c_int32), ("table_rows", ctypes.c_int32 * FC_MAX_TABLES),
+        ("table_dim", ctypes.c_int32 * FC_MAX_TABLES), ("table_string", ctypes.c_int32 * FC_MAX_TABLES),
+        ("blocks", FcBlock * FC_MAX_BLOCKS),
+    ]
+
+
+class FcDnnArgs(ctypes.Structure):  # b200_fc_dnn_args_t
+    _fields_ = [
+        ("B", ctypes.c_int64), ("n_numeric", ctypes.c_int32), ("n_ids", ctypes.c_int32),
+        ("n_strings", ctypes.c_int32), ("W", ctypes.c_int32),
+        ("numeric", ctypes.c_void_p), ("ids", ctypes.c_void_p), ("strings", ctypes.c_void_p),
+        ("inv", ctypes.c_void_p), ("n_unique", ctypes.c_void_p), ("rows", ctypes.c_void_p),
+        ("labels", ctypes.c_void_p), ("params", ctypes.c_void_p), ("loss", ctypes.c_void_p),
+        ("logits", ctypes.c_void_p), ("grads", ctypes.c_void_p), ("gsum", ctypes.c_void_p),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 LR_MAX_BOUNDARIES = 32  # B200PS_LR_MAX_BOUNDARIES
 LR_PIECEWISE, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_POLYNOMIAL = 1, 2, 3, 4
 
@@ -243,6 +272,16 @@ FRAPPE_SYMBOLS = {
     "b200_frappe_last_error": (ctypes.c_char_p, []),
     "b200_frappe_launch_count": (_i64, []),
 }
+# include/b200_fc_dnn.h
+FC_DNN_SYMBOLS = {
+    "b200_fc_dnn_params": (_i64, [ctypes.POINTER(FcLayout)]),
+    "b200_fc_dnn_workspace_bytes": (_sz, [ctypes.POINTER(FcLayout), _i64]),
+    "b200_fc_dnn_fill_empty": (_i, [ctypes.POINTER(FcLayout), _vp, _vp, _i64, _i, _vp]),
+    "b200_fc_dnn_tower": (_i, [ctypes.POINTER(FcLayout), ctypes.POINTER(FcDnnArgs), _vp]),
+    "b200_fc_dnn_forward": (_i, [ctypes.POINTER(FcLayout), ctypes.POINTER(FcDnnArgs), _vp]),
+    "b200_fc_dnn_last_error": (ctypes.c_char_p, []),
+    "b200_fc_dnn_launch_count": (_i64, []),
+}
 # include/b200_metrics.h
 METRICS_MAX_THRESHOLDS = 16384  # B200_METRICS_MAX_THRESHOLDS
 METRICS_SYMBOLS = {
@@ -263,7 +302,7 @@ def lib():
             path = _build.build()
         handle = ctypes.CDLL(path)
         for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items())\
-                + list(METRICS_SYMBOLS.items()):
+                + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args
