@@ -18,23 +18,19 @@
 #include "ps_flat.cuh"
 #include "ps_unique.cuh"
 #include "ps_exchange.cuh"
+#include "launch.cuh"
 
 using namespace b200ps_impl;
 
 namespace {
 
-thread_local std::string g_err;
-
-int fail(int code, const std::string& msg) {
-  g_err = msg;
-  return code;
-}
+using E = entry::Entry<entry::Ps>;
 
 #define CUDA_OK(expr)                                                                 \
   do {                                                                                \
     cudaError_t e_ = (expr);                                                          \
     if (e_ != cudaSuccess)                                                            \
-      return fail(B200PS_ECUDA, std::string(#expr) + ": " + cudaGetErrorString(e_)); \
+      return E::fail(B200PS_ECUDA, std::string(#expr) + ": " + cudaGetErrorString(e_)); \
   } while (0)
 
 struct DeviceGuard {
@@ -168,7 +164,7 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
       {"Nadam", {"learning_rate", "beta_1", "beta_2", "epsilon"}},
   };
   auto it = want.find(type);
-  if (it == want.end()) return fail(B200PS_EINVAL, "Unknown optimizer type " + type);
+  if (it == want.end()) return E::fail(B200PS_EINVAL, "Unknown optimizer type " + type);
   std::map<std::string, std::string> kv;
   size_t pos = 0;
   while (pos <= args.size()) {  // strings.Split(optArgs, ";")
@@ -176,50 +172,50 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
     std::string item = args.substr(pos, semi == std::string::npos ? std::string::npos : semi - pos);
     if (!item.empty()) {
       size_t eq = item.find('=');
-      if (eq == std::string::npos) return fail(B200PS_EINVAL, "malformed optimizer argument " + item);
+      if (eq == std::string::npos) return E::fail(B200PS_EINVAL, "malformed optimizer argument " + item);
       kv[item.substr(0, eq)] = item.substr(eq + 1);
     }
     if (semi == std::string::npos) break;
     pos = semi + 1;
   }
   for (auto& k : it->second)
-    if (!kv.count(k)) return fail(B200PS_EINVAL, "Args passed to ps should contain " + k);
-  if (kv.size() != it->second.size()) return fail(B200PS_EINVAL, "Args passed to ps contain redundant items");
+    if (!kv.count(k)) return E::fail(B200PS_EINVAL, "Args passed to ps should contain " + k);
+  if (kv.size() != it->second.size()) return E::fail(B200PS_EINVAL, "Args passed to ps contain redundant items");
   memset(o, 0, sizeof(*o));
-  if (parse_float(kv["learning_rate"], &o->lr)) return fail(B200PS_EINVAL, "Having error converting learning rate to number");
+  if (parse_float(kv["learning_rate"], &o->lr)) return E::fail(B200PS_EINVAL, "Having error converting learning rate to number");
   if (type == "SGD") {
     bool nes;
-    if (parse_float(kv["momentum"], &o->mu) || parse_bool(kv["nesterov"], &nes)) return fail(B200PS_EINVAL, "bad SGD argument");
+    if (parse_float(kv["momentum"], &o->mu) || parse_bool(kv["nesterov"], &nes)) return E::fail(B200PS_EINVAL, "bad SGD argument");
     o->nesterov = nes;
     o->kind = o->mu > 0.0f ? kMomentum : kSGD;  // optimizer.go:353-356
   } else if (type == "Adam") {
     bool ams;
     if (parse_float(kv["beta_1"], &o->beta1) || parse_float(kv["beta_2"], &o->beta2) ||
         parse_float(kv["epsilon"], &o->epsilon) || parse_bool(kv["amsgrad"], &ams))
-      return fail(B200PS_EINVAL, "bad Adam argument");
+      return E::fail(B200PS_EINVAL, "bad Adam argument");
     o->kind = ams ? kAMSGrad : kAdam;
     o->c1 = (float)(1.0 - (double)o->beta1);
     o->c2 = (float)(1.0 - (double)o->beta2);
   } else if (type == "Adagrad") {
-    if (parse_float(kv["epsilon"], &o->epsilon)) return fail(B200PS_EINVAL, "bad Adagrad argument");
+    if (parse_float(kv["epsilon"], &o->epsilon)) return E::fail(B200PS_EINVAL, "bad Adagrad argument");
     o->kind = kAdagrad;
   } else if (type == "RMSprop") {
     bool centered;
     if (parse_float(kv["rho"], &o->beta1) || parse_float(kv["momentum"], &o->mu) ||
         parse_float(kv["epsilon"], &o->epsilon) || parse_bool(kv["centered"], &centered))
-      return fail(B200PS_EINVAL, "bad RMSprop argument");
+      return E::fail(B200PS_EINVAL, "bad RMSprop argument");
     const bool mom = o->mu > 0.0f;  // Keras: self._momentum = momentum > 0 (the momentum slot exists only then)
     o->kind = centered ? (mom ? kRMSpropCenteredMomentum : kRMSpropCentered) : (mom ? kRMSpropMomentum : kRMSprop);
     o->c1 = (float)(1.0 - (double)o->beta1);  // rho, 1 - rho (OptParams)
   } else if (type == "Adadelta") {
     if (parse_float(kv["rho"], &o->beta1) || parse_float(kv["epsilon"], &o->epsilon))
-      return fail(B200PS_EINVAL, "bad Adadelta argument");
+      return E::fail(B200PS_EINVAL, "bad Adadelta argument");
     o->kind = kAdadelta;
     o->c1 = (float)(1.0 - (double)o->beta1);  // rho, 1 - rho (OptParams)
   } else if (type == "Adamax" || type == "Nadam") {
     if (parse_float(kv["beta_1"], &o->beta1) || parse_float(kv["beta_2"], &o->beta2) ||
         parse_float(kv["epsilon"], &o->epsilon))
-      return fail(B200PS_EINVAL, "bad " + type + " argument");
+      return E::fail(B200PS_EINVAL, "bad " + type + " argument");
     o->kind = type == "Adamax" ? kAdamax : kNadam;
     o->c1 = (float)(1.0 - (double)o->beta1);
     o->c2 = (float)(1.0 - (double)o->beta2);
@@ -228,7 +224,7 @@ int parse_optimizer(const char* type_c, const char* args_c, OptParams* o) {
         parse_float(kv["l1_regularization_strength"], &o->l1) ||
         parse_float(kv["l2_regularization_strength"], &o->l2) ||
         parse_float(kv["l2_shrinkage_regularization_strength"], &o->l2s) || parse_float(kv["beta"], &o->beta))
-      return fail(B200PS_EINVAL, "bad Ftrl argument");
+      return E::fail(B200PS_EINVAL, "bad Ftrl argument");
     o->kind = kFTRL;
   }
   return B200PS_OK;
@@ -245,8 +241,8 @@ int nadam_schedule(float beta1, std::vector<float>* s) {
     if (cur == prev && (cur == 0.0f || (beta1 >= 0.0f && beta1 <= 1.0f))) return B200PS_OK;
   }
   s->clear();
-  return fail(B200PS_EINVAL, "Nadam: the momentum schedule of beta_1 = " + std::to_string(beta1) +
-                                 " does not settle within " + std::to_string(kNadamMaxSteps) + " steps");
+  return E::fail(B200PS_EINVAL, "Nadam: the momentum schedule of beta_1 = " + std::to_string(beta1) +
+                                    " does not settle within " + std::to_string(kNadamMaxSteps) + " steps");
 }
 
 // Copies the host schedule to the client device, where k_push_begin reads it.
@@ -296,12 +292,12 @@ int grid_for(b200ps_t* ps, long long work_items, int per_block = 256) {
 }
 
 int ready(b200ps_t* ps) {
-  if (!ps) return fail(B200PS_EINVAL, "null group");
+  if (!ps) return E::fail(B200PS_EINVAL, "null group");
   for (int s = 0; s < ps->n_shards; ++s)
-    if (!ps->shard[s].attached) return fail(B200PS_ESTATE, "shard " + std::to_string(s) + " is not attached");
-  if (ps->dirty) return fail(B200PS_ESTATE, "b200ps_commit() not called after the last registration/import");
+    if (!ps->shard[s].attached) return E::fail(B200PS_ESTATE, "shard " + std::to_string(s) + " is not attached");
+  if (ps->dirty) return E::fail(B200PS_ESTATE, "b200ps_commit() not called after the last registration/import");
   if (ps->opt.kind < 0 || ps->opt.kind >= kNumOptKinds)  // parse_optimizer sets every kind; DISPATCH_OPT relies on it
-    return fail(B200PS_EINVAL, "unknown optimizer kind " + std::to_string(ps->opt.kind));
+    return E::fail(B200PS_EINVAL, "unknown optimizer kind " + std::to_string(ps->opt.kind));
   return B200PS_OK;
 }
 
@@ -396,16 +392,16 @@ struct Split {
 };
 
 int split_segs(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, bool want_dense, Split* out, bool push = false) {
-  if (nseg < 0 || nseg > kMaxSegs) return fail(B200PS_EINVAL, "nseg out of range (max " + std::to_string(kMaxSegs) + ")");
+  if (nseg < 0 || nseg > kMaxSegs) return E::fail(B200PS_EINVAL, "nseg out of range (max " + std::to_string(kMaxSegs) + ")");
   for (int c = 0; c < kClasses; ++c) out->b[c].nseg = 0;
   out->flat_n = 0;
   const bool flat_ok = ps->n_shards <= 8;  // the flat kernels carry <= 8 per-shard pointers per segment in their parameters
   for (int i = 0; i < nseg; ++i) {
     const b200ps_seg_t& sg = segs[i];
-    if (sg.table < 0 || sg.table >= (int)ps->tables.size()) return fail(B200PS_ENOTFOUND, "unknown table id " + std::to_string(sg.table));
+    if (sg.table < 0 || sg.table >= (int)ps->tables.size()) return E::fail(B200PS_ENOTFOUND, "unknown table id " + std::to_string(sg.table));
     const Table& t = ps->tables[sg.table];
-    if (want_dense && !t.is_dense) return fail(B200PS_EINVAL, t.name + " is not a dense parameter");
-    if (sg.n < 0) return fail(B200PS_EINVAL, "negative segment length");
+    if (want_dense && !t.is_dense) return E::fail(B200PS_EINVAL, t.name + " is not a dense parameter");
+    if (sg.n < 0) return E::fail(B200PS_EINVAL, "negative segment length");
     if (sg.n == 0 && !want_dense) continue;
     if (!want_dense && !t.hashed && flat_ok && t.row_stride < (1LL << 31)) {
       const int k = out->flat_n++;
@@ -495,8 +491,7 @@ int for_each_class(b200ps_t* ps, Split& sp, F&& launch) {
 // Persistent grid of the flat kernels.  The grid must not exceed what is RESIDENT at once: a block that waits for
 // a free slot starts after the first wave has finished and pays the block prologue (76 device-side counts ->
 // scan -> barrier) and the launch ramp again.  Sized for 8 blocks per SM the 48-register kernels (5 resident)
-// would run 1.6 waves, so the grid follows cudaOccupancyMaxActiveBlocksPerMultiprocessor of the kernel actually
-// launched.
+// would run 1.6 waves, so the grid follows the occupancy of the kernel actually launched.
 // U rows in flight per thread only once the work is several times what the resident threads cover.  (U = 4
 // measured slower: its 80 registers cost more resident warps than the unroll adds.)
 int flat_u(b200ps_t* ps, long long items) {
@@ -506,21 +501,15 @@ int flat_u(b200ps_t* ps, long long items) {
 
 // blocks of `kern` (256 threads, no dynamic shared memory) resident on the whole device
 template <typename K>
-int flat_grid(b200ps_t* ps, K kern, long long items, int U) {
-  static std::mutex mu;
-  static std::unordered_map<const void*, int> occ;
-  std::lock_guard<std::mutex> lk(mu);
-  auto it = occ.find((const void*)kern);
-  if (it == occ.end()) {
-    int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 256, 0) != cudaSuccess || v < 1) v = 4;
-    it = occ.emplace((const void*)kern, v).first;
-  }
-  const long long cap = (long long)ps->n_sm * it->second;
+int flat_grid(b200ps_t* ps, K* kern, long long items, int U, int* grid) {
+  int per = 0;
+  if (int rc = E::blocks_per_sm(kern, 256, 0, &per)) return rc;
+  const long long cap = (long long)ps->n_sm * per;
   long long blocks = (items + 256LL * U - 1) / (256LL * U);
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  return (int)blocks;
+  *grid = (int)blocks;
+  return 0;
 }
 
 #define DISPATCH_U(UVAL, ...)                          \
@@ -534,13 +523,13 @@ int flat_grid(b200ps_t* ps, K kern, long long items, int U) {
 // =============================================================================
 extern "C" {
 
-const char* b200ps_last_error(void) { return g_err.c_str(); }
+const char* b200ps_last_error(void) { return E::last_error().c_str(); }
 int b200ps_abi_version(void) { return B200PS_ABI_VERSION; }
 
 int b200ps_create(int n_shards, int client_device, const char* opt_type, const char* opt_args,
                   int lr_staleness_modulation, unsigned flags, b200ps_t** out) {
-  if (!out) return fail(B200PS_EINVAL, "out is null");
-  if (n_shards < 1 || n_shards > kMaxShards) return fail(B200PS_EINVAL, "n_shards must be in [1, 16]");
+  if (!out) return E::fail(B200PS_EINVAL, "out is null");
+  if (n_shards < 1 || n_shards > kMaxShards) return E::fail(B200PS_EINVAL, "n_shards must be in [1, 16]");
   OptParams o;
   int rc = parse_optimizer(opt_type, opt_args, &o);
   if (rc) return rc;
@@ -548,7 +537,7 @@ int b200ps_create(int n_shards, int client_device, const char* opt_type, const c
   if (o.kind == kNadam && (rc = nadam_schedule(o.beta1, &sched))) return rc;
   int ndev = 0;
   CUDA_OK(cudaGetDeviceCount(&ndev));
-  if (client_device < 0 || client_device >= ndev) return fail(B200PS_ECUDA, "client device " + std::to_string(client_device) + " not present");
+  if (client_device < 0 || client_device >= ndev) return E::fail(B200PS_ECUDA, "client device " + std::to_string(client_device) + " not present");
   b200ps_t* ps = new b200ps();
   ps->n_shards = n_shards;
   ps->client_device = client_device;
@@ -572,7 +561,7 @@ int b200ps_create(int n_shards, int client_device, const char* opt_type, const c
   if (e == cudaSuccess) e = upload_nadam(ps);
   if (e != cudaSuccess) {
     delete ps;
-    return fail(B200PS_ECUDA, std::string("b200ps_create: ") + cudaGetErrorString(e));
+    return E::fail(B200PS_ECUDA, std::string("b200ps_create: ") + cudaGetErrorString(e));
   }
   *out = ps;
   return B200PS_OK;
@@ -609,9 +598,9 @@ int b200ps_destroy(b200ps_t* ps) {
 }
 
 int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
-  if (!src || !out) return fail(B200PS_EINVAL, "bad argument");
+  if (!src || !out) return E::fail(B200PS_EINVAL, "bad argument");
   for (int s = 0; s < src->n_shards; ++s)
-    if (!src->shard[s].attached) return fail(B200PS_ESTATE, "source group has unattached shards");
+    if (!src->shard[s].attached) return E::fail(B200PS_ESTATE, "source group has unattached shards");
   std::lock_guard<std::mutex> lk(src->mu);
   b200ps_t* ps = new b200ps();
   ps->n_shards = src->n_shards;
@@ -635,7 +624,7 @@ int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
     for (int s = 0; s < src->n_shards; ++s) {
       if (src->shard[s].device == client_device) continue;
       cudaError_t e = cudaDeviceEnablePeerAccess(src->shard[s].device, 0);
-      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { delete ps; return fail(B200PS_ECUDA, cudaGetErrorString(e)); }
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { delete ps; return E::fail(B200PS_ECUDA, cudaGetErrorString(e)); }
       cudaGetLastError();
     }
   }
@@ -649,7 +638,7 @@ int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
   if (e == cudaSuccess) e = upload_nadam(ps);
   if (e != cudaSuccess) {
     delete ps;
-    return fail(B200PS_ECUDA, std::string("b200ps_clone_view: ") + cudaGetErrorString(e));
+    return E::fail(B200PS_ECUDA, std::string("b200ps_clone_view: ") + cudaGetErrorString(e));
   }
   ps->dirty = true;
   *out = ps;
@@ -657,16 +646,16 @@ int b200ps_clone_view(b200ps_t* src, int client_device, b200ps_t** out) {
 }
 
 int b200ps_shard_create_local(b200ps_t* ps, int shard_id, int device) {
-  if (!ps || shard_id < 0 || shard_id >= ps->n_shards) return fail(B200PS_EINVAL, "bad shard id");
+  if (!ps || shard_id < 0 || shard_id >= ps->n_shards) return E::fail(B200PS_EINVAL, "bad shard id");
   Shard& sh = ps->shard[shard_id];
-  if (sh.attached) return fail(B200PS_ESTATE, "shard already attached");
+  if (sh.attached) return E::fail(B200PS_ESTATE, "shard already attached");
   int ndev = 0;
   CUDA_OK(cudaGetDeviceCount(&ndev));
-  if (device < 0 || device >= ndev) return fail(B200PS_ECUDA, "shard device not present");
+  if (device < 0 || device >= ndev) return E::fail(B200PS_ECUDA, "shard device not present");
   if (device != ps->client_device) {
     int can = 0;
     CUDA_OK(cudaDeviceCanAccessPeer(&can, ps->client_device, device));
-    if (!can) return fail(B200PS_ECUDA, "no peer access from client device to shard device");
+    if (!can) return E::fail(B200PS_ECUDA, "no peer access from client device to shard device");
     DeviceGuard g(ps->client_device);
     cudaError_t e = cudaDeviceEnablePeerAccess(device, 0);
     if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CUDA_OK(e);
@@ -699,9 +688,9 @@ int b200ps_shard_create_local(b200ps_t* ps, int shard_id, int device) {
 }
 
 int b200ps_shard_export(b200ps_t* ps, int shard_id, void* blob, size_t cap, size_t* size) {
-  if (!ps || shard_id < 0 || shard_id >= ps->n_shards || !size) return fail(B200PS_EINVAL, "bad argument");
+  if (!ps || shard_id < 0 || shard_id >= ps->n_shards || !size) return E::fail(B200PS_EINVAL, "bad argument");
   Shard& sh = ps->shard[shard_id];
-  if (!sh.local) return fail(B200PS_ESTATE, "only a local shard can be exported");
+  if (!sh.local) return E::fail(B200PS_ESTATE, "only a local shard can be exported");
   std::vector<BlobEntry> entries;
   DeviceGuard g(sh.device);
   BlobEntry ce{};
@@ -720,7 +709,7 @@ int b200ps_shard_export(b200ps_t* ps, int shard_id, void* blob, size_t cap, size
   }
   size_t need = sizeof(BlobHeader) + entries.size() * sizeof(BlobEntry);
   *size = need;
-  if (!blob || cap < need) return blob ? fail(B200PS_EINVAL, "blob buffer too small") : B200PS_OK;
+  if (!blob || cap < need) return blob ? E::fail(B200PS_EINVAL, "blob buffer too small") : B200PS_OK;
   BlobHeader h{kBlobMagic, shard_id, (int)entries.size(), 0};
   memcpy(blob, &h, sizeof(h));
   memcpy((char*)blob + sizeof(h), entries.data(), entries.size() * sizeof(BlobEntry));
@@ -728,20 +717,20 @@ int b200ps_shard_export(b200ps_t* ps, int shard_id, void* blob, size_t cap, size
 }
 
 int b200ps_shard_import(b200ps_t* ps, int shard_id, const void* blob, size_t size) {
-  if (!ps || shard_id < 0 || shard_id >= ps->n_shards || !blob || size < sizeof(BlobHeader)) return fail(B200PS_EINVAL, "bad argument");
+  if (!ps || shard_id < 0 || shard_id >= ps->n_shards || !blob || size < sizeof(BlobHeader)) return E::fail(B200PS_EINVAL, "bad argument");
   Shard& sh = ps->shard[shard_id];
-  if (sh.local) return fail(B200PS_ESTATE, "shard is local to this process");
+  if (sh.local) return E::fail(B200PS_ESTATE, "shard is local to this process");
   BlobHeader h;
   memcpy(&h, blob, sizeof(h));
-  if (h.magic != kBlobMagic || h.shard != shard_id) return fail(B200PS_EINVAL, "blob does not describe this shard");
-  if (size < sizeof(h) + (size_t)h.n_entries * sizeof(BlobEntry)) return fail(B200PS_EINVAL, "truncated blob");
+  if (h.magic != kBlobMagic || h.shard != shard_id) return E::fail(B200PS_EINVAL, "blob does not describe this shard");
+  if (size < sizeof(h) + (size_t)h.n_entries * sizeof(BlobEntry)) return E::fail(B200PS_EINVAL, "truncated blob");
   DeviceGuard g(ps->client_device);
   const BlobEntry* e = (const BlobEntry*)((const char*)blob + sizeof(h));
   for (int i = 0; i < h.n_entries; ++i) {
     Alloc* a = nullptr;
     if (e[i].table < 0) a = &sh.ctl;
     else {
-      if (e[i].table >= (int)ps->tables.size()) return fail(B200PS_ESTATE, "peer registered a table this process has not (register on every process first)");
+      if (e[i].table >= (int)ps->tables.size()) return E::fail(B200PS_ESTATE, "peer registered a table this process has not (register on every process first)");
       a = &ps->tables[e[i].table].alloc[shard_id];
     }
     if (a->ptr) continue;  // already mapped
@@ -762,9 +751,9 @@ int b200ps_shard_import(b200ps_t* ps, int shard_id, const void* blob, size_t siz
 }
 
 int b200ps_lookup(b200ps_t* ps, const char* name) {
-  if (!ps || !name) return fail(B200PS_EINVAL, "bad argument");
+  if (!ps || !name) return E::fail(B200PS_EINVAL, "bad argument");
   auto it = ps->by_name.find(name);
-  if (it == ps->by_name.end()) return fail(B200PS_ENOTFOUND, std::string(name) + " not in Parameter");
+  if (it == ps->by_name.end()) return E::fail(B200PS_ENOTFOUND, std::string(name) + " not in Parameter");
   return it->second;
 }
 
@@ -775,7 +764,7 @@ static bool is_borrowed_view(b200ps_t* ps) {
 }
 
 static int register_common(b200ps_t* ps, Table&& t) {
-  if (is_borrowed_view(ps)) return fail(B200PS_ESTATE, "tables are registered on the owning group, then b200ps_clone_view again");
+  if (is_borrowed_view(ps)) return E::fail(B200PS_ESTATE, "tables are registered on the owning group, then b200ps_clone_view again");
   t.n_slots = opt_slots(ps->opt.kind);
   int id = (int)ps->tables.size();
   ps->tables.push_back(std::move(t));
@@ -793,7 +782,7 @@ static int register_common(b200ps_t* ps, Table&& t) {
 
 int b200ps_table_register(b200ps_t* ps, const char* name, int dim, const char* initializer, int64_t capacity,
                           uint64_t seed) {
-  if (!ps || !name || dim < 1 || capacity < 1) return fail(B200PS_EINVAL, "bad table definition");
+  if (!ps || !name || dim < 1 || capacity < 1) return E::fail(B200PS_EINVAL, "bad table definition");
   std::lock_guard<std::mutex> lk(ps->mu);
   auto it = ps->by_name.find(name);
   if (it != ps->by_name.end()) return it->second;  // model.go:57-63 idempotent
@@ -820,11 +809,11 @@ int b200ps_table_register(b200ps_t* ps, const char* name, int dim, const char* i
 
 int b200ps_table_register_pair(b200ps_t* ps, const char* name_a, const char* name_b, const char* initializer,
                                int64_t capacity, uint64_t seed) {
-  if (!ps || !name_a || !name_b || capacity < 1) return fail(B200PS_EINVAL, "bad table definition");
+  if (!ps || !name_a || !name_b || capacity < 1) return E::fail(B200PS_EINVAL, "bad table definition");
   std::lock_guard<std::mutex> lk(ps->mu);
   auto ia = ps->by_name.find(name_a), ib = ps->by_name.find(name_b);
   if (ia != ps->by_name.end() && ib != ps->by_name.end()) return ia->second;
-  if (ia != ps->by_name.end() || ib != ps->by_name.end()) return fail(B200PS_ESTATE, "one table of the pair is already registered");
+  if (ia != ps->by_name.end() || ib != ps->by_name.end()) return E::fail(B200PS_ESTATE, "one table of the pair is already registered");
   const int slots = opt_slots(ps->opt.kind);
   const int64_t sec = 12;  // [A(8) | B(1) | pad(3)] floats
   Table a;
@@ -841,7 +830,7 @@ int b200ps_table_register_pair(b200ps_t* ps, const char* name_a, const char* nam
   a.uniform = initializer && strcmp(initializer, "uniform") == 0;
   a.seed = seed;
   a.pair_b = (int)ps->tables.size() + 1;
-  if (a.uniform) return fail(B200PS_EINVAL, "paired tables support the zero initializer only (set rows explicitly)");
+  if (a.uniform) return E::fail(B200PS_EINVAL, "paired tables support the zero initializer only (set rows explicitly)");
   int id_a = register_common(ps, std::move(a));
   if (id_a < 0) return id_a;
   Table b;
@@ -870,7 +859,7 @@ int b200ps_table_register_pair(b200ps_t* ps, const char* name_a, const char* nam
 
 int b200ps_table_register_hashed(b200ps_t* ps, const char* name, int dim, const char* initializer,
                                  int64_t expected_rows, uint64_t seed) {
-  if (!ps || !name || dim < 1 || expected_rows < 1) return fail(B200PS_EINVAL, "bad table definition");
+  if (!ps || !name || dim < 1 || expected_rows < 1) return E::fail(B200PS_EINVAL, "bad table definition");
   std::lock_guard<std::mutex> lk(ps->mu);
   auto it = ps->by_name.find(name);
   if (it != ps->by_name.end()) return it->second;
@@ -899,7 +888,7 @@ int b200ps_table_register_hashed(b200ps_t* ps, const char* name, int dim, const 
 }
 
 int b200ps_dense_register(b200ps_t* ps, const char* name, int shard, int64_t rows, int dim) {
-  if (!ps || !name || dim < 1 || rows < 1 || shard < 0 || shard >= ps->n_shards) return fail(B200PS_EINVAL, "bad dense parameter definition");
+  if (!ps || !name || dim < 1 || rows < 1 || shard < 0 || shard >= ps->n_shards) return E::fail(B200PS_EINVAL, "bad dense parameter definition");
   std::lock_guard<std::mutex> lk(ps->mu);
   auto it = ps->by_name.find(name);
   if (it != ps->by_name.end()) return it->second;
@@ -921,7 +910,7 @@ int b200ps_dense_register(b200ps_t* ps, const char* name, int shard, int64_t row
 }
 
 int b200ps_commit(b200ps_t* ps) {
-  if (!ps) return fail(B200PS_EINVAL, "null group");
+  if (!ps) return E::fail(B200PS_EINVAL, "null group");
   std::lock_guard<std::mutex> lk(ps->mu);
   DeviceGuard g(ps->client_device);
   int n = (int)ps->tables.size();
@@ -947,7 +936,7 @@ int b200ps_commit(b200ps_t* ps) {
 static int rows_copy(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream, bool write, int slot = 0) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (slot < 0 || slot > opt_slots(ps->opt.kind)) return fail(B200PS_EINVAL, "optimizer has no such slot");
+  if (slot < 0 || slot > opt_slots(ps->opt.kind)) return E::fail(B200PS_EINVAL, "optimizer has no such slot");
   DeviceGuard g(ps->client_device);
   Split sp;
   rc = split_segs(ps, segs, nseg, false, &sp);
@@ -961,15 +950,17 @@ static int rows_copy(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
       FlatArgs<1> fa;
       fill_flat(ps, sp, false, slot, &fa);
       DISPATCH_U(u_rt, {
-        if (write) { grid = flat_grid(ps, k_copy_flat<true, U, 1>, sp.flat_items, U); k_copy_flat<true, U, 1><<<grid, 256, 0, st>>>(fa); }
-        else { grid = flat_grid(ps, k_copy_flat<false, U, 1>, sp.flat_items, U); k_copy_flat<false, U, 1><<<grid, 256, 0, st>>>(fa); }
+        auto kern = write ? k_copy_flat<true, U, 1> : k_copy_flat<false, U, 1>;
+        if ((rc = flat_grid(ps, kern, sp.flat_items, U, &grid))) return rc;
+        kern<<<grid, 256, 0, st>>>(fa);
       });
     } else {
       FlatArgs<8> fa;
       fill_flat(ps, sp, false, slot, &fa);
       DISPATCH_U(u_rt, {
-        if (write) { grid = flat_grid(ps, k_copy_flat<true, U, 8>, sp.flat_items, U); k_copy_flat<true, U, 8><<<grid, 256, 0, st>>>(fa); }
-        else { grid = flat_grid(ps, k_copy_flat<false, U, 8>, sp.flat_items, U); k_copy_flat<false, U, 8><<<grid, 256, 0, st>>>(fa); }
+        auto kern = write ? k_copy_flat<true, U, 8> : k_copy_flat<false, U, 8>;
+        if ((rc = flat_grid(ps, kern, sp.flat_items, U, &grid))) return rc;
+        kern<<<grid, 256, 0, st>>>(fa);
       });
     }
     ps->launches++;
@@ -998,7 +989,7 @@ int b200ps_set_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stre
 static int dense_copy(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* stream, bool write, int slot = 0) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (slot < 0 || slot > opt_slots(ps->opt.kind)) return fail(B200PS_EINVAL, "optimizer has no such slot");
+  if (slot < 0 || slot > opt_slots(ps->opt.kind)) return E::fail(B200PS_EINVAL, "optimizer has no such slot");
   DeviceGuard g(ps->client_device);
   Split sp;
   rc = split_segs(ps, segs, nseg, true, &sp);
@@ -1028,7 +1019,7 @@ int b200ps_slot_dense(b200ps_t* ps, int slot, int write, const b200ps_seg_t* seg
 static int push_begin_impl(b200ps_t* ps, float lr, const int32_t* mv, void* stream, int bump_only, int only_shard = -1) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (only_shard >= ps->n_shards) return fail(B200PS_EINVAL, "bad shard id");
+  if (only_shard >= ps->n_shards) return E::fail(B200PS_EINVAL, "bad shard id");
   DeviceGuard g(ps->client_device);
   VersionsIn v{};
   for (int s = 0; s < ps->n_shards; ++s) v.v[s] = mv ? mv[s] : 0;
@@ -1045,29 +1036,29 @@ int b200ps_push_begin(b200ps_t* ps, float learning_rate, const int32_t* model_ve
   return push_begin_impl(ps, learning_rate, model_versions, stream, 0);
 }
 int b200ps_set_lr_schedule(b200ps_t* ps, const b200ps_lr_schedule_t* s) {
-  if (!ps) return fail(B200PS_EINVAL, "null group");
+  if (!ps) return E::fail(B200PS_EINVAL, "null group");
   if (!s) {
     ps->lr_sched = b200ps_lr_schedule_t{};
     return B200PS_OK;
   }
   if (s->kind < B200PS_LR_PIECEWISE || s->kind > B200PS_LR_POLYNOMIAL)
-    return fail(B200PS_EINVAL, "unknown learning-rate schedule kind " + std::to_string(s->kind));
+    return E::fail(B200PS_EINVAL, "unknown learning-rate schedule kind " + std::to_string(s->kind));
   if (s->kind == B200PS_LR_PIECEWISE) {
     if (s->n_boundaries < 0 || s->n_boundaries > B200PS_LR_MAX_BOUNDARIES)
-      return fail(B200PS_EINVAL, "PiecewiseConstantDecay takes 0 to " + std::to_string(B200PS_LR_MAX_BOUNDARIES) +
-                                     " boundaries, not " + std::to_string(s->n_boundaries));
+      return E::fail(B200PS_EINVAL, "PiecewiseConstantDecay takes 0 to " + std::to_string(B200PS_LR_MAX_BOUNDARIES) +
+                                        " boundaries, not " + std::to_string(s->n_boundaries));
     for (int i = 0; i < s->n_boundaries; ++i) {
-      if (!std::isfinite(s->boundaries[i])) return fail(B200PS_EINVAL, "PiecewiseConstantDecay: a boundary is not finite");
+      if (!std::isfinite(s->boundaries[i])) return E::fail(B200PS_EINVAL, "PiecewiseConstantDecay: a boundary is not finite");
       if (i > 0 && !(s->boundaries[i] > s->boundaries[i - 1]))
-        return fail(B200PS_EINVAL, "PiecewiseConstantDecay: boundaries must be strictly increasing");
+        return E::fail(B200PS_EINVAL, "PiecewiseConstantDecay: boundaries must be strictly increasing");
     }
     for (int i = 0; i <= s->n_boundaries; ++i)
-      if (!std::isfinite(s->values[i])) return fail(B200PS_EINVAL, "PiecewiseConstantDecay: a value is not finite");
+      if (!std::isfinite(s->values[i])) return E::fail(B200PS_EINVAL, "PiecewiseConstantDecay: a value is not finite");
   } else {
     const double p[] = {s->initial_learning_rate, s->decay_steps, s->decay_rate, s->end_learning_rate, s->power};
     for (double x : p)
-      if (!std::isfinite(x)) return fail(B200PS_EINVAL, "learning-rate schedule: a parameter is not finite");
-    if (!(s->decay_steps > 0)) return fail(B200PS_EINVAL, "learning-rate schedule: decay_steps must be > 0");
+      if (!std::isfinite(x)) return E::fail(B200PS_EINVAL, "learning-rate schedule: a parameter is not finite");
+    if (!(s->decay_steps > 0)) return E::fail(B200PS_EINVAL, "learning-rate schedule: decay_steps must be > 0");
   }
   ps->lr_sched = *s;
   return B200PS_OK;
@@ -1075,7 +1066,7 @@ int b200ps_set_lr_schedule(b200ps_t* ps, const b200ps_lr_schedule_t* s) {
 
 int b200ps_bump_step(b200ps_t* ps, void* stream) { return push_begin_impl(ps, 0.f, nullptr, stream, 1); }
 int b200ps_push_begin_shard(b200ps_t* ps, int shard, float learning_rate, const int32_t* model_versions, void* stream) {
-  if (shard < 0) return fail(B200PS_EINVAL, "bad shard id");
+  if (shard < 0) return E::fail(B200PS_EINVAL, "bad shard id");
   return push_begin_impl(ps, learning_rate, model_versions, stream, 0, shard);
 }
 
@@ -1115,14 +1106,14 @@ int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
       FlatArgs<1> fa;
       fill_flat(ps, sp, true, 0, &fa);
       DISPATCH_OPT(o.kind, DISPATCH_U(u_rt, {
-        grid = flat_grid(ps, k_push_flat<OPT, U, 1>, sp.flat_items, U);
+        if ((rc = flat_grid(ps, k_push_flat<OPT, U, 1>, sp.flat_items, U, &grid))) return rc;
         k_push_flat<OPT, U, 1><<<grid, 256, 0, st>>>(fa, o);
       }));
     } else {
       FlatArgs<8> fa;
       fill_flat(ps, sp, true, 0, &fa);
       DISPATCH_OPT(o.kind, DISPATCH_U(u_rt, {
-        grid = flat_grid(ps, k_push_flat<OPT, U, 8>, sp.flat_items, U);
+        if ((rc = flat_grid(ps, k_push_flat<OPT, U, 8>, sp.flat_items, U, &grid))) return rc;
         k_push_flat<OPT, U, 8><<<grid, 256, 0, st>>>(fa, o);
       }));
     }
@@ -1140,13 +1131,13 @@ int b200ps_push_rows(b200ps_t* ps, const b200ps_seg_t* segs, int nseg, void* str
 
 static int pair_batch(b200ps_t* ps, const b200ps_seg_t* segs_a, float* const* rows_b, int nseg, PairBatch* pb,
                       long long* max_n) {
-  if (nseg < 1 || nseg > kMaxSegs / 2) return fail(B200PS_EINVAL, "pair launches take 1.." + std::to_string(kMaxSegs / 2) + " segments");
+  if (nseg < 1 || nseg > kMaxSegs / 2) return E::fail(B200PS_EINVAL, "pair launches take 1.." + std::to_string(kMaxSegs / 2) + " segments");
   *max_n = 0;
   for (int i = 0; i < nseg; ++i) {
     const b200ps_seg_t& sg = segs_a[i];
     if (sg.table < 0 || sg.table >= (int)ps->tables.size() || ps->tables[sg.table].pair_b < 0)
-      return fail(B200PS_EINVAL, "segment table is not the first table of a registered pair");
-    if (!aligned16(sg.rows_dev) || !rows_b[i]) return fail(B200PS_EINVAL, "pair rows must be 16 B aligned / non-null");
+      return E::fail(B200PS_EINVAL, "segment table is not the first table of a registered pair");
+    if (!aligned16(sg.rows_dev) || !rows_b[i]) return E::fail(B200PS_EINVAL, "pair rows must be 16 B aligned / non-null");
     pb->a[i] = sg;
     pb->rows_b[i] = rows_b[i];
     pb->table_b[i] = ps->tables[sg.table].pair_b;
@@ -1199,35 +1190,35 @@ int b200ps_push_rows_pair(b200ps_t* ps, const b200ps_seg_t* segs_a, float* const
 
 // ---- owner-computes exchange (ps_exchange.cuh) ----------------------------------
 int b200ps_xchg_create(b200ps_t* ps, int G, int B, const int32_t* deep_tables, const int32_t* wide_tables) {
-  if (!ps || B < 1 || !deep_tables || !wide_tables) return fail(B200PS_EINVAL, "bad exchange definition");
-  if (G < 1 || G > kXMaxG) return fail(B200PS_EINVAL, "the exchange moves 1 to " + std::to_string(kXMaxG) + " table pairs");
-  if (ps->x_table >= 0) return fail(B200PS_ESTATE, "exchange already created");
+  if (!ps || B < 1 || !deep_tables || !wide_tables) return E::fail(B200PS_EINVAL, "bad exchange definition");
+  if (G < 1 || G > kXMaxG) return E::fail(B200PS_EINVAL, "the exchange moves 1 to " + std::to_string(kXMaxG) + " table pairs");
+  if (ps->x_table >= 0) return E::fail(B200PS_ESTATE, "exchange already created");
   int me = -1, n_local = 0;
   for (int s = 0; s < ps->n_shards; ++s)
     if (ps->shard[s].local) { me = s; ++n_local; }
-  if (n_local != 1) return fail(B200PS_ESTATE, "the exchange needs exactly one local shard per process (rank-per-GPU)");
+  if (n_local != 1) return E::fail(B200PS_ESTATE, "the exchange needs exactly one local shard per process (rank-per-GPU)");
   // the owner-side constants of every pair on my shard: the exchange kernels take them instead of the table directory
   XTabs xt{};
   xt.shard_shift = group_view(ps).shard_shift;
   for (int g = 0; g < G; ++g) {
     if (deep_tables[g] < 0 || deep_tables[g] >= (int)ps->tables.size() || wide_tables[g] < 0 ||
         wide_tables[g] >= (int)ps->tables.size())
-      return fail(B200PS_ENOTFOUND, "unknown table id in exchange definition");
+      return E::fail(B200PS_ENOTFOUND, "unknown table id in exchange definition");
     const Table& d = ps->tables[deep_tables[g]];
     const Table& w = ps->tables[wide_tables[g]];
-    if (d.dim != 8 || w.dim != 1) return fail(B200PS_EWIDTH, "the exchange moves dim-8 / dim-1 table pairs");
+    if (d.dim != 8 || w.dim != 1) return E::fail(B200PS_EWIDTH, "the exchange moves dim-8 / dim-1 table pairs");
     if (d.hashed || w.hashed || d.is_dense || w.is_dense || d.owner >= 0 || w.owner >= 0 || d.raw || w.raw)
-      return fail(B200PS_EINVAL, "the exchange moves direct-indexed tables striped over every shard "
-                                 "(not hashed, dense, pinned to one shard or raw)");
+      return E::fail(B200PS_EINVAL, "the exchange moves direct-indexed tables striped over every shard "
+                                    "(not hashed, dense, pinned to one shard or raw)");
     for (int j = 0; j <= kMaxSlots; ++j) {
       if (g == 0) {
         xt.deep_soff[j] = (int)d.slot_off[j];
         xt.wide_soff[j] = (int)w.slot_off[j];
       } else if (xt.deep_soff[j] != (int)d.slot_off[j] || xt.wide_soff[j] != (int)w.slot_off[j]) {
-        return fail(B200PS_EINVAL, "the exchanged deep tables, and the wide tables, need one slot layout each");
+        return E::fail(B200PS_EINVAL, "the exchanged deep tables, and the wide tables, need one slot layout each");
       }
     }
-    if (!d.alloc[me].ptr || !w.alloc[me].ptr) return fail(B200PS_ESTATE, "an exchanged table is not allocated on the local shard");
+    if (!d.alloc[me].ptr || !w.alloc[me].ptr) return E::fail(B200PS_ESTATE, "an exchanged table is not allocated on the local shard");
     xt.deep[g] = (float*)((char*)d.alloc[me].ptr + d.base_off);
     xt.wide[g] = (float*)((char*)w.alloc[me].ptr + w.base_off);
     xt.deep_pres[g] = d.present_off ? (uint32_t*)((char*)d.alloc[me].ptr + d.present_off) : nullptr;
@@ -1269,10 +1260,10 @@ int b200ps_xchg_create(b200ps_t* ps, int G, int B, const int32_t* deep_tables, c
 static int xview(b200ps_t* ps, XView* x) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (ps->x_table < 0) return fail(B200PS_ESTATE, "b200ps_xchg_create not called");
+  if (ps->x_table < 0) return E::fail(B200PS_ESTATE, "b200ps_xchg_create not called");
   const Table& t = ps->tables[ps->x_table];
   for (int s = 0; s < ps->n_shards; ++s) {
-    if (!t.alloc[s].ptr) return fail(B200PS_ESTATE, "exchange buffer of shard " + std::to_string(s) + " is not mapped (sync peers)");
+    if (!t.alloc[s].ptr) return E::fail(B200PS_ESTATE, "exchange buffer of shard " + std::to_string(s) + " is not mapped (sync peers)");
     x->buf[s] = (char*)t.alloc[s].ptr;
   }
   x->off_ids = ps->x_off_ids;
@@ -1342,7 +1333,7 @@ int b200ps_xchg_push(b200ps_t* ps, const float* gsum_deep_dev, const float* gsum
   XView x;
   int rc = xview(ps, &x);
   if (rc) return rc;
-  if (!ps->x_pulled) return fail(B200PS_ESTATE, "b200ps_xchg_push follows the b200ps_xchg_pull of the same id lists");
+  if (!ps->x_pulled) return E::fail(B200PS_ESTATE, "b200ps_xchg_push follows the b200ps_xchg_pull of the same id lists");
   ps->x_pulled = false;
   DeviceGuard g(ps->client_device);
   xchg_push_kernels(ps, x, gsum_deep_dev, gsum_wide_dev, (cudaStream_t)stream);
@@ -1374,7 +1365,7 @@ int b200ps_xchg_profile(b200ps_t* ps, const int64_t* uniq_dev, const int32_t* n_
 
 // ---- raw peer-visible buffers + device-side barrier (the allreduce controller's data path) ----
 int b200ps_raw_register(b200ps_t* ps, const char* name, size_t bytes) {
-  if (!ps || !name || bytes < 1) return fail(B200PS_EINVAL, "bad raw buffer definition");
+  if (!ps || !name || bytes < 1) return E::fail(B200PS_EINVAL, "bad raw buffer definition");
   std::lock_guard<std::mutex> lk(ps->mu);
   auto it = ps->by_name.find(name);
   if (it != ps->by_name.end()) return it->second;
@@ -1391,10 +1382,10 @@ int b200ps_raw_register(b200ps_t* ps, const char* name, size_t bytes) {
 
 int b200ps_raw_ptr(b200ps_t* ps, int table, int shard, void** ptr, size_t* bytes) {
   if (!ps || table < 0 || table >= (int)ps->tables.size() || shard < 0 || shard >= ps->n_shards || !ptr)
-    return fail(B200PS_EINVAL, "bad argument");
+    return E::fail(B200PS_EINVAL, "bad argument");
   const Table& t = ps->tables[table];
-  if (!t.raw) return fail(B200PS_EINVAL, t.name + " is not a raw buffer");
-  if (!t.alloc[shard].ptr) return fail(B200PS_ESTATE, "shard not attached (sync peers after registering)");
+  if (!t.raw) return E::fail(B200PS_EINVAL, t.name + " is not a raw buffer");
+  if (!t.alloc[shard].ptr) return E::fail(B200PS_ESTATE, "shard not attached (sync peers after registering)");
   *ptr = t.alloc[shard].ptr;
   if (bytes) *bytes = t.alloc[shard].bytes;
   return B200PS_OK;
@@ -1404,10 +1395,10 @@ int b200ps_table_rows_ptr(b200ps_t* ps, int table, int shard, float** base, int6
                           int64_t* rows) {
   if (!ps || table < 0 || table >= (int)ps->tables.size() || shard < 0 || shard >= ps->n_shards || !base ||
       !row_stride || !param_off || !rows)
-    return fail(B200PS_EINVAL, "bad argument");
+    return E::fail(B200PS_EINVAL, "bad argument");
   const Table& t = ps->tables[table];
-  if (t.raw || t.is_dense || t.hashed) return fail(B200PS_EINVAL, t.name + " is not a direct-indexed embedding table");
-  if (!t.alloc[shard].ptr) return fail(B200PS_ESTATE, "shard not attached (sync peers after registering)");
+  if (t.raw || t.is_dense || t.hashed) return E::fail(B200PS_EINVAL, t.name + " is not a direct-indexed embedding table");
+  if (!t.alloc[shard].ptr) return E::fail(B200PS_ESTATE, "shard not attached (sync peers after registering)");
   *base = (float*)((char*)t.alloc[shard].ptr + t.base_off);
   *row_stride = t.row_stride;
   *param_off = t.slot_off[0];
@@ -1421,7 +1412,7 @@ int b200ps_barrier(b200ps_t* ps, void* stream) {
   int me = -1, n_local = 0;
   for (int s = 0; s < ps->n_shards; ++s)
     if (ps->shard[s].local) { me = s; ++n_local; }
-  if (n_local != 1) return fail(B200PS_ESTATE, "b200ps_barrier needs exactly one local shard per process (rank-per-GPU)");
+  if (n_local != 1) return E::fail(B200PS_ESTATE, "b200ps_barrier needs exactly one local shard per process (rank-per-GPU)");
   DeviceGuard g(ps->client_device);
   k_group_barrier<<<1, 32, 0, (cudaStream_t)stream>>>(group_view(ps), me, ps->d_err);
   ps->launches++;
@@ -1453,11 +1444,11 @@ static int push_dense_reduce_impl(b200ps_t* ps, int dense_id, const float* const
                                   float scale, int divide, const float* param_dev, const float* adam, void* stream) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (dense_id < 0 || dense_id >= (int)ps->tables.size() || !ps->tables[dense_id].is_dense) return fail(B200PS_ENOTFOUND, "not a dense parameter");
-  if (n_replicas < 1 || n_replicas > kMaxShards || !grads_dev) return fail(B200PS_EINVAL, "n_replicas out of range");
-  if (divide && scale == 0.0f) return fail(B200PS_EINVAL, "divisor is zero");
+  if (dense_id < 0 || dense_id >= (int)ps->tables.size() || !ps->tables[dense_id].is_dense) return E::fail(B200PS_ENOTFOUND, "not a dense parameter");
+  if (n_replicas < 1 || n_replicas > kMaxShards || !grads_dev) return E::fail(B200PS_EINVAL, "n_replicas out of range");
+  if (divide && scale == 0.0f) return E::fail(B200PS_EINVAL, "divisor is zero");
   if (param_dev && ps->opt.kind != kSGD && ps->opt.kind != kMomentum && ps->opt.kind != kAdam && ps->opt.kind != kAMSGrad)
-    return fail(B200PS_EINVAL, "the torch allreduce update covers SGD, momentum, Adam and AMSGrad only");
+    return E::fail(B200PS_EINVAL, "the torch allreduce update covers SGD, momentum, Adam and AMSGrad only");
   DeviceGuard g(ps->client_device);
   const Table& t = ps->tables[dense_id];
   ReplicaGrads rg{};
@@ -1508,7 +1499,7 @@ int b200ps_push_dense_reduce(b200ps_t* ps, int dense_id, const float* const* gra
 int b200ps_push_dense_allreduce(b200ps_t* ps, int dense_id, const float* param_dev, const float* const* grads_dev,
                                 int n_replicas, float scale, float alpha, float epsilon, float one_minus_beta1,
                                 float one_minus_beta2, void* stream) {
-  if (!param_dev) return fail(B200PS_EINVAL, "param_dev is null");
+  if (!param_dev) return E::fail(B200PS_EINVAL, "param_dev is null");
   const float adam[4] = {alpha, epsilon, one_minus_beta1, one_minus_beta2};
   return push_dense_reduce_impl(ps, dense_id, grads_dev, n_replicas, scale, 0, param_dev, adam, stream);
 }
@@ -1518,7 +1509,7 @@ int b200ps_push_end(b200ps_t* ps, int32_t* versions_out_host, void* stream) {
   return push_end_impl(ps, versions_out_host, stream, -1);
 }
 int b200ps_push_end_shard(b200ps_t* ps, int shard, void* stream) {
-  if (!ps || shard < 0 || shard >= ps->n_shards) return fail(B200PS_EINVAL, "bad shard id");
+  if (!ps || shard < 0 || shard >= ps->n_shards) return E::fail(B200PS_EINVAL, "bad shard id");
   return push_end_impl(ps, nullptr, stream, shard);
 }
 static int push_end_impl(b200ps_t* ps, int32_t* versions_out_host, void* stream, int only_shard) {
@@ -1540,7 +1531,7 @@ static int push_end_impl(b200ps_t* ps, int32_t* versions_out_host, void* stream,
 template <int OPT>
 static int raw_dense(const float* g, float* p, float* s0, float* s1, float* s2, long long n, float lr, float alpha,
                      float l2adj, const OptParams& o, void* stream) {
-  if (!g || !p || n < 0) return fail(B200PS_EINVAL, "null array");
+  if (!g || !p || n < 0) return E::fail(B200PS_EINVAL, "null array");
   if (n == 0) return B200PS_OK;
   bool vec = n % 4 == 0 && aligned16(g) && aligned16(p) && (!s0 || aligned16(s0)) && (!s1 || aligned16(s1)) &&
              (!s2 || aligned16(s2));
@@ -1564,7 +1555,7 @@ int b200ps_kernel_sgd(const float* grad, float* param, float lr, long long size,
 
 int b200ps_kernel_momentum(const float* grad, float* param, float* velocity, float mu, int nesterov, float lr,
                            long long size, void* stream) {
-  if (!velocity) return fail(B200PS_EINVAL, "null velocity");
+  if (!velocity) return E::fail(B200PS_EINVAL, "null velocity");
   OptParams o{};
   o.kind = kMomentum;
   o.mu = mu;
@@ -1574,7 +1565,7 @@ int b200ps_kernel_momentum(const float* grad, float* param, float* velocity, flo
 
 int b200ps_kernel_adam(const float* grad, float* param, float* m, float* v, float lr, long long size, long long step,
                        float beta1, float beta2, float epsilon, float* max_square, void* stream) {
-  if (!m || !v) return fail(B200PS_EINVAL, "null moment array");
+  if (!m || !v) return E::fail(B200PS_EINVAL, "null moment array");
   OptParams o{};
   o.kind = max_square ? kAMSGrad : kAdam;
   o.beta1 = beta1;
@@ -1591,7 +1582,7 @@ int b200ps_kernel_adam(const float* grad, float* param, float* m, float* v, floa
 
 int b200ps_kernel_adagrad(const float* grad, float* param, float* m, float lr, long long size, float epsilon,
                           void* stream) {
-  if (!m) return fail(B200PS_EINVAL, "null accumulator");
+  if (!m) return E::fail(B200PS_EINVAL, "null accumulator");
   OptParams o{};
   o.kind = kAdagrad;
   o.epsilon = epsilon;
@@ -1637,9 +1628,9 @@ static size_t g_dbg_bytes = 0;
 static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int64_t k, const int64_t* bounds,
                        int64_t* uniq_dev, int32_t* inv_dev, int32_t* n_unique_dev, void* workspace_dev,
                        size_t workspace_bytes, void* stream, int blocks_per_sm = 0, const int32_t* widths = nullptr) {
-  if (T < 1 || T > 65535 || k < 1 || k > (1LL << 29)) return fail(B200PS_EINVAL, "bad unique shape");
-  if (!ids_dev || !uniq_dev || !inv_dev || !n_unique_dev || !workspace_dev) return fail(B200PS_EINVAL, "null argument");
-  if (workspace_bytes < b200ps_unique_workspace(T, k)) return fail(B200PS_EINVAL, "unique workspace too small");
+  if (T < 1 || T > 65535 || k < 1 || k > (1LL << 29)) return E::fail(B200PS_EINVAL, "bad unique shape");
+  if (!ids_dev || !uniq_dev || !inv_dev || !n_unique_dev || !workspace_dev) return E::fail(B200PS_EINVAL, "null argument");
+  if (workspace_bytes < b200ps_unique_workspace(T, k)) return E::fail(B200PS_EINVAL, "unique workspace too small");
   if (bounds && workspace_bytes < b200ps_unique_bounded_workspace(T, k, bounds)) bounds = nullptr;  // no room: hash everything
   const int dev = client_dev(ps);
   DeviceGuard g(dev);
@@ -1650,20 +1641,15 @@ static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int6
   a.k = k;
   a.T = T;
   a.cap = uniq_cap(k);
-  // co-resident grid (the kernel synchronises its phases with a grid barrier)
-  static int occ[64] = {0};
-  static int sms[64] = {0};
-  if (dev < 64 && occ[dev] == 0) {
-    int o = 0, n = 0;
-    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_unique, kUThreads, 0));
-    CUDA_OK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-    occ[dev] = o < 1 ? 1 : (o > 4 ? 4 : o);
-    sms[dev] = n < 1 ? 1 : n;
-  }
-  long long max_blocks = dev < 64 ? (long long)occ[dev] * sms[dev] : 132;
+  // co-resident grid (the kernel synchronises its phases with a grid barrier), at most 4 blocks per SM
+  entry::Device d;
+  int occ = 0;
+  if (int rc = E::device(&d)) return rc;
+  if (int rc = E::blocks_per_sm(k_unique, kUThreads, 0, &occ)) return rc;
+  long long max_blocks = (long long)(occ > 4 ? 4 : occ) * d.sms;
   // a caller that overlaps the dedup with other kernels (lookahead pipeline) asks for a thin grid: the
   // persistent blocks hold their registers for the whole call, including the time spent at the grid barriers
-  if (blocks_per_sm > 0 && dev < 64 && (long long)blocks_per_sm * sms[dev] < max_blocks) max_blocks = (long long)blocks_per_sm * sms[dev];
+  if (blocks_per_sm > 0 && (long long)blocks_per_sm * d.sms < max_blocks) max_blocks = (long long)blocks_per_sm * d.sms;
   a.ntiles = (int)((k + kUUnit - 1) / kUUnit);  // units per segment
   char* p = (char*)workspace_dev;
   a.keys = (long long*)p; p += align256((size_t)T * a.cap * 8);
@@ -1744,11 +1730,11 @@ static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int6
   if (any_large) CUDA_OK(cudaMemsetAsync(a.hdr + 4, 0, 8, st));  // the grid-barrier counter
   UIdLayout idl{};
   if (widths != nullptr) {  // packed ids: segment t holds k elements of widths[t] bytes, segments back to back, 16 B aligned
-    if (T > kMaxSegs) return fail(B200PS_EINVAL, "per-segment id widths need T <= " + std::to_string(kMaxSegs));
+    if (T > kMaxSegs) return E::fail(B200PS_EINVAL, "per-segment id widths need T <= " + std::to_string(kMaxSegs));
     long long off = 0;
     for (int t = 0; t < T; ++t) {
       const int w = widths[t];
-      if (w != 1 && w != 2 && w != 4 && w != 8) return fail(B200PS_EINVAL, "id width must be 1, 2, 4 or 8 bytes");
+      if (w != 1 && w != 2 && w != 4 && w != 8) return E::fail(B200PS_EINVAL, "id width must be 1, 2, 4 or 8 bytes");
       idl.off[t] = off;
       idl.width[t] = (unsigned char)w;
       off += ((long long)k * w + 15) / 16 * 16;
@@ -1756,13 +1742,8 @@ static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int6
     a.ids32 = 2;
   }
   if (us.n > 0) {
-    static bool attr_done[64] = {};
-    if (dev < 64 && !attr_done[dev]) {
-      CUDA_OK(cudaFuncSetAttribute(k_unique_small<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kUSmallMax * 4));
-      CUDA_OK(cudaFuncSetAttribute(k_unique_small<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kUSmallMax * 4));
-      CUDA_OK(cudaFuncSetAttribute(k_unique_small<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kUSmallMax * 4));
-      attr_done[dev] = true;
-    }
+    auto small = k <= 8LL * kUSThreads ? k_unique_small<8> : k <= 16LL * kUSThreads ? k_unique_small<16> : k_unique_small<32>;
+    if (int rc = E::raise_smem_limit(small, kUSmallMax * 4)) return rc;
     const size_t smem = (size_t)small_bound * 4;
     // with a handle and work for both kernels the small-segment kernel runs on the handle's side stream, beside
     // the grid-wide one (fork / join through events: also valid inside a stream capture); they share no output
@@ -1778,9 +1759,7 @@ static int unique_impl(b200ps_t* ps, const void* ids_dev, int ids32, int T, int6
       CUDA_OK(cudaEventRecord(ps->u_fork, st));
       CUDA_OK(cudaStreamWaitEvent(ss, ps->u_fork, 0));
     }
-    if (k <= 8LL * kUSThreads) k_unique_small<8><<<(unsigned)us.n, kUSThreads, smem, ss>>>(a, idl, us);
-    else if (k <= 16LL * kUSThreads) k_unique_small<16><<<(unsigned)us.n, kUSThreads, smem, ss>>>(a, idl, us);
-    else k_unique_small<32><<<(unsigned)us.n, kUSThreads, smem, ss>>>(a, idl, us);
+    small<<<(unsigned)us.n, kUSThreads, smem, ss>>>(a, idl, us);
     count_launch(ps, 1);
     if (fork) CUDA_OK(cudaEventRecord(ps->u_join, ss));
     if (any_large) {
@@ -1826,7 +1805,7 @@ int b200ps_unique_bounded_ex(b200ps_t* ps, const void* ids_dev, int ids_are_int3
 int b200ps_unique_packed(b200ps_t* ps, const void* ids_dev, const int32_t* widths, int T, int64_t k, const int64_t* bounds,
                          int64_t* uniq_dev, int32_t* inv_dev, int32_t* n_unique_dev, void* workspace_dev,
                          size_t workspace_bytes, int blocks_per_sm, void* stream) {
-  if (!widths) return fail(B200PS_EINVAL, "widths is null");
+  if (!widths) return E::fail(B200PS_EINVAL, "widths is null");
   return unique_impl(ps, ids_dev, 2, T, k, bounds, uniq_dev, inv_dev, n_unique_dev, workspace_dev, workspace_bytes, stream,
                      blocks_per_sm, widths);
 }
@@ -1850,14 +1829,14 @@ static int dim_class(int dim, const void* a, const void* b) {
 
 int b200ps_segment_sum(b200ps_t* ps, const float* values_dev, const int32_t* inv_dev, int T, int64_t k, int dim,
                        float* out_dev, void* stream) {
-  if (T < 1 || T > 65535 || k < 1 || dim < 1) return fail(B200PS_EINVAL, "bad segment_sum shape");
+  if (T < 1 || T > 65535 || k < 1 || dim < 1) return E::fail(B200PS_EINVAL, "bad segment_sum shape");
   int c = dim_class(dim, values_dev, out_dev);
   int W = c == 0 ? 1 : 4 * c;
   // the kernel's 32-bit warp key is row * chunks + chunk (a 64-bit one made the dim-1 sum of a DeepFM batch 17 %
   // slower): refuse what would wrap it
   if (k * (dim / W) > INT32_MAX)
-    return fail(B200PS_EINVAL, "segment_sum: k * (dim / " + std::to_string(W) + ") = " + std::to_string(k * (dim / W)) +
-                                   " work items per segment, more than INT32_MAX (2147483647)");
+    return E::fail(B200PS_EINVAL, "segment_sum: k * (dim / " + std::to_string(W) + ") = " + std::to_string(k * (dim / W)) +
+                                      " work items per segment, more than INT32_MAX (2147483647)");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_OK(cudaMemsetAsync(out_dev, 0, (size_t)T * k * dim * sizeof(float), st));
@@ -1872,7 +1851,7 @@ int b200ps_segment_sum(b200ps_t* ps, const float* values_dev, const int32_t* inv
 
 int b200ps_gather_rows(b200ps_t* ps, const float* bet_dev, const int32_t* inv_dev, int T, int64_t k, int dim,
                        float* out_dev, void* stream) {
-  if (T < 1 || T > 65535 || k < 1 || dim < 1) return fail(B200PS_EINVAL, "bad gather shape");
+  if (T < 1 || T > 65535 || k < 1 || dim < 1) return E::fail(B200PS_EINVAL, "bad gather shape");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   int c = dim_class(dim, bet_dev, out_dev);
@@ -1889,12 +1868,12 @@ int b200ps_gather_rows(b200ps_t* ps, const float* bet_dev, const int32_t* inv_de
 // ---- pooled lookup of sparse input --------------------------------------------
 
 static int sparse_shape(int64_t B, int64_t nnz, int dim, const void* ws, size_t ws_bytes) {
-  if (B < 1 || nnz < 0 || dim < 1) return fail(B200PS_EINVAL, "sparse lookup: bad shape (B >= 1, nnz >= 0, dim >= 1)");
+  if (B < 1 || nnz < 0 || dim < 1) return E::fail(B200PS_EINVAL, "sparse lookup: bad shape (B >= 1, nnz >= 0, dim >= 1)");
   if (nnz + B > INT32_MAX)
-    return fail(B200PS_EINVAL, "sparse lookup: nnz + B = " + std::to_string(nnz + B) + " filled entries, more than INT32_MAX");
-  if (!ws || ((uintptr_t)ws & 15u)) return fail(B200PS_EINVAL, "sparse lookup: workspace null or not 16 B aligned");
+    return E::fail(B200PS_EINVAL, "sparse lookup: nnz + B = " + std::to_string(nnz + B) + " filled entries, more than INT32_MAX");
+  if (!ws || ((uintptr_t)ws & 15u)) return E::fail(B200PS_EINVAL, "sparse lookup: workspace null or not 16 B aligned");
   if (ws_bytes < b200ps_sparse_workspace(B, nnz, dim))
-    return fail(B200PS_EINVAL, "sparse lookup: workspace smaller than b200ps_sparse_workspace(B, nnz, dim)");
+    return E::fail(B200PS_EINVAL, "sparse lookup: workspace smaller than b200ps_sparse_workspace(B, nnz, dim)");
   return B200PS_OK;
 }
 
@@ -1906,7 +1885,7 @@ size_t b200ps_sparse_workspace(int64_t B, int64_t nnz, int dim) {
 int b200ps_sparse_prep(b200ps_t* ps, const int64_t* rows_dev, const void* vals_dev, int vals_are_int32, int64_t B,
                        int64_t nnz, int dim, int64_t* ids_dev, void* ws, size_t ws_bytes, void* stream) {
   if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
-  if (!ids_dev || (nnz > 0 && (!rows_dev || !vals_dev))) return fail(B200PS_EINVAL, "sparse_prep: null pointer");
+  if (!ids_dev || (nnz > 0 && (!rows_dev || !vals_dev))) return E::fail(B200PS_EINVAL, "sparse_prep: null pointer");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   const SparseLayout L(B, nnz, dim);
@@ -1934,11 +1913,11 @@ int b200ps_sparse_prep(b200ps_t* ps, const int64_t* rows_dev, const void* vals_d
 int b200ps_bag_prep(b200ps_t* ps, const void* ids_dev, int ids_are_int32, const int64_t* offsets_dev, int64_t width,
                     int include_last_offset, int64_t padding_idx, int64_t B, int64_t nnz, int dim, int64_t* out_ids_dev,
                     void* ws, size_t ws_bytes, void* stream) {
-  if (!ps) return fail(B200PS_EINVAL, "bag_prep: needs a group (its error word reports bad offsets and ids)");
+  if (!ps) return E::fail(B200PS_EINVAL, "bag_prep: needs a group (its error word reports bad offsets and ids)");
   if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
-  if (!out_ids_dev || (nnz > 0 && !ids_dev)) return fail(B200PS_EINVAL, "bag_prep: null pointer");
-  if (!offsets_dev && (width < 0 || width * B != nnz)) return fail(B200PS_EINVAL, "bag_prep: 2-D input needs nnz = B * width");
-  if (padding_idx < -1) return fail(B200PS_EINVAL, "bag_prep: padding_idx must be -1 (none) or >= 0");
+  if (!out_ids_dev || (nnz > 0 && !ids_dev)) return E::fail(B200PS_EINVAL, "bag_prep: null pointer");
+  if (!offsets_dev && (width < 0 || width * B != nnz)) return E::fail(B200PS_EINVAL, "bag_prep: 2-D input needs nnz = B * width");
+  if (padding_idx < -1) return E::fail(B200PS_EINVAL, "bag_prep: padding_idx must be -1 (none) or >= 0");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   const SparseLayout L(B, nnz, dim);
@@ -1974,9 +1953,9 @@ static int sparse_combine(b200ps_t* ps, const float* bet_dev, const int32_t* inv
   const char* fn = weighted ? "sparse_combine_weighted" : "sparse_combine";
   if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
   if (combiner < kSpSum || combiner > kSpSqrtn)
-    return fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
   if (!bet_dev || !inv_dev || !out_dev || (weighted && nnz > 0 && !weights_dev))
-    return fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   const SparseLayout L(B, nnz, dim);
@@ -2021,20 +2000,20 @@ static int sparse_combine_grad(b200ps_t* ps, const float* gout_dev, const int32_
   const char* fn = weighted ? "sparse_combine_weighted_grad" : "sparse_combine_grad";
   if (int rc = sparse_shape(B, nnz, dim, ws, ws_bytes)) return rc;
   if (combiner < kSpSum || combiner > kSpSqrtn)
-    return fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": combiner must be 0 (sum), 1 (mean) or 2 (sqrtn)");
   if (n_unique < 1 || n_unique > nnz + B)
-    return fail(B200PS_EINVAL, std::string(fn) + ": n_unique outside [1, nnz + B]");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": n_unique outside [1, nnz + B]");
   if (!gout_dev || !inv_dev || !gbet_dev || (weighted && nnz > 0 && !weights_dev))
-    return fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": null pointer");
   if (gweights_dev && combiner != kSpSum)
-    return fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient is defined for the sum combiner only");
-  if (gweights_dev && !bet_dev) return fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient needs bet_dev");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient is defined for the sum combiner only");
+  if (gweights_dev && !bet_dev) return E::fail(B200PS_EINVAL, std::string(fn) + ": the weight gradient needs bet_dev");
   const SparseLayout L(B, nnz, dim);
   const int c = dim_class(dim, gout_dev, gbet_dev);
   const int W = c == 0 ? 1 : 4 * c;
   if (L.K * (dim / W) > INT32_MAX)  // segment_sum_loop's 32-bit warp key, as in b200ps_segment_sum
-    return fail(B200PS_EINVAL, std::string(fn) + ": (nnz + B) * (dim / " + std::to_string(W) + ") = " +
-                                   std::to_string(L.K * (dim / W)) + " work items, more than INT32_MAX (2147483647)");
+    return E::fail(B200PS_EINVAL, std::string(fn) + ": (nnz + B) * (dim / " + std::to_string(W) + ") = " +
+                                      std::to_string(L.K * (dim / W)) + " work items, more than INT32_MAX (2147483647)");
   DeviceGuard g(client_dev(ps));
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_OK(cudaMemsetAsync(gbet_dev, 0, (size_t)n_unique * dim * sizeof(float), st));
@@ -2072,7 +2051,7 @@ int b200ps_sparse_combine_weighted_grad(b200ps_t* ps, const float* gout_dev, con
 // ---- state ---------------------------------------------------------------------
 
 int b200ps_shard_state(b200ps_t* ps, int shard, int32_t* version, int64_t* step, int32_t* initialized) {
-  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return fail(B200PS_EINVAL, "bad shard");
+  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return E::fail(B200PS_EINVAL, "bad shard");
   DeviceGuard g(ps->client_device);
   CUDA_OK(cudaDeviceSynchronize());
   ShardCtl c;
@@ -2084,7 +2063,7 @@ int b200ps_shard_state(b200ps_t* ps, int shard, int32_t* version, int64_t* step,
 }
 
 int b200ps_set_shard_state(b200ps_t* ps, int shard, int32_t version, int64_t step, int32_t initialized) {
-  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return fail(B200PS_EINVAL, "bad shard");
+  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return E::fail(B200PS_EINVAL, "bad shard");
   DeviceGuard g(ps->client_device);
   CUDA_OK(cudaDeviceSynchronize());
   ShardCtl c;
@@ -2099,7 +2078,7 @@ int b200ps_set_shard_state(b200ps_t* ps, int shard, int32_t version, int64_t ste
 int b200ps_snapshot_state(b200ps_t* ps, int64_t* out_host, void* stream) {
   int rc = ready(ps);
   if (rc) return rc;
-  if (!out_host) return fail(B200PS_EINVAL, "out_host is null");
+  if (!out_host) return E::fail(B200PS_EINVAL, "out_host is null");
   DeviceGuard g(ps->client_device);
   cudaStream_t st = (cudaStream_t)stream;
   k_snapshot<<<1, 32, 0, st>>>(group_view(ps), (long long*)ps->d_state);
@@ -2110,7 +2089,7 @@ int b200ps_snapshot_state(b200ps_t* ps, int64_t* out_host, void* stream) {
 }
 
 int b200ps_try_init(b200ps_t* ps, int shard, int* won) {
-  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached || !won) return fail(B200PS_EINVAL, "bad shard");
+  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached || !won) return E::fail(B200PS_EINVAL, "bad shard");
   DeviceGuard g(ps->client_device);
   CUDA_OK(cudaDeviceSynchronize());  // synchronous query on the legacy stream: order it after the caller's non-blocking streams
   k_try_init<<<1, 1>>>((ShardCtl*)ps->shard[shard].ctl.ptr, (int*)ps->d_count);
@@ -2123,7 +2102,7 @@ int b200ps_try_init(b200ps_t* ps, int shard, int* won) {
 }
 
 int b200ps_finish_init(b200ps_t* ps, int shard, int32_t version, void* stream) {
-  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return fail(B200PS_EINVAL, "bad shard");
+  if (!ps || shard < 0 || shard >= ps->n_shards || !ps->shard[shard].attached) return E::fail(B200PS_EINVAL, "bad shard");
   DeviceGuard g(ps->client_device);
   k_finish_init<<<1, 1, 0, (cudaStream_t)stream>>>((ShardCtl*)ps->shard[shard].ctl.ptr, version);
   ps->launches++;
@@ -2132,10 +2111,10 @@ int b200ps_finish_init(b200ps_t* ps, int shard, int32_t version, void* stream) {
 }
 
 static int present_scan(b200ps_t* ps, int table, int shard, int64_t* ids_dev, int64_t cap, int64_t* n) {
-  if (!ps || table < 0 || table >= (int)ps->tables.size() || shard < 0 || shard >= ps->n_shards || !n) return fail(B200PS_EINVAL, "bad argument");
+  if (!ps || table < 0 || table >= (int)ps->tables.size() || shard < 0 || shard >= ps->n_shards || !n) return E::fail(B200PS_EINVAL, "bad argument");
   const Table& t = ps->tables[table];
-  if (t.is_dense || (!t.present_off && !t.hashed)) return fail(B200PS_ESTATE, "created rows are not tracked for " + t.name);
-  if (!t.alloc[shard].ptr) return fail(B200PS_ESTATE, "shard not attached");
+  if (t.is_dense || (!t.present_off && !t.hashed)) return E::fail(B200PS_ESTATE, "created rows are not tracked for " + t.name);
+  if (!t.alloc[shard].ptr) return E::fail(B200PS_ESTATE, "shard not attached");
   DeviceGuard g(ps->client_device);
   CUDA_OK(cudaDeviceSynchronize());  // synchronous query on the legacy stream: order it after the caller's non-blocking streams
   CUDA_OK(cudaMemsetAsync(ps->d_count, 0, 8, 0));
@@ -2165,20 +2144,20 @@ int b200ps_table_ids(b200ps_t* ps, int table, int shard, int64_t* ids_dev, int64
 }
 
 int b200ps_check(b200ps_t* ps) {
-  if (!ps) return fail(B200PS_EINVAL, "null group");
+  if (!ps) return E::fail(B200PS_EINVAL, "null group");
   DeviceGuard g(ps->client_device);
   CUDA_OK(cudaDeviceSynchronize());
   unsigned e = 0;
   CUDA_OK(cudaMemcpy(&e, ps->d_err, 4, cudaMemcpyDeviceToHost));
   if (e) {
     CUDA_OK(cudaMemset(ps->d_err, 0, 4));
-    if (e & kErrTimeout) return fail(B200PS_ESTATE, "exchange wait timed out: a peer rank did not run the same step");
-    if (e & kErrFull) return fail(B200PS_ERANGE, "hashed embedding table is full (raise expected_rows)");
+    if (e & kErrTimeout) return E::fail(B200PS_ESTATE, "exchange wait timed out: a peer rank did not run the same step");
+    if (e & kErrFull) return E::fail(B200PS_ERANGE, "hashed embedding table is full (raise expected_rows)");
     if (e & kErrOffsets)
-      return fail(B200PS_EINVAL, "EmbeddingBag offsets must start at 0, be non-decreasing and end at most at the "
-                                 "number of ids");
-    if (e & kErrRange) return fail(B200PS_ERANGE, "embedding id outside the registered table capacity (or negative)");
-    return fail(B200PS_EINVAL, "device-side error word " + std::to_string(e));
+      return E::fail(B200PS_EINVAL, "EmbeddingBag offsets must start at 0, be non-decreasing and end at most at the "
+                                    "number of ids");
+    if (e & kErrRange) return E::fail(B200PS_ERANGE, "embedding id outside the registered table capacity (or negative)");
+    return E::fail(B200PS_EINVAL, "device-side error word " + std::to_string(e));
   }
   return B200PS_OK;
 }

@@ -16,20 +16,16 @@
 // writes the outputs, compacts the touched rows and resets the arrival counter.
 #include <cuda_runtime.h>
 
-#include <atomic>
 #include <cstdint>
 #include <string>
 
 #include "../../include/b200_census.h"
+#include "launch.cuh"
 
 namespace {
 
-thread_local std::string g_err;
-std::atomic<long long> g_launches{0};
-int fail(int code, const std::string& m) {
-  g_err = m;
-  return code;
-}
+using E = entry::Entry<entry::Census>;
+entry::LaunchCount g_launches{0};
 
 constexpr int TILE = B200_CENSUS_TILE;
 constexpr int THREADS = 288;  // 256 samples in the forward; 218 row columns + 50 dense sums in the sweep
@@ -43,7 +39,6 @@ constexpr int NDQ = 50;                    // dense sums: dz, dz x[24] @1, dz h1
 constexpr int CQ = 5;                      // per column: wide, slot 0, slot 1, slot 2, occurrences
 constexpr int Q = NDQ + NCOL * CQ;         // floats of one CTA's partial
 constexpr int SV = TILE + 1;               // padded: the dense sums read column q of row r conflict-free
-constexpr size_t WS_HEADER = 64;           // arrival counter
 
 struct Smem {
   int4 ent[3][TILE];   // the four ids of DNN input slot k of tile row r
@@ -244,8 +239,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_tower(b200_census_args_t 
     __syncthreads();
   }
 
-  unsigned* counter = reinterpret_cast<unsigned*>(a.workspace);
-  float* parts = reinterpret_cast<float*>(reinterpret_cast<char*>(a.workspace) + WS_HEADER);
+  unsigned* counter = entry::arrival_counter(a.workspace);
+  float* parts = entry::partials(a.workspace);
   float* mine = parts + (size_t)blockIdx.x * Q;
   if (cg >= 0) {
     float* c = mine + NDQ + t * CQ;
@@ -258,19 +253,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_tower(b200_census_args_t 
     mine[dq] = acc_q;
   }
   if (bad) atomicAdd(a.error, bad);
-  __threadfence();
-  __syncthreads();
-  if (t == 0) s.last = atomicAdd(counter, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s.last) return;
-  __threadfence();
+  if (!entry::last_to_arrive(counter, s.last)) return;
 
   float* tot = &s.sv[0][0];
-  for (int q = t; q < Q; q += THREADS) {
-    float acc = 0.f;
-    for (unsigned c = 0; c < gridDim.x; ++c) acc += __ldcg(parts + (size_t)c * Q + q);
-    tot[q] = acc;
-  }
+  entry::sum_partials<THREADS>(parts, Q, [&](int q, float v) { tot[q] = v; });
   __syncthreads();
   const float* v3 = s.v;
   const float* v2 = s.v + 8;
@@ -316,65 +302,48 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_tower(b200_census_args_t 
   if (t == 0) *counter = 0u;
 }
 
-constexpr int kMaxDevices = 64;
-std::atomic<int> g_sms[kMaxDevices];
-std::atomic<bool> g_attr[kMaxDevices];
-
-int sm_count(int dev) {
-  int n = dev < kMaxDevices ? g_sms[dev].load() : 0;
-  if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 1;
-    if (dev < kMaxDevices) g_sms[dev].store(n);
-  }
-  return n;
-}
-
-int grid_for(int64_t B, int dev) {
+// at most one CTA per SM
+int grid_for(int64_t B, int* grid) {
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
   const int64_t tiles = (B + TILE - 1) / TILE;
-  return (int)(tiles < sm_count(dev) ? tiles : sm_count(dev));
+  *grid = (int)(tiles < d.sms ? tiles : d.sms);
+  return 0;
 }
 
 }  // namespace
 
 extern "C" {
 
-const char* b200_census_last_error(void) { return g_err.c_str(); }
+const char* b200_census_last_error(void) { return E::last_error().c_str(); }
 int64_t b200_census_launch_count(void) { return g_launches.load(); }
 
 size_t b200_census_workspace_bytes(int64_t B) {
-  int dev = 0;
-  if (B < 1 || cudaGetDevice(&dev) != cudaSuccess) return 0;
-  return WS_HEADER + (size_t)grid_for(B, dev) * Q * sizeof(float);
+  int grid = 0;
+  if (B < 1 || grid_for(B, &grid)) return 0;
+  return entry::partials_bytes(grid, Q);
 }
 
 int b200_census_tower(const b200_census_args_t* args, void* stream) {
-  if (!args) return fail(-1, "args is null");
+  if (!args) return E::fail(-1, "args is null");
   const b200_census_args_t& a = *args;
   // 12 B ids must be addressable with a 32-bit row stride times 12
-  if (a.B < 1 || (int64_t)a.B * 12 > INT32_MAX) return fail(-1, "batch size must be in [1, 2^31 / 12)");
-  if (a.reference_reshape != 0 && a.reference_reshape != 1) return fail(-1, "reference_reshape must be 0 or 1");
+  if (a.B < 1 || (int64_t)a.B * 12 > INT32_MAX) return E::fail(-1, "batch size must be in [1, 2^31 / 12)");
+  if (a.reference_reshape != 0 && a.reference_reshape != 1) return E::fail(-1, "reference_reshape must be 0 or 1");
   if (!a.ids || !a.labels || !a.params || !a.loss || !a.logits || !a.grads || !a.uniq || !a.n_unique || !a.gsum ||
       !a.error || !a.workspace)
-    return fail(-1, "a buffer is null");
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(-2, "cudaGetDevice failed");
-  const int grid = grid_for(a.B, dev);
-  const size_t need = WS_HEADER + (size_t)grid * Q * sizeof(float);
+    return E::fail(-1, "a buffer is null");
+  int grid = 0;
+  if (int rc = grid_for(a.B, &grid)) return rc;
+  const size_t need = entry::partials_bytes(grid, Q);
   if (a.workspace_bytes < need)
-    return fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, batch " + std::to_string(a.B) +
-                        " needs " + std::to_string(need));
+    return E::fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, batch " + std::to_string(a.B) +
+                           " needs " + std::to_string(need));
   const size_t smem = sizeof(Smem);
-  if (dev >= kMaxDevices || !g_attr[dev].load()) {
-    cudaError_t e = cudaFuncSetAttribute(k_census_tower, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(-2, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-    if (dev < kMaxDevices) g_attr[dev].store(true);
-  }
+  if (int rc = E::raise_smem_limit(k_census_tower, smem)) return rc;
   const int ntiles = (int)((a.B + TILE - 1) / TILE);
   k_census_tower<<<grid, THREADS, smem, (cudaStream_t)stream>>>(a, ntiles);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_census_tower: ") + cudaGetErrorString(e));
-  g_launches.fetch_add(1);
-  return 0;
+  return E::launched("k_census_tower", g_launches);
 }
 
 }  // extern "C"

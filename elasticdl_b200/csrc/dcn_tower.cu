@@ -38,7 +38,7 @@ constexpr int SPART = 2;              // threads per small gradient (174 threads
 constexpr int SPLEN = TS / SPART;
 static_assert(DSTATE % 4 == 0 && SPART * NSMALL_X <= THREADS, "state record / small gradients");
 
-long long g_launches = 0;
+entry::LaunchCount g_launches{0};
 
 // shared memory carve-up (floats)
 constexpr int SM_W1X = NCOL * UP;          // 6400
@@ -389,7 +389,7 @@ extern "C" {
 
 size_t b200_deepfm_dcn_param_count(int G) { return G < 1 ? 0 : (size_t)dcn_layout(G).l.total; }
 
-int64_t b200_deepfm_dcn_launch_count(void) { return g_launches; }
+int64_t b200_deepfm_dcn_launch_count(void) { return g_launches.load(); }
 
 int b200_deepfm_dcn_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
   return launch<true>(args, stream);

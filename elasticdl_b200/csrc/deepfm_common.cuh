@@ -1,15 +1,15 @@
 // What the three DeepFM towers (deepfm_tower.cu "fused", deepfm_tower2.cu "tile", deepfm_tower_mma.cu "mma") share:
 // the model and its flat parameter layout (include/b200_deepfm.h), the zeroing of the step's outputs, the
 // per-sample tail, the per-sample backward state and the small gradients read from it, the warp-level id dedup
-// of the row gradients, the loss reduction, cp.async, and the host side of an entry point (argument checks,
-// shared-memory limit, launch errors and the one error message of b200_deepfm_last_error).
+// of the row gradients, the loss reduction, cp.async, the argument checks of an entry point and the one error
+// message of b200_deepfm_last_error (E::last_error).
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <string>
 
 #include "../../include/b200_deepfm.h"
+#include "launch.cuh"
 
 namespace deepfm {
 
@@ -182,49 +182,18 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 // ---- host side of the entry points
 
-// The message of the last refusal or launch error of any tower entry point (b200_deepfm_last_error).
-inline std::string& last_error() {
-  static thread_local std::string msg;
-  return msg;
-}
-inline int fail(int rc, const char* msg) {
-  last_error() = msg;
-  return rc;
-}
+// The tower entry points share one error message (b200_deepfm_last_error).
+using E = entry::Entry<entry::DeepFm>;
 
 // The checks every tower makes (-1 and the message, or 0).  A tower adds its group limit, what it needs of
 // `scratch` and whether it takes a row source.  Training needs every output but `logits`, forward-only `logits`.
 inline int check_common(const b200_deepfm_args_t* a, bool backward) {
-  if (!a || a->G < 1 || a->B < 1) return fail(-1, "bad shape");
-  if (!a->inv || !a->dense || !a->params || (!a->rows && (!a->bet_wide || !a->bet_deep))) return fail(-1, "null input");
+  if (!a || a->G < 1 || a->B < 1) return E::fail(-1, "bad shape");
+  if (!a->inv || !a->dense || !a->params || (!a->rows && (!a->bet_wide || !a->bet_deep)))
+    return E::fail(-1, "null input");
   if (backward ? (!a->labels || !a->grads || !a->gsum_wide || !a->gsum_deep || !a->loss || !a->n_unique) : !a->logits)
-    return fail(-1, "null output");
+    return E::fail(-1, "null output");
   return 0;
-}
-
-// the current device and its SM count
-inline int current_device(int* n_sm) {
-  int dev = 0;
-  *n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(n_sm, cudaDevAttrMultiProcessorCount, dev);
-  return dev;
-}
-
-// Raise Kernel's dynamic shared memory limit to `bytes`, once per device (it is a driver call).
-template <auto Kernel>
-void max_dynamic_smem_once(int dev, int bytes) {
-  static bool done[64] = {};
-  if (dev < 64 && !done[dev]) {
-    cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    done[dev] = true;
-  }
-}
-
-// After an entry point's launches: 0, or -2 and the launch error's message.
-inline int launch_status() {
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail(-2, cudaGetErrorString(e));
 }
 
 }  // namespace deepfm

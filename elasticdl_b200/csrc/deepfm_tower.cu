@@ -16,7 +16,7 @@ namespace {
 
 using namespace deepfm;
 
-long long g_launches = 0;
+entry::LaunchCount g_launches{0};
 
 __global__ void __launch_bounds__(256) k_tower_prep(b200_deepfm_args_t a, int n_params) {
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -426,9 +426,9 @@ __global__ void __launch_bounds__(TB_THREADS, 4) k_tower_b(b200_deepfm_args_t a)
 
 int check_args(const b200_deepfm_args_t* a, bool backward) {
   if (check_common(a, backward)) return -1;
-  if (ND + a->G * D + 1 > TB_COLW * TB_CPT) return fail(-1, "too many id groups for the fused tower (max 46)");
-  if (a->rows) return fail(-1, "the fused tower reads pulled rows only");
-  if (backward && !a->scratch) return fail(-1, "null output");
+  if (ND + a->G * D + 1 > TB_COLW * TB_CPT) return E::fail(-1, "too many id groups for the fused tower (max 46)");
+  if (a->rows) return E::fail(-1, "the fused tower reads pulled rows only");
+  if (backward && !a->scratch) return E::fail(-1, "null output");
   return 0;
 }
 
@@ -442,34 +442,34 @@ unsigned tower_a_grid(int B, int n_sm) {
 extern "C" {
 
 size_t b200_deepfm_param_count(int G) { return (size_t)layout(G).total; }
-int64_t b200_deepfm_launch_count(void) { return g_launches; }
-const char* b200_deepfm_last_error(void) { return last_error().c_str(); }
+int64_t b200_deepfm_launch_count(void) { return g_launches.load(); }
+const char* b200_deepfm_last_error(void) { return E::last_error().c_str(); }
 
 int b200_deepfm_fwd_bwd(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, true)) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const Layout l = layout(args->G);
-  int n_sm;
-  const int dev = current_device(&n_sm);
-  max_dynamic_smem_once<k_tower_a<true>>(dev, 110 * 1024);
-  max_dynamic_smem_once<k_tower_b>(dev, 110 * 1024);
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
+  if (int rc = E::raise_smem_limit(k_tower_a<true>, 110 * 1024)) return rc;
+  if (int rc = E::raise_smem_limit(k_tower_b, 110 * 1024)) return rc;
   k_tower_prep<<<dim3(8, args->G), 256, 0, st>>>(*args, l.total);
-  k_tower_a<true><<<tower_a_grid(args->B, n_sm), TA_THREADS, tower_a_smem(args->G), st>>>(*args);
+  if (int rc = E::launched("k_tower_prep", g_launches)) return rc;
+  k_tower_a<true><<<tower_a_grid(args->B, d.sms), TA_THREADS, tower_a_smem(args->G), st>>>(*args);
+  if (int rc = E::launched("k_tower_a", g_launches)) return rc;
   const long long chunks = ((long long)args->B + S_CHUNK - 1) / S_CHUNK;
-  const long long cap = (long long)n_sm * 4;  // 4 blocks per SM by shared memory / registers
+  const long long cap = (long long)d.sms * 4;  // 4 blocks per SM by shared memory / registers
   k_tower_b<<<(unsigned)(chunks < cap ? chunks : cap), TB_THREADS, tower_b_smem(args->G), st>>>(*args);
-  g_launches += 3;
-  return launch_status();
+  return E::launched("k_tower_b", g_launches);
 }
 
 int b200_deepfm_forward(const b200_deepfm_args_t* args, void* stream) {
   if (check_args(args, false)) return -1;
-  int n_sm;
-  const int dev = current_device(&n_sm);
-  max_dynamic_smem_once<k_tower_a<false>>(dev, 110 * 1024);
-  k_tower_a<false><<<tower_a_grid(args->B, n_sm), TA_THREADS, tower_a_smem(args->G), (cudaStream_t)stream>>>(*args);
-  g_launches += 1;
-  return launch_status();
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
+  if (int rc = E::raise_smem_limit(k_tower_a<false>, 110 * 1024)) return rc;
+  k_tower_a<false><<<tower_a_grid(args->B, d.sms), TA_THREADS, tower_a_smem(args->G), (cudaStream_t)stream>>>(*args);
+  return E::launched("k_tower_a", g_launches);
 }
 
 }  // extern "C"

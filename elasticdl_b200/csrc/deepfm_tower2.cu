@@ -36,7 +36,7 @@ constexpr int RW = H1 + D + 2;  // partial record: h[16] | s[8] | q | lin
 constexpr int SPART = 3;                       // threads per small gradient (255 threads, 11 samples each)
 constexpr int SPLEN = (TS + SPART - 1) / SPART;
 
-long long g_launches = 0;
+entry::LaunchCount g_launches{0};
 
 // shared memory carve-up (floats)
 constexpr int SM_W1X = NCOL * H1;          // 5120
@@ -351,18 +351,18 @@ int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
 namespace deepfm {
 
 template <bool BACKWARD>
-int launch_xdeepfm_tile(const b200_deepfm_args_t* args, void* stream, int what, long long& launches) {
+int launch_xdeepfm_tile(const b200_deepfm_args_t* args, void* stream, int what, entry::LaunchCount& launches) {
   return launch_tile_tower<BACKWARD, k_tower_tile<BACKWARD, false, false, true>, k_tower_tile<true, true, false, true>>(
       args, stream, what, SMEM_BYTES, prep, launches);
 }
-template int launch_xdeepfm_tile<true>(const b200_deepfm_args_t*, void*, int, long long&);
-template int launch_xdeepfm_tile<false>(const b200_deepfm_args_t*, void*, int, long long&);
+template int launch_xdeepfm_tile<true>(const b200_deepfm_args_t*, void*, int, entry::LaunchCount&);
+template int launch_xdeepfm_tile<false>(const b200_deepfm_args_t*, void*, int, entry::LaunchCount&);
 
 }  // namespace deepfm
 
 extern "C" {
 
-int64_t b200_deepfm_tile_launch_count(void) { return g_launches; }
+int64_t b200_deepfm_tile_launch_count(void) { return g_launches.load(); }
 
 int b200_deepfm_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
   return launch<true>(args, stream);
@@ -377,10 +377,9 @@ int b200_deepfm_tile_main(const b200_deepfm_args_t* args, void* stream) {
 }
 
 int b200_deepfm_publish_loss(const float* loss_dev, float* ring_host_mapped, int ring_len, unsigned* cursor_dev, void* stream) {
-  if (!loss_dev || !ring_host_mapped || ring_len < 1 || !cursor_dev) return fail(-1, "bad publish_loss arguments");
+  if (!loss_dev || !ring_host_mapped || ring_len < 1 || !cursor_dev) return E::fail(-1, "bad publish_loss arguments");
   k_publish_loss<<<1, 1, 0, (cudaStream_t)stream>>>(loss_dev, ring_host_mapped, ring_len, cursor_dev);
-  g_launches += 1;
-  return launch_status();
+  return E::launched("k_publish_loss", g_launches);
 }
 
 int b200_deepfm_forward_tile(const b200_deepfm_args_t* args, void* stream) {

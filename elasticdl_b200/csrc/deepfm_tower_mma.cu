@@ -44,7 +44,7 @@ __host__ inline size_t mma_smem_bytes(int G) {
   return f * sizeof(float) + (size_t)G * MT * sizeof(int);
 }
 
-long long g_launches_mma = 0;
+entry::LaunchCount g_launches_mma{0};
 
 // Fragment coordinates: mma_tf32.cuh
 template <bool BACKWARD>  // 2 resident CTAs per SM: up to 255 registers (3 would cap them at 168)
@@ -323,32 +323,28 @@ static_assert(MT == 32, "the per-sample phase and the loss reduction assume one 
 
 extern "C" {
 
-int64_t b200_deepfm_mma_launch_count(void) { return g_launches_mma; }
+int64_t b200_deepfm_mma_launch_count(void) { return g_launches_mma.load(); }
 
 int b200_deepfm_fwd_bwd_mma(const b200_deepfm_args_t* a, void* stream) {
   if (check_common(a, true)) return -1;
-  if (tile_of(a->G).kp / 8 > 4 * MAX_NT_W) return fail(-1, "too many id groups for the mma tower (max 46)");
-  if (a->rows) return fail(-1, "the mma tower reads pulled rows only");
+  if (tile_of(a->G).kp / 8 > 4 * MAX_NT_W) return E::fail(-1, "too many id groups for the mma tower (max 46)");
+  if (a->rows) return E::fail(-1, "the mma tower reads pulled rows only");
   const size_t smem = mma_smem_bytes(a->G);
-  if (smem > 100 * 1024) return fail(-1, "the mma tower's tile does not fit in shared memory");
+  if (smem > 100 * 1024) return E::fail(-1, "the mma tower's tile does not fit in shared memory");
   cudaStream_t st = (cudaStream_t)stream;
-  int n_sm;
-  const int dev = current_device(&n_sm);
-  max_dynamic_smem_once<k_tower_mma<true>>(dev, 100 * 1024);
-  static int per_sm[64] = {0};  // resident CTAs per SM, once per device
-  if (dev < 64 && per_sm[dev] == 0) {
-    int nb = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tower_mma<true>, THREADS, smem);
-    per_sm[dev] = e != cudaSuccess || nb < 1 ? 1 : nb;
-  }
+  entry::Device d;
+  int per_sm = 0;  // resident CTAs per SM
+  if (int rc = E::device(&d)) return rc;
+  if (int rc = E::raise_smem_limit(k_tower_mma<true>, 100 * 1024)) return rc;
+  if (int rc = E::blocks_per_sm(k_tower_mma<true>, THREADS, smem, &per_sm)) return rc;
   const Layout l = layout(a->G);
   k_mma_prep<<<dim3(8, a->G), 256, 0, st>>>(*a, l.total);
+  if (int rc = E::launched("k_mma_prep", g_launches_mma)) return rc;
   const long long nchunk = ((long long)a->B + MT - 1) / MT;
-  const long long cap = (long long)n_sm * (dev < 64 ? per_sm[dev] : 1);
+  const long long cap = (long long)d.sms * per_sm;
   const unsigned grid = (unsigned)(nchunk < cap ? nchunk : cap);
   k_tower_mma<true><<<grid, THREADS, smem, st>>>(*a);
-  g_launches_mma += 2;
-  return launch_status();
+  return E::launched("k_tower_mma", g_launches_mma);
 }
 
 }  // extern "C"

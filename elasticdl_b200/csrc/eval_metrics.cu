@@ -11,20 +11,16 @@
 // at most one).
 #include <cuda_runtime.h>
 
-#include <atomic>
 #include <cstdint>
 #include <string>
 
 #include "../../include/b200_metrics.h"
+#include "launch.cuh"
 
 namespace {
 
-thread_local std::string g_err;
-std::atomic<long long> g_launches{0};
-int fail(int code, const std::string& m) {
-  g_err = m;
-  return code;
-}
+using E = entry::Entry<entry::Metrics>;
+entry::LaunchCount g_launches{0};
 
 constexpr int THREADS = B200_METRICS_THREADS;
 constexpr int WARPS = THREADS / 32;
@@ -95,67 +91,40 @@ __global__ void __launch_bounds__(THREADS) k_auc_update(const float* __restrict_
   if (threadIdx.x == 0 && *bad) atomicAdd(invalid, (unsigned long long)*bad);
 }
 
-constexpr int kMaxDevices = 64;
-std::atomic<int> g_smem_optin[kMaxDevices], g_sms[kMaxDevices];
-
-// (opt-in shared memory per block, SM count) of `dev`; the kernel's dynamic shared memory limit is raised to the
-// opt-in maximum the first time
-int device_limits(int dev, int* smem, int* sms) {
-  int s = dev < kMaxDevices ? g_smem_optin[dev].load() : 0;
-  int m = dev < kMaxDevices ? g_sms[dev].load() : 0;
-  if (s == 0 || m == 0) {
-    if (cudaDeviceGetAttribute(&s, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&m, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      return fail(-2, "cudaDeviceGetAttribute failed");
-    cudaError_t e = cudaFuncSetAttribute(k_auc_update, cudaFuncAttributeMaxDynamicSharedMemorySize, s);
-    if (e != cudaSuccess) return fail(-2, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-    if (dev < kMaxDevices) {
-      g_smem_optin[dev].store(s);
-      g_sms[dev].store(m);
-    }
-  }
-  *smem = s;
-  *sms = m;
-  return 0;
-}
-
 }  // namespace
 
 extern "C" {
 
-const char* b200_metrics_last_error(void) { return g_err.c_str(); }
+const char* b200_metrics_last_error(void) { return E::last_error().c_str(); }
 int64_t b200_metrics_launch_count(void) { return g_launches.load(); }
 
 int b200_metrics_auc_update(const float* probs, const float* labels, int64_t n, const float* thresholds, int32_t T,
                             uint64_t* hist, uint64_t* invalid, void* stream) {
   if (T < B200_METRICS_MIN_THRESHOLDS || T > B200_METRICS_MAX_THRESHOLDS)
-    return fail(-1, "num_thresholds must be in [" + std::to_string(B200_METRICS_MIN_THRESHOLDS) + ", " +
-                        std::to_string(B200_METRICS_MAX_THRESHOLDS) + "], not " + std::to_string(T));
-  if (n < 0 || n > INT32_MAX) return fail(-1, "n must be in [0, 2^31), not " + std::to_string(n));
-  if (!thresholds || !hist || !invalid) return fail(-1, "a buffer is null");
+    return E::fail(-1, "num_thresholds must be in [" + std::to_string(B200_METRICS_MIN_THRESHOLDS) + ", " +
+                           std::to_string(B200_METRICS_MAX_THRESHOLDS) + "], not " + std::to_string(T));
+  if (n < 0 || n > INT32_MAX) return E::fail(-1, "n must be in [0, 2^31), not " + std::to_string(n));
+  if (!thresholds || !hist || !invalid) return E::fail(-1, "a buffer is null");
   if (n == 0) return 0;
-  if (!probs || !labels) return fail(-1, "a buffer is null");
-  int dev = 0, smem_max = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(-2, "cudaGetDevice failed");
-  if (int rc = device_limits(dev, &smem_max, &sms)) return rc;
+  if (!probs || !labels) return E::fail(-1, "a buffer is null");
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
+  const int smem_max = d.smem_optin;
   int copies = WARPS;
   while (copies > 1 && smem_bytes(T, copies) > (size_t)smem_max) --copies;
   const size_t smem = smem_bytes(T, copies);
   if (smem > (size_t)smem_max)
-    return fail(-1, std::to_string(T) + " thresholds need " + std::to_string(smem) + " bytes of shared memory, the "
-                        "device has " + std::to_string(smem_max));
-  int per = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_auc_update, THREADS, smem) != cudaSuccess || per < 1)
-    per = 1;
+    return E::fail(-1, std::to_string(T) + " thresholds need " + std::to_string(smem) + " bytes of shared memory, the "
+                           "device has " + std::to_string(smem_max));
+  int per = 0;
+  if (int rc = E::raise_smem_limit(k_auc_update, smem_max)) return rc;
+  if (int rc = E::blocks_per_sm(k_auc_update, THREADS, smem, &per)) return rc;
   const int64_t want = (n + B200_METRICS_MIN_PER_CTA - 1) / B200_METRICS_MIN_PER_CTA;
-  const int grid = (int)(want < (int64_t)sms * per ? want : (int64_t)sms * per);
+  const int grid = (int)(want < (int64_t)d.sms * per ? want : (int64_t)d.sms * per);
   k_auc_update<<<grid, THREADS, smem, (cudaStream_t)stream>>>(probs, labels, n, thresholds, T, copies,
                                                               reinterpret_cast<unsigned long long*>(hist),
                                                               reinterpret_cast<unsigned long long*>(invalid));
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_auc_update: ") + cudaGetErrorString(e));
-  g_launches.fetch_add(1);
-  return 0;
+  return E::launched("k_auc_update", g_launches);
 }
 
 }  // extern "C"

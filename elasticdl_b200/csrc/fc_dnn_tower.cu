@@ -12,20 +12,16 @@
 // CTA to arrive adds the partials in CTA order, forms the outputs and resets the arrival counter.
 #include <cuda_runtime.h>
 
-#include <atomic>
 #include <cstdint>
 #include <string>
 
 #include "../../include/b200_fc_dnn.h"
+#include "launch.cuh"
 
 namespace {
 
-thread_local std::string g_err;
-std::atomic<long long> g_launches{0};
-int fail(int code, const std::string& m) {
-  g_err = m;
-  return code;
-}
+using E = entry::Entry<entry::FcDnn>;
+entry::LaunchCount g_launches{0};
 
 constexpr int H = B200_FC_DNN_HIDDEN;
 constexpr int TILE = B200_FC_DNN_TILE;
@@ -33,7 +29,6 @@ constexpr int THREADS = 256;
 constexpr int MAXT = B200_FC_DNN_MAX_TABLES;
 constexpr int NP_MAX = H * B200_FC_DNN_MAX_F + 305;
 constexpr int KP = (NP_MAX + 1 + THREADS - 1) / THREADS;  // dense sums per thread (the MLP gradients + the loss)
-constexpr size_t WS_HEADER = 64;                          // arrival counter
 static_assert(THREADS == 4 * TILE, "four threads per sample");
 
 // What the kernel derives from a checked layout.
@@ -237,8 +232,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_fc_dnn_tower(b200_fc_dnn_args_t 
   }
   if (!train) return;
 
-  unsigned* counter = reinterpret_cast<unsigned*>(a.workspace);
-  float* parts = reinterpret_cast<float*>(reinterpret_cast<char*>(a.workspace) + WS_HEADER);
+  unsigned* counter = entry::arrival_counter(a.workspace);
+  float* parts = entry::partials(a.workspace);
   float* mine = parts + (size_t)blockIdx.x * pl.Q;
 #pragma unroll
   for (int k = 0; k < KP; ++k) {
@@ -246,20 +241,13 @@ __global__ void __launch_bounds__(THREADS, 1) k_fc_dnn_tower(b200_fc_dnn_args_t 
     if (p <= NP) mine[p] = acc[k];
   }
   for (int i = t; i < pl.slots * H; i += THREADS) mine[NP + 1 + i] = R[i];
-  __threadfence();
-  __syncthreads();
-  if (t == 0) last = atomicAdd(counter, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
+  if (!entry::last_to_arrive(counter, last)) return;
 
   // totals: the dense sums into S, the row sums into R
-  for (int i = t; i < pl.Q; i += THREADS) {
-    float s = 0.f;
-    for (unsigned c = 0; c < gridDim.x; ++c) s += __ldcg(parts + (size_t)c * pl.Q + i);
+  entry::sum_partials<THREADS>(parts, pl.Q, [&](int i, float s) {
     if (i <= NP) S[i] = s;
     else R[i - NP - 1] = s;
-  }
+  });
   __syncthreads();
   for (int i = t; i < NP; i += THREADS) a.grads[i] = S[i];
   if (t == 0) {
@@ -291,22 +279,13 @@ __global__ void k_fc_dnn_fill_empty(b200_fc_layout_t L, int32_t* ids, const uint
   }
 }
 
-constexpr int kMaxDevices = 64;
-std::atomic<int> g_sms[kMaxDevices];
-std::atomic<int> g_attr[kMaxDevices];  // the dynamic shared memory size set for the device (bytes)
-
-int sm_count(int dev) {
-  int n = dev < kMaxDevices ? g_sms[dev].load() : 0;
-  if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 1;
-    if (dev < kMaxDevices) g_sms[dev].store(n);
-  }
-  return n;
-}
-
-int grid_for(int64_t B, int dev) {
+// at most one CTA per SM
+int grid_for(int64_t B, int* grid) {
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
   const int64_t tiles = (B + TILE - 1) / TILE;
-  return (int)(tiles < sm_count(dev) ? tiles : sm_count(dev));
+  *grid = (int)(tiles < d.sms ? tiles : d.sms);
+  return 0;
 }
 
 // Check a layout and derive its plan; "" when it is sound.
@@ -363,103 +342,86 @@ std::string make_plan(const b200_fc_layout_t* layout, Plan* out) {
 }
 
 int check_args(const Plan& p, const b200_fc_dnn_args_t* args, int train) {
-  if (!args) return fail(-1, "args is null");
+  if (!args) return E::fail(-1, "args is null");
   const b200_fc_dnn_args_t& a = *args;
   const b200_fc_layout_t& L = p.L;
-  if (a.B < 1 || a.B > INT32_MAX) return fail(-1, "batch size must be in [1, 2^31)");
-  if (a.W < 1 || a.n_numeric < 0 || a.n_ids < 0 || a.n_strings < 0) return fail(-1, "bad input shape");
+  if (a.B < 1 || a.B > INT32_MAX) return E::fail(-1, "batch size must be in [1, 2^31)");
+  if (a.W < 1 || a.n_numeric < 0 || a.n_ids < 0 || a.n_strings < 0) return E::fail(-1, "bad input shape");
   for (int bi = 0; bi < L.n_blocks; ++bi) {
     const b200_fc_block_t& b = L.blocks[bi];
-    if (b.kind == B200_FC_NUMERIC && b.src >= a.n_numeric) return fail(-1, "a numeric block reads a missing row");
-    if (b.kind == B200_FC_BUCKET && b.src >= a.n_ids) return fail(-1, "a bucket block reads a missing ids row");
+    if (b.kind == B200_FC_NUMERIC && b.src >= a.n_numeric) return E::fail(-1, "a numeric block reads a missing row");
+    if (b.kind == B200_FC_BUCKET && b.src >= a.n_ids) return E::fail(-1, "a bucket block reads a missing ids row");
   }
   for (int k = 0; k < L.n_tables; ++k)
-    if (L.table_string[k] >= a.n_strings) return fail(-1, "a table's string column is missing");
+    if (L.table_string[k] >= a.n_strings) return E::fail(-1, "a table's string column is missing");
   const bool need_num = a.n_numeric > 0, need_ids = a.n_ids > 0, need_tab = L.n_tables > 0;
   if ((need_num && !a.numeric) || (need_ids && !a.ids) || (need_tab && (!a.strings || !a.inv || !a.rows)) ||
       !a.params || !a.logits)
-    return fail(-1, "a buffer is null");
+    return E::fail(-1, "a buffer is null");
   if (train && (!a.labels || !a.loss || !a.grads || !a.workspace || (need_tab && (!a.n_unique || !a.gsum))))
-    return fail(-1, "a buffer is null");
+    return E::fail(-1, "a buffer is null");
   return 0;
 }
 
 int launch(const b200_fc_layout_t* layout, const b200_fc_dnn_args_t* args, void* stream, int train) {
   Plan p;
   const std::string why = make_plan(layout, &p);
-  if (!why.empty()) return fail(-1, why);
+  if (!why.empty()) return E::fail(-1, why);
   int rc = check_args(p, args, train);
   if (rc) return rc;
   const b200_fc_dnn_args_t& a = *args;
-  if (reinterpret_cast<uintptr_t>(a.params) & 3u) return fail(-1, "params must be 4-byte aligned");
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(-2, "cudaGetDevice failed");
-  const int grid = grid_for(a.B, dev);
+  if (reinterpret_cast<uintptr_t>(a.params) & 3u) return E::fail(-1, "params must be 4-byte aligned");
+  int grid = 0;
+  if (int rc = grid_for(a.B, &grid)) return rc;
   if (train) {
-    const size_t need = WS_HEADER + (size_t)grid * p.Q * sizeof(float);
+    const size_t need = entry::partials_bytes(grid, p.Q);
     if (a.workspace_bytes < need)
-      return fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, batch " + std::to_string(a.B) +
-                          " needs " + std::to_string(need));
+      return E::fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, batch " + std::to_string(a.B) +
+                             " needs " + std::to_string(need));
   }
   const int smem = p.smem_floats * (int)sizeof(float);
-  if (dev >= kMaxDevices || g_attr[dev].load() < smem) {
-    cudaError_t e = cudaFuncSetAttribute(k_fc_dnn_tower, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return fail(-2, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-    if (dev < kMaxDevices) {
-      int cur = g_attr[dev].load();
-      while (cur < smem && !g_attr[dev].compare_exchange_weak(cur, smem)) {
-      }
-    }
-  }
+  if (int rc = E::raise_smem_limit(k_fc_dnn_tower, smem)) return rc;
   const int ntiles = (int)((a.B + TILE - 1) / TILE);
   k_fc_dnn_tower<<<grid, THREADS, smem, (cudaStream_t)stream>>>(a, p, ntiles, train);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_fc_dnn_tower: ") + cudaGetErrorString(e));
-  g_launches.fetch_add(1);
-  return 0;
+  return E::launched("k_fc_dnn_tower", g_launches);
 }
 
 }  // namespace
 
 extern "C" {
 
-const char* b200_fc_dnn_last_error(void) { return g_err.c_str(); }
+const char* b200_fc_dnn_last_error(void) { return E::last_error().c_str(); }
 int64_t b200_fc_dnn_launch_count(void) { return g_launches.load(); }
 
 int64_t b200_fc_dnn_params(const b200_fc_layout_t* layout) {
   Plan p;
   const std::string why = make_plan(layout, &p);
-  if (!why.empty()) {
-    g_err = why;
-    return 0;
-  }
+  if (!why.empty()) return E::fail(0, why);
   return p.NP;
 }
 
 size_t b200_fc_dnn_workspace_bytes(const b200_fc_layout_t* layout, int64_t B) {
   Plan p;
-  int dev = 0;
-  if (B < 1 || !make_plan(layout, &p).empty() || cudaGetDevice(&dev) != cudaSuccess) return 0;
-  return WS_HEADER + (size_t)grid_for(B, dev) * p.Q * sizeof(float);
+  int grid = 0;
+  if (B < 1 || !make_plan(layout, &p).empty() || grid_for(B, &grid)) return 0;
+  return entry::partials_bytes(grid, p.Q);
 }
 
 int b200_fc_dnn_fill_empty(const b200_fc_layout_t* layout, int32_t* ids, const uint8_t* strings, int64_t B, int W,
                            void* stream) {
   Plan p;
   const std::string why = make_plan(layout, &p);
-  if (!why.empty()) return fail(-1, why);
-  if (B < 1 || W < 1) return fail(-1, "batch size and string width must be >= 1");
+  if (!why.empty()) return E::fail(-1, why);
+  if (B < 1 || W < 1) return E::fail(-1, "batch size and string width must be >= 1");
   if (p.L.n_tables == 0) return 0;
-  if (!ids || !strings) return fail(-1, "a buffer is null");
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(-2, "cudaGetDevice failed");
+  if (!ids || !strings) return E::fail(-1, "a buffer is null");
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
   const int64_t n = (int64_t)p.L.n_tables * B;
   const int64_t want = (n + 255) / 256;
-  const int grid = (int)(want < 4 * sm_count(dev) ? want : 4 * sm_count(dev));
+  const int grid = (int)(want < 4 * d.sms ? want : 4 * d.sms);
   k_fc_dnn_fill_empty<<<grid, 256, 0, (cudaStream_t)stream>>>(p.L, ids, strings, B, W);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_fc_dnn_fill_empty: ") + cudaGetErrorString(e));
-  return 0;
+  return E::launched("k_fc_dnn_fill_empty", g_launches, 0);
 }
 
 int b200_fc_dnn_tower(const b200_fc_layout_t* layout, const b200_fc_dnn_args_t* args, void* stream) {

@@ -19,15 +19,12 @@
 #include <type_traits>
 
 #include "../../include/b200_features.h"
+#include "launch.cuh"
 
 namespace {
 
-thread_local std::string g_err;
-long long g_launches = 0;
-int fail(int code, const std::string& m) {
-  g_err = m;
-  return code;
-}
+using E = entry::Entry<entry::Features>;
+entry::LaunchCount g_launches{0};
 
 constexpr int kMaxGroups = 64, kMaxDense = 32, kMaxBoundaries = 256, kMaxW = 64;
 
@@ -289,16 +286,15 @@ __global__ void __launch_bounds__(256) k_fingerprint(const uint8_t* __restrict__
 }
 
 // 8 resident blocks of 256 threads per SM of the current device
-int max_blocks() {
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  return n_sm * 8;
+int max_blocks(int* out) {
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
+  *out = d.sms * 8;
+  return 0;
 }
 
-int grid_x(long long n) {
+int grid_x(long long n, int cap) {
   long long b = (n + 255) / 256;
-  const int cap = max_blocks();
   if (b > cap) b = cap;
   return (int)(b < 1 ? 1 : b);
 }
@@ -307,8 +303,8 @@ int grid_x(long long n) {
 
 extern "C" {
 
-const char* b200feat_last_error(void) { return g_err.c_str(); }
-int64_t b200feat_launch_count(void) { return g_launches; }
+const char* b200feat_last_error(void) { return E::last_error().c_str(); }
+int64_t b200feat_launch_count(void) { return g_launches.load(); }
 
 int b200feat_transform(const b200feat_group_t* groups, int G, const float* boundaries, int n_boundaries,
                        const b200feat_dense_t* dense, int n_dense, const void* numeric_dev, int n_numeric,
@@ -323,13 +319,13 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
                            const void* numeric_dev, int n_numeric, int numeric_is_float, const uint8_t* strings_dev,
                            int n_string, int W, int64_t B, void* ids_out_dev, int ids32, float* dense_out_dev,
                            void* stream) {
-  if (G < 0 || G > kMaxGroups) return fail(-1, "bad group count (max 64)");
-  if (n_dense < 0 || n_dense > kMaxDense) return fail(-1, "bad dense column count (max 32)");
-  if (B < 1) return fail(-1, "bad batch size");
-  if (n_boundaries < 0 || n_boundaries > kMaxBoundaries) return fail(-1, "too many boundaries (max 256)");
-  if (G > 0 && (!groups || !ids_out_dev)) return fail(-1, "groups / ids_out is null");
-  if (n_dense > 0 && (!dense || !dense_out_dev)) return fail(-1, "dense / dense_out is null");
-  if (W < 0 || W > kMaxW) return fail(-1, "strings longer than 64 bytes are not supported (FarmHash restated for lengths 0..64)");
+  if (G < 0 || G > kMaxGroups) return E::fail(-1, "bad group count (max 64)");
+  if (n_dense < 0 || n_dense > kMaxDense) return E::fail(-1, "bad dense column count (max 32)");
+  if (B < 1) return E::fail(-1, "bad batch size");
+  if (n_boundaries < 0 || n_boundaries > kMaxBoundaries) return E::fail(-1, "too many boundaries (max 256)");
+  if (G > 0 && (!groups || !ids_out_dev)) return E::fail(-1, "groups / ids_out is null");
+  if (n_dense > 0 && (!dense || !dense_out_dev)) return E::fail(-1, "dense / dense_out is null");
+  if (W < 0 || W > kMaxW) return E::fail(-1, "strings longer than 64 bytes are not supported (FarmHash restated for lengths 0..64)");
   PlanExt p;
   memset(&p, 0, sizeof(p));
   bool ext_kinds = false;
@@ -339,35 +335,35 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
     const b200feat_group_t& gr = groups[g];
     int64_t lo = 0, hi;  // smallest and largest id before the offset
     if (gr.kind == B200FEAT_DISCRETIZE) {
-      if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "discretize: bad numeric column");
+      if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return E::fail(-1, "discretize: bad numeric column");
       if (gr.n_boundaries < 0 || gr.boundary_off < 0 || gr.boundary_off + gr.n_boundaries > n_boundaries || (gr.n_boundaries && !boundaries))
-        return fail(-1, "discretize: boundaries out of range");
+        return E::fail(-1, "discretize: boundaries out of range");
       // the kernel binary-searches them; TF's Bucketize refuses unsorted boundaries
       for (int i = gr.boundary_off; i < gr.boundary_off + gr.n_boundaries; ++i)
         if (boundaries[i] != boundaries[i] || (i > gr.boundary_off && boundaries[i] < boundaries[i - 1]))
-          return fail(-1, "discretize: boundaries are not sorted in ascending order (or hold a NaN)");
+          return E::fail(-1, "discretize: boundaries are not sorted in ascending order (or hold a NaN)");
       hi = gr.n_boundaries;
     } else if (gr.kind == B200FEAT_HASH_STRING) {
-      if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1) return fail(-1, "hash: bad string column");
-      if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");  // hashing.py:53-56
+      if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1) return E::fail(-1, "hash: bad string column");
+      if (gr.num_bins <= 0) return E::fail(-1, "`num_bins` cannot be `None` or non-positive values.");  // hashing.py:53-56
       hi = gr.num_bins - 1;
     } else if (gr.kind == B200FEAT_HASH_INT) {
-      if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return fail(-1, "hash: bad numeric column");
-      if (gr.num_bins <= 0) return fail(-1, "`num_bins` cannot be `None` or non-positive values.");
+      if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev) return E::fail(-1, "hash: bad numeric column");
+      if (gr.num_bins <= 0) return E::fail(-1, "`num_bins` cannot be `None` or non-positive values.");
       // Hashing converts integer inputs only (hashing.py:63-72); to_hash_bucket_fast refuses float tensors
-      if (numeric_is_float) return fail(-1, "hash_int: Hashing takes integer columns, these numeric columns are float32");
+      if (numeric_is_float) return E::fail(-1, "hash_int: Hashing takes integer columns, these numeric columns are float32");
       hi = gr.num_bins - 1;
     } else if (ext && gr.kind == B200FEAT_LOOKUP) {
       const b200feat_group_ext_t& e = ext[g];
       if (gr.column < 0 || gr.column >= n_string || !strings_dev || W < 1)
-        return fail(-1, "lookup: bad string column (IndexLookup takes string columns)");
-      if (!e.slots_dev || !e.terms_dev) return fail(-1, "lookup: null table");
-      if (e.V < 1) return fail(-1, "lookup: vocabulary size V must be >= 1");
-      if (e.Wv < 1 || e.Wv > kMaxW) return fail(-1, "lookup: term width Wv must be 1..64");
+        return E::fail(-1, "lookup: bad string column (IndexLookup takes string columns)");
+      if (!e.slots_dev || !e.terms_dev) return E::fail(-1, "lookup: null table");
+      if (e.V < 1) return E::fail(-1, "lookup: vocabulary size V must be >= 1");
+      if (e.Wv < 1 || e.Wv > kMaxW) return E::fail(-1, "lookup: term width Wv must be 1..64");
       if (e.n_slots < 2 * (int64_t)e.V || (e.n_slots & (e.n_slots - 1)))
-        return fail(-1, "lookup: n_slots must be a power of two >= 2V");
-      if (gr.num_bins < 0) return fail(-1, "lookup: num_oov_tokens must be >= 0");
-      if (gr.num_bins > INT64_MAX - e.V) return fail(-1, "lookup: V + num_oov_tokens overflows int64");
+        return E::fail(-1, "lookup: n_slots must be a power of two >= 2V");
+      if (gr.num_bins < 0) return E::fail(-1, "lookup: num_oov_tokens must be >= 0");
+      if (gr.num_bins > INT64_MAX - e.V) return E::fail(-1, "lookup: V + num_oov_tokens overflows int64");
       if (gr.num_bins == 0) lo = -1;  // the table's default_value
       hi = gr.num_bins > 0 ? e.V + gr.num_bins - 1 : e.V - 1;
       p.ext[g].slots = reinterpret_cast<const ulonglong2*>(e.slots_dev);
@@ -378,7 +374,7 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
     } else if (ext && (gr.kind == B200FEAT_LOG_ROUND || gr.kind == B200FEAT_ROUND_IDENTITY)) {
       const b200feat_group_ext_t& e = ext[g];
       if (gr.column < 0 || gr.column >= n_numeric || !numeric_dev)
-        return fail(-1, gr.kind == B200FEAT_LOG_ROUND ? "log_round: bad numeric column" : "round_identity: bad numeric column");
+        return E::fail(-1, gr.kind == B200FEAT_LOG_ROUND ? "log_round: bad numeric column" : "round_identity: bad numeric column");
       // ids: [0, num_bins) u {default_value}; num_bins <= 0 is accepted (log_round.py:53-57): every id is the default
       lo = gr.num_bins > 0 ? std::min<int64_t>(0, e.default_value) : e.default_value;
       hi = gr.num_bins > 0 ? std::max<int64_t>(gr.num_bins - 1, e.default_value) : e.default_value;
@@ -386,23 +382,25 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
       p.ext[g].has_base = gr.kind == B200FEAT_LOG_ROUND && e.has_base;
       p.ext[g].log_base = std::log(e.base);  // base = 0: -inf, and log(x) / -inf = -+0 (not refused, like the reference)
     } else {
-      return fail(-1, "unknown group kind");
+      return E::fail(-1, "unknown group kind");
     }
     if (ids32 && ((__int128)gr.offset + lo < INT32_MIN || (__int128)gr.offset + hi > INT32_MAX))
-      return fail(-1, "int32 ids: offset + id range of a group does not fit int32");
+      return E::fail(-1, "int32 ids: offset + id range of a group does not fit int32");
     p.group[g] = gr;
     ext_kinds |= gr.kind > B200FEAT_HASH_INT;
   }
   for (int j = 0; j < p.n_dense; ++j) {
-    if (dense[j].column < 0 || dense[j].column >= n_numeric || !numeric_dev) return fail(-1, "normalizer: bad numeric column");
-    if (dense[j].divisor == 0.0) return fail(-1, "The divisor cannot be 0");  // normalizer.py build()
+    if (dense[j].column < 0 || dense[j].column >= n_numeric || !numeric_dev) return E::fail(-1, "normalizer: bad numeric column");
+    if (dense[j].divisor == 0.0) return E::fail(-1, "The divisor cannot be 0");  // normalizer.py build()
     p.dense[j] = dense[j];
   }
   if (p.G + p.n_dense == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_boundaries; ++i) p.bnd[i] = boundaries[i];
-  int gx = grid_x(B);
-  const int per = (max_blocks() + p.G + p.n_dense - 1) / (p.G + p.n_dense);
+  int cap = 0;
+  if (int rc = max_blocks(&cap)) return rc;
+  int gx = grid_x(B, cap);
+  const int per = (cap + p.G + p.n_dense - 1) / (p.G + p.n_dense);
   if (gx > per) gx = per < 1 ? 1 : per;
   dim3 grid(gx, p.G + p.n_dense);
   const Plan& base = p;
@@ -418,10 +416,7 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
   else
     k_feature_transform<<<grid, 256, 0, st>>>(base, (const long long*)numeric_dev, strings_dev, W, (long long)B,
                                               ids_out_dev, ids32, dense_out_dev);
-  g_launches++;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, cudaGetErrorString(e));
-  return 0;
+  return E::launched("k_feature_transform", g_launches);
 }
 
 int64_t b200feat_vocab_slots(int64_t V) {
@@ -433,10 +428,10 @@ int64_t b200feat_vocab_slots(int64_t V) {
 
 int b200feat_vocab_build(const uint8_t* terms, int64_t V, int Wv, int64_t n_slots, b200feat_vocab_slot_t* slots,
                          int64_t* dup_pos) {
-  if (V < 1 || V >= (1LL << 31)) return fail(-1, "vocab build: V must be 1 .. 2^31 - 1");
-  if (Wv < 1 || Wv > kMaxW) return fail(-1, "vocab build: term width Wv must be 1..64");
-  if (n_slots < 2 * V || (n_slots & (n_slots - 1))) return fail(-1, "vocab build: n_slots must be a power of two >= 2V");
-  if (!terms || !slots) return fail(-1, "vocab build: terms / slots is null");
+  if (V < 1 || V >= (1LL << 31)) return E::fail(-1, "vocab build: V must be 1 .. 2^31 - 1");
+  if (Wv < 1 || Wv > kMaxW) return E::fail(-1, "vocab build: term width Wv must be 1..64");
+  if (n_slots < 2 * V || (n_slots & (n_slots - 1))) return E::fail(-1, "vocab build: n_slots must be a power of two >= 2V");
+  if (!terms || !slots) return E::fail(-1, "vocab build: terms / slots is null");
   for (int64_t i = 0; i < n_slots; ++i) slots[i] = b200feat_vocab_slot_t{0, -1, 0};
   const uint64_t mask = (uint64_t)n_slots - 1;
   for (int64_t v = 0; v < V; ++v) {
@@ -444,14 +439,14 @@ int b200feat_vocab_build(const uint8_t* terms, int64_t V, int Wv, int64_t n_slot
     int len = 0;
     while (len < Wv && t[len]) ++len;
     for (int i = len; i < Wv; ++i)
-      if (t[i]) return fail(-1, "vocab build: term " + std::to_string(v) + " holds a NUL byte (rows are zero padded)");
+      if (t[i]) return E::fail(-1, "vocab build: term " + std::to_string(v) + " holds a NUL byte (rows are zero padded)");
     const uint64_t fp = fingerprint64(t, len);
     uint64_t h = fp & mask;
     for (; slots[h].index >= 0; h = (h + 1) & mask) {  // load <= 1/2: an empty slot is always reached
       const b200feat_vocab_slot_t& s = slots[h];
       if (s.fingerprint == fp && s.length == len && memcmp(terms + (int64_t)s.index * Wv, t, len) == 0) {
         if (dup_pos) *dup_pos = v;
-        return fail(-1, "vocab build: term " + std::to_string(v) + " repeats term " + std::to_string(s.index));
+        return E::fail(-1, "vocab build: term " + std::to_string(v) + " repeats term " + std::to_string(s.index));
       }
     }
     slots[h] = b200feat_vocab_slot_t{fp, (int32_t)v, len};
@@ -521,12 +516,11 @@ int b200feat_round_identity(const void* x_dev, int x_is_float, int64_t n, int64_
 }
 
 int b200feat_fingerprint64(const uint8_t* strings_dev, int W, int64_t n, uint64_t* out_dev, void* stream) {
-  if (!strings_dev || !out_dev || n < 1 || W < 1 || W > kMaxW) return fail(-1, "bad fingerprint arguments");
-  k_fingerprint<<<grid_x(n), 256, 0, (cudaStream_t)stream>>>(strings_dev, W, (long long)n, out_dev);
-  g_launches++;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, cudaGetErrorString(e));
-  return 0;
+  if (!strings_dev || !out_dev || n < 1 || W < 1 || W > kMaxW) return E::fail(-1, "bad fingerprint arguments");
+  int cap = 0;
+  if (int rc = max_blocks(&cap)) return rc;
+  k_fingerprint<<<grid_x(n, cap), 256, 0, (cudaStream_t)stream>>>(strings_dev, W, (long long)n, out_dev);
+  return E::launched("k_fingerprint", g_launches);
 }
 
 }  // extern "C"

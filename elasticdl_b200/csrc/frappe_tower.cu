@@ -20,20 +20,16 @@
 //   writes the dense gradients and the loss and zeroes the accumulators and its counter.
 #include <cuda_runtime.h>
 
-#include <atomic>
 #include <cstdint>
 #include <string>
 
 #include "../../include/b200_frappe.h"
+#include "launch.cuh"
 
 namespace {
 
-thread_local std::string g_err;
-std::atomic<long long> g_launches{0};
-int fail(int code, const std::string& m) {
-  g_err = m;
-  return code;
-}
+using E = entry::Entry<entry::Frappe>;
+entry::LaunchCount g_launches{0};
 
 constexpr int F = B200_FRAPPE_FIELDS;
 constexpr int D = B200_FRAPPE_DIM;
@@ -57,7 +53,7 @@ struct Smem {
   float red[X];               // the CTA's s; in the last CTA the total s
   float misc[4];              // G, loss sum, c
   float part[5][D];           // the last CTA's K^T s partials
-  unsigned last;
+  int last;
 };
 
 __device__ __forceinline__ float warp_sum(float x) {
@@ -246,12 +242,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_frappe_main(b200_frappe_args_t a
     atomicAdd(ws + WS_G, s.misc[0]);
     atomicAdd(ws + WS_L, s.misc[1]);
   }
-  __threadfence();
-  __syncthreads();
-  if (t == 0) s.last = atomicAdd(reinterpret_cast<unsigned*>(ws), 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s.last) return;
-  __threadfence();
+  if (!entry::last_to_arrive(entry::arrival_counter(ws), s.last)) return;
   for (int i = t; i < X; i += THREADS) s.red[i] = __ldcg(ws + WS_S + i);
   if (t == 0) {
     s.misc[0] = __ldcg(ws + WS_G);
@@ -287,63 +278,37 @@ __global__ void __launch_bounds__(THREADS, 2) k_frappe_main(b200_frappe_args_t a
   }
 }
 
-constexpr int kMaxDevices = 64;
-std::atomic<int> g_grid[kMaxDevices], g_sms[kMaxDevices];
-
-// CTAs of the main pass that fit on the device at once (its persistent grid), and the SM count
-int main_grid_cap(int dev, int* sms_out) {
-  int n = dev < kMaxDevices ? g_grid[dev].load() : 0;
-  int sms = dev < kMaxDevices ? g_sms[dev].load() : 0;
-  if (n == 0 || sms == 0) {
-    int per = 1;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) sms = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_frappe_main, THREADS, 0) != cudaSuccess || per < 1)
-      per = 1;
-    n = sms * per;
-    if (dev < kMaxDevices) {
-      g_sms[dev].store(sms);
-      g_grid[dev].store(n);
-    }
-  }
-  *sms_out = sms;
-  return n;
-}
-
 int launch(const b200_frappe_args_t* args, void* stream, int train) {
-  if (!args) return fail(-1, "args is null");
+  if (!args) return E::fail(-1, "args is null");
   const b200_frappe_args_t& a = *args;
-  if (a.B < 1 || (int64_t)a.B * F > INT32_MAX) return fail(-1, "batch size must be in [1, 2^31 / 10)");
+  if (a.B < 1 || (int64_t)a.B * F > INT32_MAX) return E::fail(-1, "batch size must be in [1, 2^31 / 10)");
   if (!a.ids || !a.inv || !a.bet_deep || !a.bet_wide || !a.params || !a.logits || !a.workspace ||
       (train && (!a.n_unique || !a.labels || !a.loss || !a.grads || !a.gsum_deep || !a.gsum_wide)))
-    return fail(-1, "a buffer is null");
+    return E::fail(-1, "a buffer is null");
   if ((reinterpret_cast<uintptr_t>(a.bet_deep) & 15u) || (train && (reinterpret_cast<uintptr_t>(a.gsum_deep) & 15u)) ||
       (reinterpret_cast<uintptr_t>(a.params) & 7u))
-    return fail(-1, "bet_deep and gsum_deep must be 16-byte aligned, params 8-byte aligned");
+    return E::fail(-1, "bet_deep and gsum_deep must be 16-byte aligned, params 8-byte aligned");
   if (a.workspace_bytes < WS_BYTES)
-    return fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, needs " + std::to_string(WS_BYTES));
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(-2, "cudaGetDevice failed");
+    return E::fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, needs " + std::to_string(WS_BYTES));
+  entry::Device d;
+  int per = 0;  // the main pass runs a persistent grid: the CTAs that fit on the device at once
+  if (int rc = E::device(&d)) return rc;
+  if (int rc = E::blocks_per_sm(k_frappe_main, THREADS, 0, &per)) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  int sms = 1;
-  const int cap = main_grid_cap(dev, &sms);
   // at least one warp per entry of v and c; two CTAs per SM for the zeroing
-  const int pro = 2 * sms > (X + 1 + 7) / 8 ? 2 * sms : (X + 1 + 7) / 8;
+  const int pro = 2 * d.sms > (X + 1 + 7) / 8 ? 2 * d.sms : (X + 1 + 7) / 8;
   k_frappe_prologue<<<pro, 256, 0, st>>>(a, train);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_frappe_prologue: ") + cudaGetErrorString(e));
-  const int ntiles = (int)((a.B + TILE - 1) / TILE);
+  if (int rc = E::launched("k_frappe_prologue", g_launches, 0)) return rc;
+  const int ntiles = (int)((a.B + TILE - 1) / TILE), cap = d.sms * per;
   k_frappe_main<<<ntiles < cap ? ntiles : cap, THREADS, 0, st>>>(a, ntiles, train);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string("k_frappe_main: ") + cudaGetErrorString(e));
-  g_launches.fetch_add(1);
-  return 0;
+  return E::launched("k_frappe_main", g_launches);
 }
 
 }  // namespace
 
 extern "C" {
 
-const char* b200_frappe_last_error(void) { return g_err.c_str(); }
+const char* b200_frappe_last_error(void) { return E::last_error().c_str(); }
 int64_t b200_frappe_launch_count(void) { return g_launches.load(); }
 size_t b200_frappe_workspace_bytes(int64_t B) { return B < 1 ? 0 : WS_BYTES; }
 int b200_frappe_tower(const b200_frappe_args_t* args, void* stream) { return launch(args, stream, 1); }

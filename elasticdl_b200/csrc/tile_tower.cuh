@@ -186,17 +186,17 @@ __device__ __forceinline__ void sum_partials(float* P, int warp, int lane) {
 // training only, with 16-byte aligned deep records.
 inline int check_tile_args(const b200_deepfm_args_t* a, bool backward, const std::string& name) {
   if (check_common(a, backward)) return -1;
-  if (a->G > MAXG) return fail(-1, ("the " + name + " holds at most 38 id groups").c_str());
-  if (!a->scratch) return fail(-1, "null input");
+  if (a->G > MAXG) return E::fail(-1, "the " + name + " holds at most 38 id groups");
+  if (!a->scratch) return E::fail(-1, "null input");
   if (a->rows) {
     const b200_deepfm_rows_t* r = a->rows;
-    if (!backward) return fail(-1, ("the forward-only " + name + " reads pulled rows only").c_str());
+    if (!backward) return E::fail(-1, "the forward-only " + name + " reads pulled rows only");
     if (!r->uniq || r->deep_stride < D || r->wide_stride < 1 || r->deep_param_off < 0 || r->wide_param_off < 0 ||
         r->deep_stride % 4 || r->deep_param_off % 4)
-      return fail(-1, "bad row source");
+      return E::fail(-1, "bad row source");
     for (int g = 0; g < a->G; ++g)
       if (!r->deep_base[g] || !r->wide_base[g] || (reinterpret_cast<uintptr_t>(r->deep_base[g]) & 15))
-        return fail(-1, "bad row source");
+        return E::fail(-1, "bad row source");
   }
   return 0;
 }
@@ -222,31 +222,30 @@ using TilePrep = void (*)(dim3 grid, cudaStream_t st, const b200_deepfm_args_t& 
 // The tile kernel runs 2 CTAs per SM (its __launch_bounds__), at most one per tile; `launches` counts the launches.
 template <bool BACKWARD, auto Pulled, auto Table>
 int launch_tile_tower(const b200_deepfm_args_t* args, void* stream, int what, size_t smem, TilePrep prep,
-                      long long& launches) {
+                      entry::LaunchCount& launches) {
   cudaStream_t st = (cudaStream_t)stream;
-  int n_sm;
-  const int dev = current_device(&n_sm);
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
   b200_deepfm_args_t a = *args;
   if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
   float* w1x = a.scratch;  // W1x at the start of the scratch buffer, then the tile counter
   const long long ntile = ((long long)a.B + TS - 1) / TS;
-  long long grid = (long long)n_sm * 2;
+  long long grid = (long long)d.sms * 2;
   if (grid > ntile) grid = ntile;
   if (what & 1) {
     prep(dim3(4, BACKWARD ? a.G : 1), st, a, w1x, (int)grid);
-    launches += 1;
+    if (int rc = E::launched("tile tower prep", launches)) return rc;
   }
-  if (!(what & 2)) return launch_status();
+  if (!(what & 2)) return 0;
   if (BACKWARD && args->rows) {
     const size_t smem_u = smem + SM_U * sizeof(int);
-    max_dynamic_smem_once<Table>(dev, (int)smem_u);
+    if (int rc = E::raise_smem_limit(Table, smem_u)) return rc;
     Table<<<(unsigned)grid, THREADS, smem_u, st>>>(a, w1x, tile_rows(args->rows, a.G));
   } else {
-    max_dynamic_smem_once<Pulled>(dev, (int)smem);
+    if (int rc = E::raise_smem_limit(Pulled, smem)) return rc;
     Pulled<<<(unsigned)grid, THREADS, smem, st>>>(a, w1x, TileRows{});
   }
-  launches += 1;
-  return launch_status();
+  return E::launched("tile tower", launches);
 }
 
 }  // namespace deepfm

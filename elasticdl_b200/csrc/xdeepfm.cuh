@@ -78,6 +78,6 @@ __host__ __device__ inline CinScratch cin_scratch(int G, long long B) {
 // The Wide & Deep prep and tile kernel with the CIN logit added to z and dz stored (deepfm_tower2.cu), as
 // launch_tile_tower runs them (what: 1 prep, 2 tile kernel, 3 both), counted on `launches`.
 template <bool BACKWARD>
-int launch_xdeepfm_tile(const b200_deepfm_args_t* args, void* stream, int what, long long& launches);
+int launch_xdeepfm_tile(const b200_deepfm_args_t* args, void* stream, int what, entry::LaunchCount& launches);
 
 }  // namespace deepfm

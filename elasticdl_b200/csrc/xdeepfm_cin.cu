@@ -31,7 +31,7 @@ namespace {
 
 using namespace deepfm;
 
-long long g_launches = 0;
+entry::LaunchCount g_launches{0};
 
 constexpr int X1S = CIN_HALF * D;  // 512: X_1 / dX_1 / dC_0 of one sample, [64][8]
 constexpr int PS = CIN_P + 1;      // 193: p row stride in shared memory (odd: lane = sample reads are conflict-free)
@@ -570,50 +570,52 @@ __global__ void __launch_bounds__(THREADS, 1) k_cin_weights(b200_deepfm_args_t a
 template <bool BACKWARD>
 int launch(const b200_deepfm_args_t* args, void* stream, int what = 3) {
   if (check_tile_args(args, BACKWARD, "xDeepFM tile tower")) return -1;
-  if (args->G < 2) return fail(-1, "the xDeepFM tile tower needs at least 2 id groups");
+  if (args->G < 2) return E::fail(-1, "the xDeepFM tile tower needs at least 2 id groups");
   cudaStream_t st = (cudaStream_t)stream;
-  int n_sm;
-  const int dev = current_device(&n_sm);
+  entry::Device d;
+  if (int rc = E::device(&d)) return rc;
+  const int n_sm = d.sms;
   b200_deepfm_args_t a = *args;
   if (!BACKWARD) { a.grads = nullptr; a.gsum_deep = nullptr; a.gsum_wide = nullptr; a.loss = nullptr; }
   const long long ntile = ((long long)a.B + TS - 1) / TS;
   const int cin_grid = (int)(ntile < n_sm ? ntile : n_sm);  // one CTA per SM: the tile kernels take 150-230 KB
   if (what & 1) {
-    if (launch_xdeepfm_tile<BACKWARD>(args, stream, 1, g_launches)) return -2;
+    if (int rc = launch_xdeepfm_tile<BACKWARD>(args, stream, 1, g_launches)) return rc;
     k_cin_prep<<<2 * n_sm, THREADS, 0, st>>>(a, cin_grid);
-    g_launches += 1;
+    if (int rc = E::launched("k_cin_prep", g_launches)) return rc;
   }
-  if (!(what & 2)) return launch_status();
+  if (!(what & 2)) return 0;
   const bool table = BACKWARD && args->rows;
   const TileRows rows = table ? tile_rows(args->rows, a.G) : TileRows{};
   const size_t u = table ? SM_U * sizeof(int) : 0;
   if (table) {
-    max_dynamic_smem_once<k_cin_fwd<true, true>>(dev, (int)(FWD_BYTES + u));
+    if (int rc = E::raise_smem_limit(k_cin_fwd<true, true>, FWD_BYTES + u)) return rc;
     k_cin_fwd<true, true><<<cin_grid, THREADS, FWD_BYTES + u, st>>>(a, rows);
   } else {
-    max_dynamic_smem_once<k_cin_fwd<BACKWARD, false>>(dev, (int)FWD_BYTES);
+    if (int rc = E::raise_smem_limit(k_cin_fwd<BACKWARD, false>, FWD_BYTES)) return rc;
     k_cin_fwd<BACKWARD, false><<<cin_grid, THREADS, FWD_BYTES, st>>>(a, rows);
   }
-  g_launches += 1;
-  if (launch_xdeepfm_tile<BACKWARD>(args, stream, 2, g_launches)) return -2;
-  if (!BACKWARD) return launch_status();
+  if (int rc = E::launched("k_cin_fwd", g_launches)) return rc;
+  if (int rc = launch_xdeepfm_tile<BACKWARD>(args, stream, 2, g_launches)) return rc;
+  if (!BACKWARD) return 0;
   const CinShape sh = cin_shape(a.G);
   const int nb0 = (sh.k0 + 127) / 128, nb = nb0 + (sh.k1 + 127) / 128;
   const long long per = (ntile + (4LL * n_sm / nb) - 1) / max(1LL, 4LL * n_sm / nb);  // about 4 waves
   const unsigned ny = (unsigned)((ntile + per - 1) / per);
   if (table) {
-    max_dynamic_smem_once<k_cin_data<true>>(dev, (int)(DATA_BYTES + u));
+    if (int rc = E::raise_smem_limit(k_cin_data<true>, DATA_BYTES + u)) return rc;
     k_cin_data<true><<<cin_grid, THREADS, DATA_BYTES + u, st>>>(a, rows);
-    max_dynamic_smem_once<k_cin_weights<true>>(dev, (int)WGT_BYTES);
+    if (int rc = E::launched("k_cin_data", g_launches)) return rc;
+    if (int rc = E::raise_smem_limit(k_cin_weights<true>, WGT_BYTES)) return rc;
     k_cin_weights<true><<<dim3(nb, ny), THREADS, WGT_BYTES, st>>>(a, rows, nb0, (int)per);
   } else {
-    max_dynamic_smem_once<k_cin_data<false>>(dev, (int)DATA_BYTES);
+    if (int rc = E::raise_smem_limit(k_cin_data<false>, DATA_BYTES)) return rc;
     k_cin_data<false><<<cin_grid, THREADS, DATA_BYTES, st>>>(a, rows);
-    max_dynamic_smem_once<k_cin_weights<false>>(dev, (int)WGT_BYTES);
+    if (int rc = E::launched("k_cin_data", g_launches)) return rc;
+    if (int rc = E::raise_smem_limit(k_cin_weights<false>, WGT_BYTES)) return rc;
     k_cin_weights<false><<<dim3(nb, ny), THREADS, WGT_BYTES, st>>>(a, rows, nb0, (int)per);
   }
-  g_launches += 2;
-  return launch_status();
+  return E::launched("k_cin_weights", g_launches);
 }
 
 }  // namespace
@@ -626,7 +628,7 @@ size_t b200_deepfm_xdeepfm_scratch_floats(int G, int B) {
   return G < 1 || B < 1 ? 0 : (size_t)cin_scratch(G, B).total;
 }
 
-int64_t b200_deepfm_xdeepfm_launch_count(void) { return g_launches; }
+int64_t b200_deepfm_xdeepfm_launch_count(void) { return g_launches.load(); }
 
 int b200_deepfm_xdeepfm_fwd_bwd_tile(const b200_deepfm_args_t* args, void* stream) {
   return launch<true>(args, stream);
