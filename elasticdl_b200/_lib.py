@@ -65,6 +65,10 @@ class CensusArgs(ctypes.Structure):  # b200_census_args_t (include/b200_census.h
     ]
 
 
+class CsqlArgs(ctypes.Structure):  # b200_csql_args_t (include/b200_census_sqlflow.h)
+    _fields_ = CensusArgs._fields_
+
+
 class FrappeArgs(ctypes.Structure):  # b200_frappe_args_t (include/b200_frappe.h)
     _fields_ = [
         ("B", ctypes.c_int32), ("pad_", ctypes.c_int32),
@@ -264,6 +268,14 @@ CENSUS_SYMBOLS = {
     "b200_census_last_error": (ctypes.c_char_p, []),
     "b200_census_launch_count": (_i64, []),
 }
+# include/b200_census_sqlflow.h
+CSQL_SYMBOLS = {
+    "b200_csql_workspace_bytes": (_sz, [_i64]),
+    "b200_csql_tower": (_i, [ctypes.POINTER(CsqlArgs), _vp]),
+    "b200_csql_forward": (_i, [ctypes.POINTER(CsqlArgs), _vp]),
+    "b200_csql_last_error": (ctypes.c_char_p, []),
+    "b200_csql_launch_count": (_i64, []),
+}
 # include/b200_frappe.h
 FRAPPE_SYMBOLS = {
     "b200_frappe_workspace_bytes": (_sz, [_i64]),
@@ -302,7 +314,7 @@ def lib():
             path = _build.build()
         handle = ctypes.CDLL(path)
         for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items())\
-                + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()):
+                + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()) + list(CSQL_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args

@@ -159,6 +159,7 @@ struct Plan {  // passed by value (< 4 KB): the launch is self-contained and cap
   b200feat_dense_t dense[kMaxDense];
   float bnd[kMaxBoundaries];
   int G, n_dense;
+  unsigned long long absent;  // bit g: group g's ToSparse-dropped cells are absent (b200feat_group_ext_t::absent)
 };
 // A transform with LOOKUP / LOG_ROUND / ROUND_IDENTITY groups launches this one (7.4 KB, still by value); one without
 // them launches the Plan instance, whose parameters and code are those of the dac_ctr kinds alone.
@@ -189,6 +190,15 @@ __device__ inline long long vocab_lookup(uint64_t fp, const unsigned char* buf, 
   return num_oov > 0 ? (long long)e.V + (long long)(fp % (unsigned long long)num_oov) : -1;
 }
 
+// ToSparse's default ignore_value of a numeric column (to_sparse.py:55-63): -1 for integers, 0.0 for floats
+__device__ __forceinline__ bool ignored(long long x) { return x == -1; }
+__device__ __forceinline__ bool ignored(float x) { return x == 0.f; }
+
+// The id written for a cell: -1 for an absent one (the offset is not added), else id + offset
+__device__ __forceinline__ long long placed(long long id, bool absent, long long offset) {
+  return absent ? -1 : id + offset;
+}
+
 // LogRound / RoundIdentity: tf.cast(r, int64) then `r < 0 || r >= num_bins -> default`.  NaN, +-inf and
 // r >= 2^63 go to the default too: TF on x86 casts them to INT64_MIN (cvttsd2si), which is < 0.
 __device__ inline long long rounded_id(double r, long long num_bins, long long dflt) {
@@ -199,29 +209,34 @@ __device__ inline long long rounded_id(double r, long long num_bins, long long d
 
 // LOOKUP / LOG_ROUND / ROUND_IDENTITY ids of group g (the kind is uniform over the block row)
 template <typename T>
-__device__ __forceinline__ void ext_group_ids(const b200feat_group_t& gr, const GroupExt& ex, int g, const T* numeric,
-                                              const uint8_t* __restrict__ strings, int W, long long B, void* ids_out,
-                                              int ids32) {
+__device__ __forceinline__ void ext_group_ids(const b200feat_group_t& gr, const GroupExt& ex, int g, bool drop,
+                                              const T* numeric, const uint8_t* __restrict__ strings, int W, long long B,
+                                              void* ids_out, int ids32) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += stride) {
     long long id;
+    bool absent;
     if (gr.kind == B200FEAT_LOOKUP) {
       unsigned char buf[kMaxW];
       const int len = load_string(strings + ((long long)gr.column * B + b) * W, W, buf);
       id = vocab_lookup(fingerprint64(buf, len), buf, len, ex, gr.num_bins);
+      absent = drop && len == 0;
     } else if (gr.kind == B200FEAT_LOG_ROUND) {
       // tf.cast(x, float64), then log(x) or log(x) / log(base) in float64, tf.math.round = half to even
-      double q = log((double)numeric[(long long)gr.column * B + b]);
+      const T x = numeric[(long long)gr.column * B + b];
+      double q = log((double)x);
       if (ex.has_base) q = q / ex.log_base;
       id = rounded_id(rint(q), gr.num_bins, ex.dflt);
+      absent = drop && ignored(x);
     } else {  // ROUND_IDENTITY
       const T x = numeric[(long long)gr.column * B + b];
       if constexpr (std::is_same<T, long long>::value)  // integers pass through K.round unchanged
         id = x >= 0 && x < gr.num_bins ? x : ex.dflt;
       else  // K.round of float32 = rint in float32
         id = rounded_id((double)rintf(x), gr.num_bins, ex.dflt);
+      absent = drop && ignored(x);
     }
-    id += gr.offset;
+    id = placed(id, absent, gr.offset);
     if (ids32) reinterpret_cast<int*>(ids_out)[(long long)g * B + b] = (int)id;
     else reinterpret_cast<long long*>(ids_out)[(long long)g * B + b] = id;
   }
@@ -235,9 +250,10 @@ __global__ void __launch_bounds__(256) k_feature_transform(P p, const T* numeric
   const int g = blockIdx.y;
   if (g < p.G) {
     const b200feat_group_t& gr = p.group[g];
+    const bool drop = (p.absent >> g) & 1ull;
     if constexpr (std::is_same<P, PlanExt>::value) {
       if (gr.kind > B200FEAT_HASH_INT) {
-        ext_group_ids(gr, p.ext[g], g, numeric, strings, W, B, ids_out, ids32);
+        ext_group_ids(gr, p.ext[g], g, drop, numeric, strings, W, B, ids_out, ids32);
         return;
       }
     }
@@ -248,20 +264,26 @@ __global__ void __launch_bounds__(256) k_feature_transform(P p, const T* numeric
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += stride) {
       long long id;
+      bool absent = false;
       if (gr.kind == B200FEAT_DISCRETIZE) {
         // int64 inputs compare against float boundaries in float, like TF's BucketizeOp<T>
-        id = bucketize((float)numeric[(long long)gr.column * B + b], s_bnd, gr.n_boundaries);
+        const T x = numeric[(long long)gr.column * B + b];
+        id = bucketize((float)x, s_bnd, gr.n_boundaries);
+        absent = drop && ignored(x);
       } else {
         unsigned char buf[kMaxW];
         int len = 0;
         if (gr.kind == B200FEAT_HASH_STRING) {
           len = load_string(strings + ((long long)gr.column * B + b) * W, W, buf);
+          absent = drop && len == 0;
         } else if constexpr (std::is_same<T, long long>::value) {  // the host refuses HASH_INT over float columns
-          len = as_string(numeric[(long long)gr.column * B + b], buf);
+          const long long x = numeric[(long long)gr.column * B + b];
+          len = as_string(x, buf);
+          absent = drop && ignored(x);
         }
         id = (long long)(fingerprint64(buf, len) % (uint64_t)gr.num_bins);
       }
-      id += gr.offset;
+      id = placed(id, absent, gr.offset);
       if (ids32) reinterpret_cast<int*>(ids_out)[(long long)g * B + b] = (int)id;
       else reinterpret_cast<long long*>(ids_out)[(long long)g * B + b] = id;
     }
@@ -386,6 +408,8 @@ int b200feat_transform_ext(const b200feat_group_t* groups, const b200feat_group_
     }
     if (ids32 && ((__int128)gr.offset + lo < INT32_MIN || (__int128)gr.offset + hi > INT32_MAX))
       return E::fail(-1, "int32 ids: offset + id range of a group does not fit int32");
+    if (ext && ext[g].absent != 0 && ext[g].absent != 1) return E::fail(-1, "absent must be 0 or 1");
+    if (ext && ext[g].absent) p.absent |= 1ull << g;
     p.group[g] = gr;
     ext_kinds |= gr.kind > B200FEAT_HASH_INT;
   }

@@ -19,6 +19,7 @@ struct Ps {};        // b200ps.h
 struct DeepFm {};    // b200_deepfm.h: the fused, tile, mma, DCN and xDeepFM towers
 struct Features {};  // b200_features.h
 struct Census {};    // b200_census.h
+struct CensusSqlflow {};  // b200_census_sqlflow.h
 struct Frappe {};    // b200_frappe.h
 struct FcDnn {};     // b200_fc_dnn.h
 struct Metrics {};   // b200_metrics.h

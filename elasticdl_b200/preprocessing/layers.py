@@ -344,7 +344,7 @@ class FeatureDense(ctypes.Structure):  # b200feat_dense_t
 class FeatureGroupExt(ctypes.Structure):  # b200feat_group_ext_t
     _fields_ = [("slots_dev", ctypes.c_void_p), ("terms_dev", ctypes.c_void_p), ("n_slots", ctypes.c_int64),
                 ("V", ctypes.c_int32), ("Wv", ctypes.c_int32), ("default_value", ctypes.c_int64),
-                ("has_base", ctypes.c_int32), ("pad", ctypes.c_int32), ("base", ctypes.c_double)]
+                ("has_base", ctypes.c_int32), ("absent", ctypes.c_int32), ("base", ctypes.c_double)]
 
 
 DISCRETIZE, HASH_STRING, HASH_INT, LOOKUP, LOG_ROUND, ROUND_IDENTITY = 0, 1, 2, 3, 4, 5
@@ -360,7 +360,8 @@ class FeatureTransform:
         {"kind": "lookup", "column": string column, "vocabulary": list | path, "num_oov_tokens": 1} or
         {"kind": "log_round", "column": numeric column, "num_bins": n, "default_value": 0, "base": None} or
         {"kind": "round_identity", "column": numeric column, "num_buckets": n, "default_value": 0},
-    plus an optional "offset"; bins are sorted; with ids_dtype=torch.int32 every group's ids (offset plus
+    plus an optional "offset" and an optional "absent": True -- a cell ToSparse drops with its default
+    ignore_value (an empty string, a float 0.0, an int64 -1) gets id -1, without the offset; bins are sorted; with ids_dtype=torch.int32 every group's ids (offset plus
     [0, max_id), and -1 / default_value where a group can give them) must fit int32.
     dense: list of (numeric column, subtractor, divisor) -- the Normalizer columns.
     device: where lookup groups keep their vocabulary tables (built at construction; default: the current device).
@@ -382,6 +383,7 @@ class FeatureTransform:
             fg, ext = self._groups[g], self._ext[g]
             fg.column = int(spec["column"])
             fg.offset = int(spec.get("offset", 0))
+            ext.absent = 1 if spec.get("absent", False) else 0
             lo, hi = 0, None  # smallest and (where it is not max_id - 1) largest id before the offset
             if spec["kind"] == "discretize":
                 fg.kind, fg.n_boundaries, fg.boundary_off = DISCRETIZE, len(spec["bins"]), len(bnd)

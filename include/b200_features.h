@@ -92,7 +92,11 @@ typedef struct {
   int32_t Wv;                             /* LOOKUP: term row width, 1..64 */
   int64_t default_value;                  /* LOG_ROUND, ROUND_IDENTITY: the id of a value outside [0, num_bins) */
   int32_t has_base;                       /* LOG_ROUND: 0 = natural log (base None), 1 = log(x) / log(base) */
-  int32_t pad;
+  int32_t absent;                         /* any kind: 0 = every cell gets an id; 1 = a cell ToSparse drops with
+                                           * its default ignore_value (to_sparse.py:55-63) -- an empty string, a
+                                           * float32 0.0 (-0.0 too) or an int64 -1 -- is absent: its id is -1,
+                                           * without the offset.  (A LOOKUP without OOV tokens still writes
+                                           * -1 + offset for an unknown string.) */
   double base;                            /* LOG_ROUND with has_base */
 } b200feat_group_ext_t;
 
