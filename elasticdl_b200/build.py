@@ -9,7 +9,7 @@ SOURCES = ["b200ps.cu", "deepfm_tower.cu", "deepfm_tower_mma.cu", "deepfm_tower2
            "feature_ids.cu", "census_tower.cu", "frappe_tower.cu", "eval_metrics.cu", "fc_dnn_tower.cu",
            "census_sqlflow_tower.cu"]
 HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "ps_unique.cuh", "deepfm_common.cuh",
-           "tile_tower.cuh", "mma_tf32.cuh", "xdeepfm.cuh", "launch.cuh",
+           "tile_tower.cuh", "mma_tf32.cuh", "xdeepfm.cuh", "launch.cuh", "census_tower.cuh",
            os.path.join("..", "..", "include", "b200ps.h"),
            os.path.join("..", "..", "include", "b200_deepfm.h"),
            os.path.join("..", "..", "include", "b200_features.h"),

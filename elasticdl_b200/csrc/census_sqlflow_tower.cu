@@ -1,49 +1,31 @@
 // census_model_sqlflow wide & deep tower (include/b200_census_sqlflow.h): mean-pooled sparse lookups over the
-// present ids, forward, loss, backward, MLP gradients and the five compacted push_rows segments in one launch.
+// present ids, forward, loss, backward, MLP gradients and the five compacted push_rows segments in one launch, on
+// the machinery of census_tower.cuh.
 //
-// The census tower's linear backward (csrc/census_tower.cu) with a per-sample divisor: the MLP has no activation
-// and its output is summed, so with v3 = W3 1, v2 = W2 v3 and v1 = W1 v2 every gradient is a batch sum of scalars
-// times a fixed vector.  A pooled vector is the mean over n_g(s) present ids, so where the census tower adds dz
-// to a (group, row) column per occurrence, this one adds dz / n_g(s):
+// A pooled vector is the mean over the n_g(s) present ids of its group and sample, so where the census tower adds
+// dz to a (group, row) column per occurrence, this one adds dz / n_g(s):
 //   wide row r of group g:  sum over samples b and occurrences of r among b's present ids of dz(b) / n_g(b)
 //   deep row r of group g:  sum over DNN input slots k of (the same sum over the samples s slot k reads) v1[8k..]
-// A group with no present id pools to zero and touches no row.  The kernel accumulates 50 dense sums and 5
-// scalars per (group, row) -- wide, slots 0..2, occurrences -- in registers of the threads that own them,
-// sweeping each tile's samples in order; no float atomics, so the summation order is fixed.
-//
-// Grid: at most one CTA per SM, grid-striding over tiles of 256 samples; the whole model (9.5 KB) is staged in
-// shared memory.  Each CTA writes one partial of its sums; the last CTA to arrive adds the partials in CTA order,
-// writes the outputs, compacts the touched rows and resets the arrival counter.  The forward form stops after
-// the logits.
-#include <cuda_runtime.h>
-
-#include <cstdint>
-#include <string>
-
+// A group with no present id pools to zero and touches no row.  The whole model (9.5 KB) is staged in shared
+// memory.  The forward form stops after the logits.
 #include "../../include/b200_census_sqlflow.h"
-#include "launch.cuh"
+#include "census_tower.cuh"
 
 namespace {
 
+using namespace census;
 using E = entry::Entry<entry::CensusSqlflow>;
+using S = Shape<27, 73, 113>;
+static_assert(S::NPARAM == B200_CSQL_PARAMS && MLP == B200_CSQL_MLP && S::UNIQ_ROWS == B200_CSQL_UNIQ_ROWS &&
+                  S::GSUM_FLOATS == B200_CSQL_GSUM_FLOATS && TILE == B200_CSQL_TILE,
+              "include/b200_census_sqlflow.h");
+static_assert(S::SDEEP == S::DEEP0, "the parameters are staged as they are");
 entry::LaunchCount g_launches{0};
-
-constexpr int TILE = B200_CSQL_TILE;
-constexpr int THREADS = 288;  // 256 samples in the forward; 213 row columns + 50 dense sums in the sweep
-// flat parameter offsets (b200_census_sqlflow.h)
-constexpr int OW1 = 0, OB1 = 384, OW2 = 400, OB2 = 528, OW3 = 536, OB3 = 568, MLP = B200_CSQL_MLP;
-constexpr int WIDE0 = 572, WIDE1 = 599, DEEP0 = 672, NPARAM = B200_CSQL_PARAMS;
-static_assert(DEEP0 % 4 == 0, "the deep block is read as float4 from shared memory");
-constexpr int NCOL = 213;  // (group, row) columns: group 0 at 0..26, 1 at 27..99, 2 at 100..212
-constexpr int NDQ = 50;    // dense sums: dz, dz x[24] @1, dz h1[16] @25, dz h2[8] @41, loss @49
-constexpr int CQ = 5;      // per column: wide, slot 0, slot 1, slot 2, occurrences
-constexpr int Q = NDQ + NCOL * CQ;  // floats of one CTA's partial
-constexpr int SV = TILE + 1;        // padded: the dense sums read column q of row r conflict-free
 
 struct Smem {
   int4 ent[3][TILE];   // the four ids of DNN input slot k of tile row r (-1 = absent)
   int4 own[2][TILE];   // the four ids of wide groups 0 and 1 of tile row r
-  float p[NPARAM];     // parameters
+  float p[S::SP];      // parameters
   float v[48];         // v3 @0, v2 @8, v1 @24
   int entg[3][TILE];   // the id group of slot k of row r
   float ds[3][TILE];   // dz of row r over the present-id count of slot k's group and sample (0 when none)
@@ -52,9 +34,6 @@ struct Smem {
   float sv[NDQ][SV];   // per-row values of the dense sums; the last CTA's totals afterwards
   int last;
 };
-
-__device__ __forceinline__ int group_rows(int g) { return g == 0 ? 27 : (g == 1 ? 73 : 113); }
-__device__ __forceinline__ int deep_off(int g) { return g == 0 ? DEEP0 : (g == 1 ? 888 : 1472); }
 
 // -1 for an absent id; an id outside [-1, rows) is counted in `bad` and read as absent
 __device__ __forceinline__ int load_id(const int32_t* ids, int row, int64_t B, int64_t s, int rows, int& bad) {
@@ -67,7 +46,7 @@ __device__ __forceinline__ int load_id(const int32_t* ids, int row, int64_t B, i
 }
 
 __device__ __forceinline__ int4 load_group(const int32_t* ids, int g, int64_t B, int64_t s, int& bad) {
-  const int rows = group_rows(g);
+  const int rows = S::rows(g);
   int4 e;
   e.x = load_id(ids, 4 * g + 0, B, s, rows, bad);
   e.y = load_id(ids, 4 * g + 1, B, s, rows, bad);
@@ -84,7 +63,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
   const int t = threadIdx.x;
   const int64_t B = a.B;
   const bool quirk = a.reference_reshape != 0;
-  for (int i = t; i < NPARAM; i += THREADS) s.p[i] = __ldg(a.params + i);
+  for (int i = t; i < S::NPARAM; i += THREADS) s.p[i] = __ldg(a.params + i);
   __syncthreads();
   if (train) {
     if (t < 8) {
@@ -109,18 +88,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
     }
   }
 
-  int cg = -1, crow = 0;  // this thread's (group, row) column in the sweep
-  if (t < 27) {
-    cg = 0;
-    crow = t;
-  } else if (t < 100) {
-    cg = 1;
-    crow = t - 27;
-  } else if (t < NCOL) {
-    cg = 2;
-    crow = t - 100;
-  }
-  const int dq = t - NCOL;  // this thread's dense sum when 0 <= dq < NDQ
+  const Column col = column_of<S>(t);
+  const int cg = col.g, crow = col.row;
   float acc_w = 0.f, acc_0 = 0.f, acc_1 = 0.f, acc_2 = 0.f, acc_q = 0.f;
   int occ = 0, bad = 0;
 
@@ -135,16 +104,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
       for (int k = 0; k < 3; ++k) {
         int g;
         int64_t smp;
-        if (quirk) {  // Q11: slot k of row b is stacked row 3b + k of [3, B, 8]
-          const int64_t f = 3 * b + k;
-          g = (int)(f / B);
-          smp = f - g * B;
-        } else {
-          g = k;
-          smp = b;
-        }
+        slot_source(quirk, b, k, B, g, smp);
         const int4 e = load_group(a.ids, g, B, smp, bad);
-        const float4* d = reinterpret_cast<const float4*>(s.p + deep_off(g));
+        const float4* d = reinterpret_cast<const float4*>(s.p + S::deep_soff(g));
         const int ids4[4] = {e.x, e.y, e.z, e.w};
         float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
 #pragma unroll
@@ -169,7 +131,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
       for (int g = 0; g < 2; ++g) {
         int dummy = 0;  // counted once, through the slots above
         const int4 o = load_group(a.ids, g, B, b, dummy);
-        const float* w = s.p + (g == 0 ? WIDE0 : WIDE1);
+        const float* w = s.p + (g == 0 ? S::WIDE0 : S::WIDE1);
         float sum = 0.f;
         if (o.x >= 0) sum += w[o.x];
         if (o.y >= 0) sum += w[o.y];
@@ -179,44 +141,20 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
         wide += sum / (wcnt[g] ? (float)wcnt[g] : 1.f);
         if (train) s.own[g][t] = o;
       }
-      float h1[16], h2[8], h3[4];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) h1[j] = s.p[OB1 + j];
-#pragma unroll
-      for (int i = 0; i < 24; ++i)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) h1[j] = fmaf(x[i], s.p[OW1 + i * 16 + j], h1[j]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) h2[j] = s.p[OB2 + j];
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) h2[j] = fmaf(h1[i], s.p[OW2 + i * 8 + j], h2[j]);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) h3[j] = s.p[OB3 + j];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) h3[j] = fmaf(h2[i], s.p[OW3 + i * 4 + j], h3[j]);
-      const float z = wide + ((h3[0] + h3[1]) + (h3[2] + h3[3]));
+      float h1[16], h2[8];
+      const float z = mlp_forward(s.p, x, wide, h1, h2);
       a.logits[b] = z;
       if (train) {
         const float y = __ldg(a.labels + b);
-        const float lb = fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));  // sigmoid cross-entropy with logits
-        const float p = 1.f / (1.f + expf(-z));
+        float p;
+        const float lb = sample_loss(z, y, p);
         const float dzb = (p - y) / (float)B;
         s.dz[t] = dzb;
 #pragma unroll
         for (int k = 0; k < 3; ++k) s.ds[k][t] = cnt[k] ? dzb / (float)cnt[k] : 0.f;
 #pragma unroll
         for (int g = 0; g < 2; ++g) s.dw[g][t] = wcnt[g] ? dzb / (float)wcnt[g] : 0.f;
-#pragma unroll
-        for (int i = 0; i < 24; ++i) s.sv[1 + i][t] = x[i];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) s.sv[25 + i][t] = h1[i];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s.sv[41 + i][t] = h2[i];
-        s.sv[49][t] = lb;
+        put_row(s.sv, t, x, h1, h2, lb);
       }
     }
     if (!train) continue;  // uniform: the forward form has no sweep and no barrier in the tile
@@ -256,14 +194,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
 #undef CSQL_SLOT
         }
       }
-    } else if (dq < NDQ) {
-      if (dq == 0) {
-        for (int r = 0; r < n; ++r) acc_q += s.dz[r];
-      } else if (dq == NDQ - 1) {
-        for (int r = 0; r < n; ++r) acc_q += s.sv[dq][r];
-      } else {
-        for (int r = 0; r < n; ++r) acc_q = fmaf(s.dz[r], s.sv[dq][r], acc_q);
-      }
+    } else if (col.dq < NDQ) {
+      acc_q = dense_sweep(s.dz, s.sv, col.dq, n, acc_q);
     }
     __syncthreads();
   }
@@ -271,101 +203,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_census_sqlflow_tower(b200_csql_a
     if (bad) atomicAdd(a.error, bad);
     return;
   }
-
-  unsigned* counter = entry::arrival_counter(a.workspace);
-  float* parts = entry::partials(a.workspace);
-  float* mine = parts + (size_t)blockIdx.x * Q;
-  if (cg >= 0) {
-    float* c = mine + NDQ + t * CQ;
-    c[0] = acc_w;
-    c[1] = quirk ? acc_0 : (cg == 0 ? acc_w : 0.f);
-    c[2] = quirk ? acc_1 : (cg == 1 ? acc_w : 0.f);
-    c[3] = quirk ? acc_2 : (cg == 2 ? acc_w : 0.f);
-    c[4] = (float)occ;
-  } else if (dq < NDQ) {
-    mine[dq] = acc_q;
-  }
-  if (bad) atomicAdd(a.error, bad);
-  if (!entry::last_to_arrive(counter, s.last)) return;
-
-  float* tot = &s.sv[0][0];
-  entry::sum_partials<THREADS>(parts, Q, [&](int q, float v) { tot[q] = v; });
-  __syncthreads();
-  const float* v3 = s.v;
-  const float* v2 = s.v + 8;
-  const float* v1 = s.v + 24;
-  if (t == 0) *a.loss = tot[NDQ - 1] / (float)B;
-  for (int i = t; i < MLP; i += THREADS) {
-    float g;
-    if (i < OB1) g = tot[1 + i / 16] * v2[i % 16];
-    else if (i < OW2) g = tot[0] * v2[i - OB1];
-    else if (i < OB2) g = tot[25 + (i - OW2) / 8] * v3[(i - OW2) % 8];
-    else if (i < OW3) g = tot[0] * v3[i - OB2];
-    else if (i < OB3) g = tot[41 + (i - OW3) / 4];
-    else g = tot[0];
-    a.grads[i] = g;
-  }
-  const int w = t >> 5, lane = t & 31;
-  if (w < 5) {  // table w: wide groups 0, 1 (w = 0, 1), deep groups 0..2 (w = 2..4)
-    const int g = w < 2 ? w : w - 2;
-    const int rows = group_rows(g);
-    const int col0 = g == 0 ? 0 : (g == 1 ? 27 : 100);
-    const int uoff = w == 0 ? 0 : w == 1 ? 27 : w == 2 ? 100 : w == 3 ? 127 : 200;
-    const int goff = w == 0 ? 0 : w == 1 ? 27 : w == 2 ? 100 : w == 3 ? 316 : 900;
-    int cnt = 0;
-    for (int r0 = 0; r0 < rows; r0 += 32) {
-      const int row = r0 + lane;
-      const float* c = tot + NDQ + (col0 + row) * CQ;
-      const bool touched = row < rows && c[4] > 0.f;
-      const unsigned m = __ballot_sync(0xffffffffu, touched);
-      if (touched) {
-        const int pos = cnt + __popc(m & ((1u << lane) - 1u));
-        a.uniq[uoff + pos] = row;
-        if (w < 2) {
-          a.gsum[goff + pos] = c[0];
-        } else {
-#pragma unroll
-          for (int d = 0; d < 8; ++d) a.gsum[goff + pos * 8 + d] = (c[1] * v1[d] + c[2] * v1[8 + d]) + c[3] * v1[16 + d];
-        }
-      }
-      cnt += __popc(m);
-    }
-    if (lane == 0) a.n_unique[w] = cnt;
-  }
-  if (t == 0) *counter = 0u;
+  finish<S>(a, s, col, Sums{acc_w, acc_0, acc_1, acc_2, occ, acc_q}, bad, quirk);
 }
 
-// at most one CTA per SM
-int grid_for(int64_t B, int* grid) {
-  entry::Device d;
-  if (int rc = E::device(&d)) return rc;
-  const int64_t tiles = (B + TILE - 1) / TILE;
-  *grid = (int)(tiles < d.sms ? tiles : d.sms);
-  return 0;
-}
-
-int launch(const b200_csql_args_t* args, void* stream, int train) {
-  if (!args) return E::fail(-1, "args is null");
-  const b200_csql_args_t& a = *args;
-  // 12 B ids must be addressable with a 32-bit row stride times 12
-  if (a.B < 1 || (int64_t)a.B * 12 > INT32_MAX) return E::fail(-1, "batch size must be in [1, 2^31 / 12)");
-  if (a.reference_reshape != 0 && a.reference_reshape != 1) return E::fail(-1, "reference_reshape must be 0 or 1");
-  if (!a.ids || !a.params || !a.logits || !a.error) return E::fail(-1, "a buffer is null");
-  if (train && (!a.labels || !a.loss || !a.grads || !a.uniq || !a.n_unique || !a.gsum || !a.workspace))
-    return E::fail(-1, "a buffer is null");
-  int grid = 0;
-  if (int rc = grid_for(a.B, &grid)) return rc;
-  if (train) {
-    const size_t need = entry::partials_bytes(grid, Q);
-    if (a.workspace_bytes < need)
-      return E::fail(-1, "workspace of " + std::to_string(a.workspace_bytes) + " bytes, batch " + std::to_string(a.B) +
-                             " needs " + std::to_string(need));
-  }
-  const size_t smem = sizeof(Smem);
-  if (int rc = E::raise_smem_limit(k_census_sqlflow_tower, smem)) return rc;
-  const int ntiles = (int)((a.B + TILE - 1) / TILE);
-  k_census_sqlflow_tower<<<grid, THREADS, smem, (cudaStream_t)stream>>>(a, ntiles, train);
-  return E::launched("k_census_sqlflow_tower", g_launches);
+int launch_tower(const b200_csql_args_t* args, void* stream, int train) {
+  return launch<S, E>(k_census_sqlflow_tower, "k_census_sqlflow_tower", g_launches, sizeof(Smem), args, stream,
+                      train != 0, train);
 }
 
 }  // namespace
@@ -374,14 +217,9 @@ extern "C" {
 
 const char* b200_csql_last_error(void) { return E::last_error().c_str(); }
 int64_t b200_csql_launch_count(void) { return g_launches.load(); }
+size_t b200_csql_workspace_bytes(int64_t B) { return workspace_bytes<S, E>(B); }
 
-size_t b200_csql_workspace_bytes(int64_t B) {
-  int grid = 0;
-  if (B < 1 || grid_for(B, &grid)) return 0;
-  return entry::partials_bytes(grid, Q);
-}
-
-int b200_csql_tower(const b200_csql_args_t* args, void* stream) { return launch(args, stream, 1); }
-int b200_csql_forward(const b200_csql_args_t* args, void* stream) { return launch(args, stream, 0); }
+int b200_csql_tower(const b200_csql_args_t* args, void* stream) { return launch_tower(args, stream, 1); }
+int b200_csql_forward(const b200_csql_args_t* args, void* stream) { return launch_tower(args, stream, 0); }
 
 }  // extern "C"

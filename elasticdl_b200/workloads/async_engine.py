@@ -54,6 +54,14 @@ class AsyncEngine:
         for t, (name, dtype, shape) in zip(tensors, self.inputs):
             check_tensor(t, name, dtype, shape, self.device)
 
+    def step(self, *inputs):
+        """One training step on a batch, one tensor per declared input; returns the loss (device scalar, not
+        synchronised)."""
+        self._check_batch(*inputs)
+        out = self._step(*inputs)
+        self.steps += 1
+        return out
+
     def _push(self, st):
         """push_begin -> push_dense -> push_rows -> push_end on stream `st`, with no host read."""
         g, lib = self.group, self.group.lib

@@ -12,6 +12,7 @@ Every table is under 2 MB, so the reference's ModelHandler keeps it a dense Kera
 IndexedSlices that the PS applies with the Indexed kernels (only the rows of the batch move).  Each is one dense
 PS parameter here, on shard string_to_id(name), and the tables' rows are pushed with b200ps_push_rows.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -90,8 +91,21 @@ def callbacks():
     return [LearningRateScheduler(PiecewiseConstantDecay([4999, 11999], [3e-4, 2e-4, 1e-4]))]
 
 
-class CensusTowerCall:
-    """The census tower's output buffers and workspace for batch B on `device`, and one launch over them."""
+# What a census-style wide & deep tower's entry points and buffers depend on (SPEC here, census_sqlflow.SPEC):
+# the entry points' prefix and argument struct, the groups' rows, the push_rows segments' offsets and sizes, the
+# flat sizes, what the range error says after its count, and whether a forward-only entry point (<prefix>_forward)
+# exists.
+TowerSpec = collections.namedtuple("TowerSpec", "prefix args group_rows uniq_off n_uniq gsum_off n_gsum n_params n_mlp "
+                                                "range_error forward")
+SPEC = TowerSpec("b200_census", CensusArgs, GROUP_ROWS, UNIQ_OFF, N_UNIQ, GSUM_OFF, N_GSUM, N_PARAMS, N_MLP,
+                 "census ids outside [0, rows of their group) %s were read as row 0" % (GROUP_ROWS,), False)
+
+
+class TowerCall:
+    """A census-style tower's output buffers and workspace for batch B on `device`, and one launch over them; a
+    subclass sets `spec`, a TowerSpec."""
+
+    spec = None
 
     def __init__(self, B, device):
         self.B = int(B)
@@ -99,18 +113,19 @@ class CensusTowerCall:
             raise ValueError("batch size must be >= 1, not %d" % self.B)
         self.device = torch.device(device)
         self.lib = _lib.lib()
+        sp = self.spec
         f32 = dict(dtype=torch.float32, device=self.device)
         self.loss = torch.zeros(1, **f32)
         self.logits = torch.zeros(self.B, **f32)
-        self.grads = torch.zeros(N_MLP, **f32)
-        self.uniq = torch.zeros(N_UNIQ, dtype=torch.int64, device=self.device)
+        self.grads = torch.zeros(sp.n_mlp, **f32)
+        self.uniq = torch.zeros(sp.n_uniq, dtype=torch.int64, device=self.device)
         self.n_unique = torch.zeros(5, dtype=torch.int32, device=self.device)
-        self.gsum = torch.zeros(N_GSUM, **f32)
+        self.gsum = torch.zeros(sp.n_gsum, **f32)
         self.error = torch.zeros(1, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
-            nbytes = self.lib.b200_census_workspace_bytes(self.B)
+            nbytes = getattr(self.lib, sp.prefix + "_workspace_bytes")(self.B)
         self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        a = CensusArgs()
+        a = sp.args()
         a.B = self.B
         a.loss, a.logits, a.grads = self.loss.data_ptr(), self.logits.data_ptr(), self.grads.data_ptr()
         a.uniq, a.n_unique, a.gsum = self.uniq.data_ptr(), self.n_unique.data_ptr(), self.gsum.data_ptr()
@@ -118,18 +133,25 @@ class CensusTowerCall:
         self.args = a
 
     def check_inputs(self, ids, labels, flat):
+        """labels may be None where the tower has a forward form."""
         check_tensor(ids, "ids", torch.int32, (12, self.B), self.device)
-        check_tensor(labels, "labels", torch.float32, (self.B,), self.device)
-        check_tensor(flat, "params", torch.float32, (N_PARAMS,), self.device)
+        if labels is not None or not self.spec.forward:
+            check_tensor(labels, "labels", torch.float32, (self.B,), self.device)
+        check_tensor(flat, "params", torch.float32, (self.spec.n_params,), self.device)
 
-    def launch(self, ids, labels, flat, reference_reshape):
-        """One tower launch on the current stream (no checks, no host read)."""
+    def launch(self, ids, labels, flat, reference_reshape, train=True):
+        """One tower launch (train=False: the forward form, logits only) on the current stream (no checks, no host
+        read)."""
+        if not (train or self.spec.forward):
+            raise ValueError("%s has no forward form" % self.spec.prefix)
         a = self.args
-        a.ids, a.labels, a.params = ids.data_ptr(), labels.data_ptr(), flat.data_ptr()
+        a.ids, a.params = ids.data_ptr(), flat.data_ptr()
+        a.labels = labels.data_ptr() if labels is not None else None
         a.reference_reshape = 1 if reference_reshape else 0
+        fn = getattr(self.lib, self.spec.prefix + ("_tower" if train else "_forward"))
         with torch.cuda.device(self.device):
-            rc = self.lib.b200_census_tower(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check_call(rc, "b200_census_tower", self.lib.b200_census_last_error)
+            rc = fn(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        _lib.check_call(rc, fn.__name__, getattr(self.lib, self.spec.prefix + "_last_error"))
 
     def check_error(self):
         """Raise PSRangeError (a ValueError) if a launch since the last check read an id outside its group, and
@@ -137,18 +159,24 @@ class CensusTowerCall:
         n = int(self.error.item())
         if n:
             self.error.zero_()
-            raise _lib.PSRangeError(_lib.ERANGE, "%d census ids outside [0, rows of their group) %s were read as "
-                                                 "row 0" % (n, GROUP_ROWS))
+            raise _lib.PSRangeError(_lib.ERANGE, "%d %s" % (n, self.spec.range_error))
 
     def outputs(self):
         """{loss, logits, grads, uniq [5], n_unique [5], gsum [5 segments: [rows, dim]]} (views of the buffers)."""
         out = {"loss": self.loss.reshape(()), "logits": self.logits, "grads": self.grads, "n_unique": self.n_unique,
                "uniq": [], "gsum": []}
+        sp = self.spec
         for t in range(5):
-            rows = GROUP_ROWS[TABLE_GROUP[t]]
-            out["uniq"].append(self.uniq[UNIQ_OFF[t]:UNIQ_OFF[t] + rows])
-            out["gsum"].append(self.gsum[GSUM_OFF[t]:GSUM_OFF[t] + rows * TABLE_DIM[t]].view(rows, TABLE_DIM[t]))
+            rows = sp.group_rows[TABLE_GROUP[t]]
+            out["uniq"].append(self.uniq[sp.uniq_off[t]:sp.uniq_off[t] + rows])
+            out["gsum"].append(self.gsum[sp.gsum_off[t]:sp.gsum_off[t] + rows * TABLE_DIM[t]].view(rows, TABLE_DIM[t]))
         return out
+
+
+class CensusTowerCall(TowerCall):
+    """The census tower's output buffers and workspace for batch B on `device`, and one launch over them."""
+
+    spec = SPEC
 
 
 def census_tower(ids, labels, flat, reference_reshape=False):
@@ -163,65 +191,108 @@ def census_tower(ids, labels, flat, reference_reshape=False):
     return call.outputs()
 
 
-class CensusWideDeepEngine(AsyncEngine):
-    """One async worker of the census wide & deep model on the parameter-server step.
+def _split(flat, shapes):
+    """Views of consecutive blocks of `flat` in `shapes`."""
+    out, o = [], 0
+    for s in shapes:
+        out.append(flat[o:o + int(np.prod(s))].view(s))
+        o += int(np.prod(s))
+    return out
 
-    group: an async PSGroup, as AsyncEngine takes it.  register=True registers the eleven parameters and sets their
-    initial values first-writer-wins (as PushModel does); register=False attaches to a group.clone_view() of a
-    group where another engine registered them, for another worker thread.
+
+class WideDeepEngine(AsyncEngine):
+    """One async worker of a census-style wide & deep model on the parameter-server step: the body of
+    CensusWideDeepEngine and census_sqlflow.CensusSqlflowEngine.
+
     step(numeric float32 [4, B], strings uint8 [8, B, 32], labels float32 [B]) runs pull_dense (into the flat
-    buffer) -> census_transform -> the tower -> push_begin -> push_dense (MLP) -> push_rows (the five tables'
+    buffer) -> the feature transform -> the tower -> push_begin -> push_dense (MLP) -> push_rows (the five tables'
     touched rows, counts on the device) -> push_end, with no host read, and returns the loss on the device.
     capture() / replay() run the same step as one CUDA graph over static inputs; a new learning rate re-captures.
-    lr_schedule: a schedule to install, as AsyncEngine.set_lr_schedule does."""
+    A subclass runs AsyncEngine.__init__, sets `reference_reshape` and calls _setup()."""
 
-    def __init__(self, group, batch, lr, reference_reshape=False, seed=0, register=True, lr_schedule=None):
-        super().__init__(group, batch, lr, register, lr_schedule)
+    def _setup(self, names, shapes, initial_params, seed, transform, tower, register):
+        """names, shapes: the eleven parameters in flat order; register=True registers them and sets their initial
+        values, initial_params(seed, device), first-writer-wins (as PushModel does).  transform: the model's feature
+        transform (raw rows -> int32 ids [12, B]); tower: its TowerCall class."""
         g, B = self.group, self.B
         self.inputs = [("numeric", torch.float32, (4, B)), ("strings", torch.uint8, (8, B, STRING_WIDTH)),
                        ("labels", torch.float32, (B,))]
-        self.reference_reshape = bool(reference_reshape)
-        self.owner = {n: string_to_id(n, g.n_shards) for n, _ in PARAMS}
+        self.names = names
+        self.owner = {n: string_to_id(n, g.n_shards) for n in names}
         if register:
-            for n, s in PARAMS:
+            for n, s in zip(names, shapes):
                 g.register_dense(n, s, self.owner[n])
             g.commit()
-            g.init_dense(flat_views(initial_params(seed, self.device)).items())
-        tids = [g.lookup(n)[0] for n, _ in PARAMS]  # PSNotFound when no engine registered them
-        self.flat = torch.zeros(N_PARAMS, dtype=torch.float32, device=self.device)
-        self.views = flat_views(self.flat)
+            g.init_dense(zip(names, _split(initial_params(seed, self.device), shapes)))
+        tids = [g.lookup(n)[0] for n in names]  # PSNotFound when no engine registered them
+        self.flat = torch.zeros(tower.spec.n_params, dtype=torch.float32, device=self.device)
         self.ids = torch.zeros((12, B), dtype=torch.int32, device=self.device)
-        self.transform = census_transform(torch.int32, device=self.device)
-        self.tower = CensusTowerCall(B, self.device)
-        t = self.tower
-        self.pull_segs = g.make_segs([(tid, 0, None, None, self.views[n]) for tid, (n, _) in zip(tids, PARAMS)])
-        self.push_dense_segs = g.make_segs([(tids[i], 0, None, None, t.grads[OFFSETS[n]:OFFSETS[n] + int(np.prod(s))])
-                                            for i, (n, s) in enumerate(PARAMS[:6])])
+        self.transform = transform
+        self.tower = t = tower(B, self.device)
+        self.pull_segs = g.make_segs([(tid, 0, None, None, v) for tid, v in zip(tids, _split(self.flat, shapes))])
+        self.push_dense_segs = g.make_segs([(tid, 0, None, None, v)
+                                            for tid, v in zip(tids, _split(t.grads, shapes[:6]))])
         out = t.outputs()
-        self.push_rows_segs = g.make_segs([(tids[6 + k], GROUP_ROWS[TABLE_GROUP[k]], out["uniq"][k],
+        self.push_rows_segs = g.make_segs([(tids[6 + k], t.spec.group_rows[TABLE_GROUP[k]], out["uniq"][k],
                                             t.n_unique[k:k + 1], out["gsum"][k]) for k in range(5)])
         self._eval_tower = None  # evaluate()'s tower buffers (lazy)
 
-    # ------------------------------------------------------------------ the step
+    def _pull(self, numeric, strings, st):
+        check(self.group.lib.b200ps_pull_dense(self.group._h, *self.pull_segs, st))
+        if numeric is not None:
+            self.transform(numeric, strings, ids_out=self.ids)
+
     def _step(self, numeric, strings, labels, ids=None):
-        g, lib = self.group, self.group.lib
         with torch.cuda.device(self.device):
-            st = g._stream()
-            arr, n = self.pull_segs
-            check(lib.b200ps_pull_dense(g._h, arr, n, st))
-            if ids is None:
-                self.transform(numeric, strings, ids_out=self.ids)
-                ids = self.ids
-            self.tower.launch(ids, labels, self.flat, self.reference_reshape)
+            st = self.group._stream()
+            self._pull(numeric, strings, st)
+            self.tower.launch(self.ids if ids is None else ids, labels, self.flat, self.reference_reshape)
             self._push(st)
         return self.tower.loss.reshape(())
 
-    def step(self, numeric, strings, labels):
-        """One training step from raw rows; returns the loss (device scalar, not synchronised)."""
+    def evaluate(self, numeric, strings, labels, metrics):
+        """Forward only from raw rows: pull_dense -> the transform -> the tower -> metrics.update_evaluation_metrics(
+        {"logits": logits, "probs": sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of eval_metrics_fn()).
+        A tower without a forward form runs its training launch, whose gradients evaluate() discards -- into
+        buffers of its own, so the step's loss and gradients stay as they were.  Pushes nothing.  Returns the
+        logits [B] on the device (overwritten by the next evaluate)."""
         self._check_batch(numeric, strings, labels)
-        out = self._step(numeric, strings, labels)
-        self.steps += 1
-        return out
+        if self._eval_tower is None:
+            self._eval_tower = type(self.tower)(self.B, self.device)
+        t = self._eval_tower
+        with torch.cuda.device(self.device):
+            self._pull(numeric, strings, self.group._stream())
+            if t.spec.forward:
+                t.launch(self.ids, None, self.flat, self.reference_reshape, train=False)
+            else:
+                t.launch(self.ids, labels, self.flat, self.reference_reshape)
+            metrics.update_evaluation_metrics({"logits": t.logits, "probs": torch.sigmoid(t.logits)}, labels)
+        return t.logits
+
+    def check(self):
+        """Raise PSRangeError (a ValueError) if a step or evaluate since the last check read an id outside its
+        group; one device read per tower."""
+        if self._eval_tower is not None:
+            self._eval_tower.check_error()
+        self.tower.check_error()
+
+
+class CensusWideDeepEngine(WideDeepEngine):
+    """One async worker of the census wide & deep model on the parameter-server step (WideDeepEngine), from raw
+    Adult rows through census_transform.
+
+    group: an async PSGroup, as AsyncEngine takes it.  register=True registers the eleven parameters and sets their
+    initial values first-writer-wins (as PushModel does); register=False attaches to a group.clone_view() of a
+    group where another engine registered them, for another worker thread.  lr_schedule: a schedule to install, as
+    AsyncEngine.set_lr_schedule does.  There is no forward-only census kernel: evaluate() runs the training launch
+    into buffers of its own."""
+
+    def __init__(self, group, batch, lr, reference_reshape=False, seed=0, register=True, lr_schedule=None):
+        super().__init__(group, batch, lr, register, lr_schedule)
+        self.reference_reshape = bool(reference_reshape)
+        self._setup([n for n, _ in PARAMS], [s for _, s in PARAMS], initial_params, seed,
+                    census_transform(torch.int32, device=self.device), CensusTowerCall, register)
+        self.views = flat_views(self.flat)
 
     def step_ids(self, ids, labels):
         """One training step from the ids census_transform(torch.int32) gives: int32 [12, B]."""
@@ -230,48 +301,16 @@ class CensusWideDeepEngine(AsyncEngine):
         self.steps += 1
         return out
 
-    def evaluate(self, numeric, strings, labels, metrics):
-        """Forward only from raw rows: pull_dense -> census_transform -> the tower -> metrics.update_evaluation_metrics(
-        {"logits": logits, "probs": sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of eval_metrics_fn()).
-        There is no forward-only census kernel: the tower launch also computes the gradients, which evaluate()
-        discards -- into buffers of its own, so the step's loss and gradients stay as they were -- and pushes
-        nothing.  Returns the logits [B] on the device (overwritten by the next evaluate)."""
-        self._check_batch(numeric, strings, labels)
-        if self._eval_tower is None:
-            self._eval_tower = CensusTowerCall(self.B, self.device)
-        g = self.group
-        with torch.cuda.device(self.device):
-            arr, n = self.pull_segs
-            check(g.lib.b200ps_pull_dense(g._h, arr, n, g._stream()))
-            self.transform(numeric, strings, ids_out=self.ids)
-            self._eval_tower.launch(self.ids, labels, self.flat, self.reference_reshape)
-            logits = self._eval_tower.logits
-            metrics.update_evaluation_metrics({"logits": logits, "probs": torch.sigmoid(logits)}, labels)
-        return logits
 
-    def check(self):
-        """Raise PSRangeError (a ValueError) if a step or evaluate since the last check read an id outside its
-        group (it used row 0 for it); one device read per tower."""
-        if self._eval_tower is not None:
-            self._eval_tower.check_error()
-        self.tower.check_error()
+class WideDeepTwin(torch.nn.Module):
+    """What the census-style models' torch twins share: the MLP (three torch Linear layers, with their optimizer),
+    the loss and the tower over pooled lookups.  wide, deep: the subclass's wide and deep tables."""
 
-
-class CensusWideDeep(torch.nn.Module):
-    """The same model as a torch module for the drop-in ParameterServerTrainer: the tables are
-    elasticdl_b200.layers.Embedding layers (row-sparse PS tables; only the rows of the batch are pulled and
-    updated), the MLP is three torch Linear layers, both reshape modes.  forward((numeric, strings)) runs
-    census_transform and sums each group's four lookups."""
-
-    def __init__(self, lr, reference_reshape=False, optimizer="sgd"):
+    def __init__(self, wide, deep, lr, reference_reshape, optimizer):
         super().__init__()
-        from elasticdl_b200.layers import Embedding
-
         self.reference_reshape = bool(reference_reshape)
-        self.wide = torch.nn.ModuleList([Embedding(1, input_dim=r, embeddings_initializer="uniform", name=n.split("/")[0])
-                                         for n, r in zip(TABLE_NAMES[:2], GROUP_ROWS[:2])])
-        self.deep = torch.nn.ModuleList([Embedding(8, input_dim=r, embeddings_initializer="uniform", name=n.split("/")[0])
-                                         for n, r in zip(TABLE_NAMES[2:], GROUP_ROWS)])
+        self.wide = torch.nn.ModuleList(wide)
+        self.deep = torch.nn.ModuleList(deep)
         self.dense = torch.nn.ModuleList([torch.nn.Linear(24, 16), torch.nn.Linear(16, 8), torch.nn.Linear(8, 4)])
         self.transform = None  # built at the first forward (its vocabulary tables live on the device)
         opt = torch.optim.SGD if optimizer == "sgd" else torch.optim.Adam
@@ -281,11 +320,11 @@ class CensusWideDeep(torch.nn.Module):
 
     def load_mlp(self, flat):
         """Copy the MLP block of a flat buffer (Keras [in, out] kernels) into the Linear layers."""
-        v = flat_views(flat)
+        v = _split(flat, [s for _, s in PARAMS[:6]])
         with torch.no_grad():
             for i, lin in enumerate(self.dense):
-                lin.weight.copy_(v[MLP_NAMES[2 * i]].t())
-                lin.bias.copy_(v[MLP_NAMES[2 * i + 1]])
+                lin.weight.copy_(v[2 * i].t())
+                lin.bias.copy_(v[2 * i + 1])
 
     def tower(self, wide, deep):
         """wide [2, B] and deep [3, B, 8] pooled lookups -> logits [B]."""
@@ -294,6 +333,22 @@ class CensusWideDeep(torch.nn.Module):
         for lin in self.dense:
             x = lin(x)
         return wide.sum(0) + x.sum(1)
+
+
+class CensusWideDeep(WideDeepTwin):
+    """The same model as a torch module for the drop-in ParameterServerTrainer: the tables are
+    elasticdl_b200.layers.Embedding layers (row-sparse PS tables; only the rows of the batch are pulled and
+    updated), the MLP is three torch Linear layers, both reshape modes.  forward((numeric, strings)) runs
+    census_transform and sums each group's four lookups."""
+
+    def __init__(self, lr, reference_reshape=False, optimizer="sgd"):
+        from elasticdl_b200.layers import Embedding
+
+        wide = [Embedding(1, input_dim=r, embeddings_initializer="uniform", name=n.split("/")[0])
+                for n, r in zip(TABLE_NAMES[:2], GROUP_ROWS[:2])]
+        deep = [Embedding(8, input_dim=r, embeddings_initializer="uniform", name=n.split("/")[0])
+                for n, r in zip(TABLE_NAMES[2:], GROUP_ROWS)]
+        super().__init__(wide, deep, lr, reference_reshape, optimizer)
 
     def forward(self, features):
         numeric, strings = features

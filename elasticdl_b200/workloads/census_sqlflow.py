@@ -15,16 +15,12 @@ embedding_weights, the column name of concatenated_categorical_column being its 
 "_C_", feature_column.py:141-147) and not verified here.  Every table is under 2 MB, so the reference keeps it a
 dense parameter; here each is one dense PS parameter whose batch rows are pushed with b200ps_push_rows.
 """
-import ctypes
-
 import numpy as np
 import torch
 
-from elasticdl_b200 import _lib
-from elasticdl_b200._lib import CsqlArgs, check
-from elasticdl_b200.common.hash_utils import string_to_id
-from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor
-from elasticdl_b200.workloads.census_sqlflow_features import GROUP_DIMS, STRING_WIDTH, transform, _check_variant
+from elasticdl_b200._lib import CsqlArgs
+from elasticdl_b200.workloads.census import TABLE_DIM, TABLE_GROUP, TowerCall, TowerSpec, WideDeepEngine, WideDeepTwin
+from elasticdl_b200.workloads.census_sqlflow_features import GROUP_DIMS, transform, _check_variant
 
 # model file -> (id rule, reference_reshape)
 MODELS = {
@@ -48,8 +44,6 @@ TABLE_NAMES = {
     "fc": ["dense_features%s/%s_embedding/embedding_weights:0" % ("_%d" % k if k else "", FC_COLUMNS[g])
            for k, g in enumerate((0, 1, 0, 1, 2))],
 }
-TABLE_GROUP = (0, 1, 0, 1, 2)
-TABLE_DIM = (1, 1, 8, 8, 8)
 N_PARAMS, N_MLP = 2376, 572
 UNIQ_OFF = (0, 27, 100, 127, 200)
 N_UNIQ = 313
@@ -116,69 +110,14 @@ def callbacks():
     return [LearningRateScheduler(PiecewiseConstantDecay([4999, 11999], [3e-4, 2e-4, 1e-4]))]
 
 
-class CsqlTowerCall:
+SPEC = TowerSpec("b200_csql", CsqlArgs, GROUP_DIMS, UNIQ_OFF, N_UNIQ, GSUM_OFF, N_GSUM, N_PARAMS, N_MLP,
+                 "census_sqlflow ids outside [-1, rows of their group) %s were read as absent" % (GROUP_DIMS,), True)
+
+
+class CsqlTowerCall(TowerCall):
     """The tower's output buffers and workspace for batch B on `device`, and one launch over them."""
 
-    def __init__(self, B, device):
-        self.B = int(B)
-        if self.B < 1:
-            raise ValueError("batch size must be >= 1, not %d" % self.B)
-        self.device = torch.device(device)
-        self.lib = _lib.lib()
-        f32 = dict(dtype=torch.float32, device=self.device)
-        self.loss = torch.zeros(1, **f32)
-        self.logits = torch.zeros(self.B, **f32)
-        self.grads = torch.zeros(N_MLP, **f32)
-        self.uniq = torch.zeros(N_UNIQ, dtype=torch.int64, device=self.device)
-        self.n_unique = torch.zeros(5, dtype=torch.int32, device=self.device)
-        self.gsum = torch.zeros(N_GSUM, **f32)
-        self.error = torch.zeros(1, dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            nbytes = self.lib.b200_csql_workspace_bytes(self.B)
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        a = CsqlArgs()
-        a.B = self.B
-        a.loss, a.logits, a.grads = self.loss.data_ptr(), self.logits.data_ptr(), self.grads.data_ptr()
-        a.uniq, a.n_unique, a.gsum = self.uniq.data_ptr(), self.n_unique.data_ptr(), self.gsum.data_ptr()
-        a.error, a.workspace, a.workspace_bytes = self.error.data_ptr(), self.workspace.data_ptr(), nbytes
-        self.args = a
-
-    def check_inputs(self, ids, labels, flat):
-        check_tensor(ids, "ids", torch.int32, (12, self.B), self.device)
-        if labels is not None:
-            check_tensor(labels, "labels", torch.float32, (self.B,), self.device)
-        check_tensor(flat, "params", torch.float32, (N_PARAMS,), self.device)
-
-    def launch(self, ids, labels, flat, reference_reshape, train=True):
-        """One tower launch (train=False: the forward form, logits only) on the current stream (no checks, no host
-        read)."""
-        a = self.args
-        a.ids, a.params = ids.data_ptr(), flat.data_ptr()
-        a.labels = labels.data_ptr() if labels is not None else None
-        a.reference_reshape = 1 if reference_reshape else 0
-        fn = self.lib.b200_csql_tower if train else self.lib.b200_csql_forward
-        with torch.cuda.device(self.device):
-            rc = fn(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check_call(rc, fn.__name__, self.lib.b200_csql_last_error)
-
-    def check_error(self):
-        """Raise PSRangeError (a ValueError) if a launch since the last check read an id outside [-1, rows of its
-        group), and clear the count.  Reads one int from the device."""
-        n = int(self.error.item())
-        if n:
-            self.error.zero_()
-            raise _lib.PSRangeError(_lib.ERANGE, "%d census_sqlflow ids outside [-1, rows of their group) %s were "
-                                                 "read as absent" % (n, GROUP_DIMS))
-
-    def outputs(self):
-        """{loss, logits, grads, uniq [5], n_unique [5], gsum [5 segments: [rows, dim]]} (views of the buffers)."""
-        out = {"loss": self.loss.reshape(()), "logits": self.logits, "grads": self.grads, "n_unique": self.n_unique,
-               "uniq": [], "gsum": []}
-        for t in range(5):
-            rows = GROUP_DIMS[TABLE_GROUP[t]]
-            out["uniq"].append(self.uniq[UNIQ_OFF[t]:UNIQ_OFF[t] + rows])
-            out["gsum"].append(self.gsum[GSUM_OFF[t]:GSUM_OFF[t] + rows * TABLE_DIM[t]].view(rows, TABLE_DIM[t]))
-        return out
+    spec = SPEC
 
 
 def census_sqlflow_tower(ids, labels, flat, reference_reshape=False, train=True):
@@ -193,85 +132,22 @@ def census_sqlflow_tower(ids, labels, flat, reference_reshape=False, train=True)
     return call.outputs()
 
 
-class CensusSqlflowEngine(AsyncEngine):
-    """One async worker of a census_model_sqlflow wide & deep model on the parameter-server step.
+class CensusSqlflowEngine(WideDeepEngine):
+    """One async worker of a census_model_sqlflow wide & deep model on the parameter-server step (census.
+    WideDeepEngine), from raw rows through the feature transform of the model's id rule.
 
     group: an async PSGroup, as AsyncEngine takes it.  model: a MODELS name, which sets the id rule and the reshape
     mode.  register=True registers the eleven parameters under the model's names and sets their initial values
     first-writer-wins (as PushModel does); register=False attaches to a group.clone_view() of a group where
-    another engine registered them, for another worker thread.
-    step(numeric float32 [4, B], strings uint8 [8, B, 32], labels float32 [B]) runs pull_dense (into the flat
-    buffer) -> the feature transform -> the tower -> push_begin -> push_dense (MLP) -> push_rows (the five tables'
-    touched rows, counts on the device) -> push_end, with no host read, and returns the loss on the device.
-    capture() / replay() run the same step as one CUDA graph over static inputs.  lr_schedule: a schedule to
-    install, as AsyncEngine.set_lr_schedule does (callbacks()[0].schedule is the zoo's)."""
+    another engine registered them, for another worker thread.  lr_schedule: a schedule to install, as
+    AsyncEngine.set_lr_schedule does (callbacks()[0].schedule is the zoo's).  evaluate() runs the tower's forward
+    form."""
 
     def __init__(self, group, model, batch, lr, seed=0, register=True, lr_schedule=None):
         self.variant, self.reference_reshape = model_of(model)
         super().__init__(group, batch, lr, register, lr_schedule)
-        g, B = self.group, self.B
-        self.inputs = [("numeric", torch.float32, (4, B)), ("strings", torch.uint8, (8, B, STRING_WIDTH)),
-                       ("labels", torch.float32, (B,))]
-        self.names = param_names(self.variant)
-        self.owner = {n: string_to_id(n, g.n_shards) for n in self.names}
-        if register:
-            for n, s in zip(self.names, SHAPES):
-                g.register_dense(n, s, self.owner[n])
-            g.commit()
-            g.init_dense(zip(self.names, flat_views(initial_params(seed, self.device))))
-        tids = [g.lookup(n)[0] for n in self.names]  # PSNotFound when no engine registered them
-        self.flat = torch.zeros(N_PARAMS, dtype=torch.float32, device=self.device)
-        views = flat_views(self.flat)
-        self.ids = torch.zeros((12, B), dtype=torch.int32, device=self.device)
-        self.transform = transform(self.variant, device=self.device)
-        self.tower = t = CsqlTowerCall(B, self.device)
-        self.pull_segs = g.make_segs([(tid, 0, None, None, v) for tid, v in zip(tids, views)])
-        self.push_dense_segs = g.make_segs([(tids[i], 0, None, None, v) for i, v in enumerate(flat_views(t.grads))])
-        out = t.outputs()
-        self.push_rows_segs = g.make_segs([(tids[6 + k], GROUP_DIMS[TABLE_GROUP[k]], out["uniq"][k],
-                                            t.n_unique[k:k + 1], out["gsum"][k]) for k in range(5)])
-        self._eval_tower = None  # evaluate()'s logits buffer (lazy)
-
-    def _pull(self, numeric, strings, st):
-        check(self.group.lib.b200ps_pull_dense(self.group._h, *self.pull_segs, st))
-        self.transform(numeric, strings, ids_out=self.ids)
-
-    def _step(self, numeric, strings, labels):
-        with torch.cuda.device(self.device):
-            st = self.group._stream()
-            self._pull(numeric, strings, st)
-            self.tower.launch(self.ids, labels, self.flat, self.reference_reshape)
-            self._push(st)
-        return self.tower.loss.reshape(())
-
-    def step(self, numeric, strings, labels):
-        """One training step from raw rows; returns the loss (device scalar, not synchronised)."""
-        self._check_batch(numeric, strings, labels)
-        out = self._step(numeric, strings, labels)
-        self.steps += 1
-        return out
-
-    def evaluate(self, numeric, strings, labels, metrics):
-        """The forward only: pull_dense -> the transform -> the tower's forward form -> metrics.update_evaluation_
-        metrics({"logits": logits, "probs": sigmoid(logits)}, labels) (an EvaluationMetrics, e.g. of
-        eval_metrics_fn()).  Pushes nothing.  Returns the logits [B] on the device (overwritten by the next
-        evaluate)."""
-        self._check_batch(numeric, strings, labels)
-        if self._eval_tower is None:
-            self._eval_tower = CsqlTowerCall(self.B, self.device)
-        with torch.cuda.device(self.device):
-            self._pull(numeric, strings, self.group._stream())
-            self._eval_tower.launch(self.ids, None, self.flat, self.reference_reshape, train=False)
-            logits = self._eval_tower.logits
-            metrics.update_evaluation_metrics({"logits": logits, "probs": torch.sigmoid(logits)}, labels)
-        return logits
-
-    def check(self):
-        """Raise PSRangeError (a ValueError) if a step or evaluate since the last check read an id outside its
-        group (read as absent); one device read per tower."""
-        if self._eval_tower is not None:
-            self._eval_tower.check_error()
-        self.tower.check_error()
+        self._setup(param_names(self.variant), SHAPES, initial_params, seed,
+                    transform(self.variant, device=self.device), CsqlTowerCall, register)
 
 
 def sparse_group_ids(ids, g):
@@ -284,39 +160,24 @@ def sparse_group_ids(ids, g):
     return torch.sparse_coo_tensor(torch.stack([rows, cols]), vals, (B, 4))
 
 
-class CensusSqlflowWideDeep(torch.nn.Module):
+class CensusSqlflowWideDeep(WideDeepTwin):
     """The same model as a torch module for the drop-in ParameterServerTrainer: the tables are
     elasticdl_b200.layers.Embedding layers with combiner="mean" over sparse ids (row-sparse PS tables under the
     model's names; safe_embedding_lookup_sparse prunes the absent ids and zeroes an empty group), the MLP is three
     torch Linear layers.  forward((numeric, strings)) runs the model's feature transform."""
 
     def __init__(self, model, lr, optimizer="sgd"):
-        super().__init__()
         from elasticdl_b200.layers import Embedding
 
-        self.variant, self.reference_reshape = model_of(model)
+        variant, reference_reshape = model_of(model)
         tables = []
-        for n, g, d in zip(TABLE_NAMES[self.variant], TABLE_GROUP, TABLE_DIM):
+        for n, g, d in zip(TABLE_NAMES[variant], TABLE_GROUP, TABLE_DIM):
             e = Embedding(d, input_dim=GROUP_DIMS[g], embeddings_initializer="uniform", combiner="mean",
                           name=n.rsplit("/", 1)[0])
             e.set_embedding_weight_name(n)
             tables.append(e)
-        self.wide = torch.nn.ModuleList(tables[:2])
-        self.deep = torch.nn.ModuleList(tables[2:])
-        self.dense = torch.nn.ModuleList([torch.nn.Linear(24, 16), torch.nn.Linear(16, 8), torch.nn.Linear(8, 4)])
-        self.transform = None  # built at the first forward (its vocabulary tables live on the device)
-        opt = torch.optim.SGD if optimizer == "sgd" else torch.optim.Adam
-        self.optimizer = opt(self.dense.parameters(), lr=lr)
-        bce = torch.nn.BCEWithLogitsLoss()
-        self.loss = lambda labels, logits: bce(logits, labels)
-
-    def load_mlp(self, flat):
-        """Copy the MLP block of a flat buffer (Keras [in, out] kernels) into the Linear layers."""
-        v = flat_views(flat)
-        with torch.no_grad():
-            for i, lin in enumerate(self.dense):
-                lin.weight.copy_(v[2 * i].t())
-                lin.bias.copy_(v[2 * i + 1])
+        super().__init__(tables[:2], tables[2:], lr, reference_reshape, optimizer)
+        self.variant = variant
 
     def forward(self, features):
         numeric, strings = features
@@ -324,10 +185,6 @@ class CensusSqlflowWideDeep(torch.nn.Module):
             self.transform = transform(self.variant, device=numeric.device)
         ids, _ = self.transform(numeric, strings)
         sp = [sparse_group_ids(ids, g) for g in range(3)]
-        wide = self.wide[0](sp[0])[:, 0] + self.wide[1](sp[1])[:, 0]
+        wide = torch.stack([self.wide[g](sp[g])[:, 0] for g in range(2)])
         deep = torch.stack([self.deep[g](sp[g]) for g in range(3)])  # [3, B, 8]
-        B = deep.shape[1]
-        x = deep.reshape(B, 24) if self.reference_reshape else deep.permute(1, 0, 2).reshape(B, 24)
-        for lin in self.dense:
-            x = lin(x)
-        return wide + x.sum(1)
+        return self.tower(wide, deep)

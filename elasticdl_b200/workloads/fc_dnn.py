@@ -393,13 +393,6 @@ class FeatureColumnDNNEngine(AsyncEngine):
             self._push(st)
         return self.tower.loss.reshape(())
 
-    def step(self, numeric, strings, labels):
-        """One training step from raw rows; returns the loss (device scalar, not synchronised)."""
-        self._check_batch(numeric, strings, labels)
-        out = self._step(numeric, strings, labels)
-        self.steps += 1
-        return out
-
     def evaluate(self, numeric, strings, labels, metrics):
         """The forward only: the step's pulls (rows are created by the pull, as the reference's evaluation
         lookups create them), the tower's forward form, then metrics.update_evaluation_metrics({"logits": logits,
