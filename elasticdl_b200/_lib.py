@@ -109,6 +109,15 @@ class FcDnnArgs(ctypes.Structure):  # b200_fc_dnn_args_t
     ]
 
 
+class DeepctrWdlArgs(ctypes.Structure):  # b200_deepctr_wdl_args_t (include/b200_deepctr_wdl.h)
+    _fields_ = [
+        ("B", ctypes.c_int64), ("ids", ctypes.c_void_p), ("dense", ctypes.c_void_p), ("labels", ctypes.c_void_p),
+        ("params", ctypes.c_void_p), ("loss", ctypes.c_void_p), ("logits", ctypes.c_void_p),
+        ("grads", ctypes.c_void_p), ("error", ctypes.c_void_p), ("workspace", ctypes.c_void_p),
+        ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 LR_MAX_BOUNDARIES = 32  # B200PS_LR_MAX_BOUNDARIES
 LR_PIECEWISE, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_POLYNOMIAL = 1, 2, 3, 4
 
@@ -294,6 +303,14 @@ FC_DNN_SYMBOLS = {
     "b200_fc_dnn_last_error": (ctypes.c_char_p, []),
     "b200_fc_dnn_launch_count": (_i64, []),
 }
+# include/b200_deepctr_wdl.h
+DEEPCTR_WDL_SYMBOLS = {
+    "b200_deepctr_wdl_workspace_bytes": (_sz, [_i64]),
+    "b200_deepctr_wdl_tower": (_i, [ctypes.POINTER(DeepctrWdlArgs), _vp]),
+    "b200_deepctr_wdl_forward": (_i, [ctypes.POINTER(DeepctrWdlArgs), _vp]),
+    "b200_deepctr_wdl_last_error": (ctypes.c_char_p, []),
+    "b200_deepctr_wdl_launch_count": (_i64, []),
+}
 # include/b200_metrics.h
 METRICS_MAX_THRESHOLDS = 16384  # B200_METRICS_MAX_THRESHOLDS
 METRICS_SYMBOLS = {
@@ -314,7 +331,8 @@ def lib():
             path = _build.build()
         handle = ctypes.CDLL(path)
         for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items())\
-                + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()) + list(CSQL_SYMBOLS.items()):
+                + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()) + list(CSQL_SYMBOLS.items())\
+                + list(DEEPCTR_WDL_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args

@@ -22,6 +22,7 @@ struct Census {};    // b200_census.h
 struct CensusSqlflow {};  // b200_census_sqlflow.h
 struct Frappe {};    // b200_frappe.h
 struct FcDnn {};     // b200_fc_dnn.h
+struct DeepctrWdl {};  // b200_deepctr_wdl.h
 struct Metrics {};   // b200_metrics.h
 
 // What an exported *_launch_count reads; entry points of several host threads add to it.
