@@ -118,6 +118,9 @@ class DeepctrWdlArgs(ctypes.Structure):  # b200_deepctr_wdl_args_t (include/b200
     ]
 
 
+DeepctrDeepfmArgs = DeepctrWdlArgs  # b200_deepctr_deepfm_args_t (include/b200_deepctr_deepfm.h) has the same fields
+
+
 LR_MAX_BOUNDARIES = 32  # B200PS_LR_MAX_BOUNDARIES
 LR_PIECEWISE, LR_EXPONENTIAL, LR_INVERSE_TIME, LR_POLYNOMIAL = 1, 2, 3, 4
 
@@ -311,6 +314,14 @@ DEEPCTR_WDL_SYMBOLS = {
     "b200_deepctr_wdl_last_error": (ctypes.c_char_p, []),
     "b200_deepctr_wdl_launch_count": (_i64, []),
 }
+# include/b200_deepctr_deepfm.h
+DEEPCTR_DEEPFM_SYMBOLS = {
+    "b200_deepctr_deepfm_workspace_bytes": (_sz, [_i64]),
+    "b200_deepctr_deepfm_tower": (_i, [ctypes.POINTER(DeepctrDeepfmArgs), _vp]),
+    "b200_deepctr_deepfm_forward": (_i, [ctypes.POINTER(DeepctrDeepfmArgs), _vp]),
+    "b200_deepctr_deepfm_last_error": (ctypes.c_char_p, []),
+    "b200_deepctr_deepfm_launch_count": (_i64, []),
+}
 # include/b200_metrics.h
 METRICS_MAX_THRESHOLDS = 16384  # B200_METRICS_MAX_THRESHOLDS
 METRICS_SYMBOLS = {
@@ -332,7 +343,7 @@ def lib():
         handle = ctypes.CDLL(path)
         for name, (res, args) in list(SYMBOLS.items()) + list(CENSUS_SYMBOLS.items()) + list(FRAPPE_SYMBOLS.items())\
                 + list(METRICS_SYMBOLS.items()) + list(FC_DNN_SYMBOLS.items()) + list(CSQL_SYMBOLS.items())\
-                + list(DEEPCTR_WDL_SYMBOLS.items()):
+                + list(DEEPCTR_WDL_SYMBOLS.items()) + list(DEEPCTR_DEEPFM_SYMBOLS.items()):
             fn = getattr(handle, name)  # AttributeError if the ABI drifted: fail loudly
             fn.restype = res
             fn.argtypes = args

@@ -7,9 +7,9 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(CSRC, "libb200ps.so")
 SOURCES = ["b200ps.cu", "deepfm_tower.cu", "deepfm_tower_mma.cu", "deepfm_tower2.cu", "dcn_tower.cu", "xdeepfm_cin.cu",
            "feature_ids.cu", "census_tower.cu", "frappe_tower.cu", "eval_metrics.cu", "fc_dnn_tower.cu",
-           "census_sqlflow_tower.cu", "deepctr_wdl_tower.cu"]
+           "census_sqlflow_tower.cu", "deepctr_wdl_tower.cu", "deepctr_deepfm_tower.cu"]
 HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "ps_unique.cuh", "deepfm_common.cuh",
-           "tile_tower.cuh", "mma_tf32.cuh", "xdeepfm.cuh", "launch.cuh", "census_tower.cuh",
+           "tile_tower.cuh", "mma_tf32.cuh", "xdeepfm.cuh", "launch.cuh", "census_tower.cuh", "deepctr_dnn.cuh",
            os.path.join("..", "..", "include", "b200ps.h"),
            os.path.join("..", "..", "include", "b200_deepfm.h"),
            os.path.join("..", "..", "include", "b200_features.h"),
@@ -18,7 +18,8 @@ HEADERS = ["ps_kernels.cuh", "ps_types.cuh", "ps_exchange.cuh", "ps_flat.cuh", "
            os.path.join("..", "..", "include", "b200_metrics.h"),
            os.path.join("..", "..", "include", "b200_fc_dnn.h"),
            os.path.join("..", "..", "include", "b200_census_sqlflow.h"),
-           os.path.join("..", "..", "include", "b200_deepctr_wdl.h")]
+           os.path.join("..", "..", "include", "b200_deepctr_wdl.h"),
+           os.path.join("..", "..", "include", "b200_deepctr_deepfm.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",

@@ -1,5 +1,6 @@
 // deepctr WDL tower (include/b200_deepctr_wdl.h): one training step of deepctr's WDL on Criteo-shaped rows, from
-// hashed ids to the loss and the dense gradient of all 61 parameters, in five launches with no float atomics.
+// hashed ids to the loss and the dense gradient of all 61 parameters, in five launches with no float atomics.  The
+// sort and the DNN are deepctr_dnn.cuh's, shared with the DeepFM estimator tower.
 //
 //   k_deepctr_wdl_hist     grid (NCH, 26): each CTA counts its sample chunk's ids per row of one table.
 //   k_deepctr_wdl_scatter  grid (NCH, 26): a stable counting sort of each table's occurrences by row -- each
@@ -23,20 +24,35 @@
 #include <string>
 
 #include "../../include/b200_deepctr_wdl.h"
+#include "deepctr_dnn.cuh"
 #include "launch.cuh"
-#include "mma_tf32.cuh"
 
 namespace {
 
 using E = entry::Entry<entry::DeepctrWdl>;
 entry::LaunchCount g_launches{0};
 
-constexpr int NF = B200_DEEPCTR_WDL_FIELDS, ND = B200_DEEPCTR_WDL_DENSE, ROWS = B200_DEEPCTR_WDL_ROWS;
-constexpr int DIM = B200_DEEPCTR_WDL_DIM;
-constexpr int NS = NF * DIM;     // 104 sparse columns of x
-constexpr int F = NS + ND;       // 117
-constexpr int N1 = 256, N2 = 128, N3 = 64;
-constexpr int TILE = B200_DEEPCTR_WDL_TILE, THREADS = 256, WARPS = THREADS / 32;
+using deepctr::DIM;
+using deepctr::F;
+using deepctr::N1;
+using deepctr::N2;
+using deepctr::N3;
+using deepctr::NCH;
+using deepctr::ND;
+using deepctr::NF;
+using deepctr::NS;
+using deepctr::S1;
+using deepctr::S2;
+using deepctr::S3;
+using deepctr::SORT_THREADS;
+using deepctr::THREADS;
+using deepctr::TILE;
+using deepctr::WARPS;
+using deepctr::XS;
+constexpr int ROWS = B200_DEEPCTR_WDL_ROWS;
+static_assert(NF == B200_DEEPCTR_WDL_FIELDS && ND == B200_DEEPCTR_WDL_DENSE && DIM == B200_DEEPCTR_WDL_DIM &&
+                  TILE == B200_DEEPCTR_WDL_TILE,
+              "shapes of include/b200_deepctr_wdl.h");
 constexpr float LAMBDA = 1e-5f;  // l2_reg_embedding = l2_reg_linear = 1e-5
 
 // flat offsets (floats)
@@ -45,19 +61,17 @@ constexpr int64_t O_DEEP = 0, O_LIN = (int64_t)NF * ROWS * DIM, O_DNN = O_LIN + 
 constexpr int P_WLIN = 0, P_W0 = P_WLIN + ND, P_B0 = P_W0 + F * N1, P_W1 = P_B0 + N1, P_B1 = P_W1 + N1 * N2;
 constexpr int P_W2 = P_B1 + N2, P_B2 = P_W2 + N2 * N3, P_WD = P_B2 + N3, P_GB = P_WD + N3, N_DNN = P_GB + 1;
 constexpr int P_BCE = N_DNN, Q = N_DNN + 1;
+struct Dnn {  // the DNN layout in the dense block and the partial
+  static constexpr int W0 = P_W0, B0 = P_B0, W1 = P_W1, B1 = P_B1, W2 = P_W2, B2 = P_B2, WD = P_WD;
+};
 static_assert(O_DNN + N_DNN == B200_DEEPCTR_WDL_PARAMS, "flat layout of include/b200_deepctr_wdl.h");
 static_assert(O_DNN + P_W0 == 1300013 && O_DNN + P_B2 == 1371309 && O_DNN + P_GB == 1371437, "flat offsets");
 
-// shared memory of the tower (floats): x [TILE][XS] (columns F .. XS-1 zero) | h1 | h2 | h3 | dz | lin / loss
-constexpr int XS = 132, S1 = N1 + 4, S2 = N2 + 4, S3 = N3 + 4;  // row strides = 4 mod 32: conflict-free rows
+// shared memory of the tower (floats): x | h1 | h2 | h3 (deepctr_dnn.cuh) | dz | lin / loss
 constexpr int SM_H1 = TILE * XS, SM_H2 = SM_H1 + TILE * S1, SM_H3 = SM_H2 + TILE * S2, SM_DZ = SM_H3 + TILE * S3;
 constexpr int SM_LS = SM_DZ + TILE, SMEM_FLOATS = SM_LS + TILE;
 constexpr int SMEM_BYTES = SMEM_FLOATS * 4;
-static_assert(XS >= 128 && XS % 4 == 0, "x is read as 128 columns by dW0 = x^T dh1");
 
-// the sort: NCH chunks of samples per table
-constexpr int NCH = 4, SORT_THREADS = 1024;
-constexpr int ROWS_PER_THREAD = (ROWS + SORT_THREADS - 1) / SORT_THREADS;
 constexpr int TABLE_BLOCKS_PER_SM = 4;
 
 struct Work {  // the workspace, carved by carve()
@@ -92,137 +106,24 @@ __host__ __device__ inline size_t carve(void* base, int64_t B, int grid, int tbl
   return o;
 }
 
-__device__ __forceinline__ int row_of(int id) { return (unsigned)id < (unsigned)ROWS ? id : 0; }
-
-// ---- the sort
-__device__ __forceinline__ void chunk_of(int64_t B, int c, int64_t* b0, int64_t* b1) {
-  const int64_t ch = (B + NCH - 1) / NCH;
-  *b0 = c * ch < B ? c * ch : B;
-  *b1 = *b0 + ch < B ? *b0 + ch : B;
-}
+struct Rows {  // an id outside [0, 10000) is read as row 0
+  static constexpr bool kSkips = false;
+  __device__ __forceinline__ static int row(int id) { return (unsigned)id < (unsigned)ROWS ? id : 0; }
+};
 
 __global__ void __launch_bounds__(SORT_THREADS) k_deepctr_wdl_hist(const int32_t* __restrict__ ids, int64_t B,
                                                                    int* __restrict__ counts) {
-  __shared__ int h[ROWS];
-  const int c = blockIdx.x, j = blockIdx.y, t = threadIdx.x;
-  int64_t b0, b1;
-  chunk_of(B, c, &b0, &b1);
-  for (int i = t; i < ROWS; i += SORT_THREADS) h[i] = 0;
-  __syncthreads();
-  for (int64_t b = b0 + t; b < b1; b += SORT_THREADS) atomicAdd(&h[row_of(__ldg(ids + j * B + b))], 1);
-  __syncthreads();
-  int* out = counts + ((size_t)j * NCH + c) * ROWS;
-  for (int i = t; i < ROWS; i += SORT_THREADS) out[i] = h[i];
+  deepctr::sort_hist<ROWS, Rows>(ids, B, counts);
 }
 
 __global__ void __launch_bounds__(SORT_THREADS) k_deepctr_wdl_scatter(const int32_t* __restrict__ ids, int64_t B,
                                                                       const int* __restrict__ counts,
                                                                       int* __restrict__ offsets,
                                                                       int* __restrict__ perm) {
-  __shared__ int cur[ROWS];
-  __shared__ int wsum[32];
-  const int c = blockIdx.x, j = blockIdx.y, t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  // row r's first position in perm[j]: the rows before it (an exclusive scan of the totals over rows), then the
-  // earlier chunks' occurrences of r
-  const int r0 = t * ROWS_PER_THREAD;
-  const int* cj = counts + (size_t)j * NCH * ROWS;
-  auto total = [&](int r, int upto) {  // occurrences of row r in chunks [0, upto)
-    int s = 0;
-    for (int cc = 0; cc < upto; ++cc) s += __ldg(cj + (size_t)cc * ROWS + r);
-    return s;
-  };
-  int mine = 0;
-  for (int r = r0; r < r0 + ROWS_PER_THREAD && r < ROWS; ++r) mine += total(r, NCH);
-  int inc = mine;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc += v;
-  }
-  if (lane == 31) wsum[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    int v = wsum[lane], s = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, s, d);
-      if (lane >= d) s += u;
-    }
-    wsum[lane] = s - v;
-  }
-  __syncthreads();
-  int start = wsum[warp] + inc - mine;
-  for (int r = r0; r < r0 + ROWS_PER_THREAD && r < ROWS; ++r) {
-    cur[r] = start + total(r, c);
-    if (c == 0) offsets[(size_t)j * (ROWS + 1) + r] = start;
-    start += total(r, NCH);
-  }
-  if (c == 0 && t == 0) offsets[(size_t)j * (ROWS + 1) + ROWS] = (int)B;
-  __syncthreads();
-  int64_t b0, b1;
-  chunk_of(B, c, &b0, &b1);
-  for (int64_t base = b0; base < b1; base += SORT_THREADS) {
-    const int64_t b = base + t;
-    const bool valid = b < b1;
-    const int key = valid ? row_of(__ldg(ids + j * B + b)) : -1;
-    const unsigned peers = __match_any_sync(0xffffffffu, key);
-    const int rank = __popc(peers & ((1u << lane) - 1u)), cnt = __popc(peers);
-    for (int w = 0; w < SORT_THREADS / 32; ++w) {  // the warps in order: a stable sort
-      if (warp == w) {
-        int pos = 0;
-        if (valid) pos = cur[key] + rank;
-        __syncwarp();
-        if (valid) {
-          if (rank == 0) cur[key] += cnt;
-          perm[(size_t)j * B + pos] = (int)b;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  deepctr::sort_scatter<ROWS, Rows>(ids, B, counts, offsets, perm);
 }
 
 // ---- the tower
-// C = A B over M x N (M a multiple of 64, N of 8), K a multiple of 8: each warp unit is 64 rows x 8 columns (four
-// m16n8k8 tiles sharing one B fragment); a(m, k), b(k, n) load the operands; epi(m, n, c) takes each result.
-template <class LA, class LB, class Epi>
-__device__ __forceinline__ void warp_gemm(int M, int N, int K, LA a, LB b, Epi epi) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gid = lane >> 2, tig = lane & 3;
-  const int nn = N / 8, units = (M / 64) * nn;
-  for (int u = warp; u < units; u += WARPS) {
-    const int m0 = (u / nn) * 64, n0 = (u % nn) * 8;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
-    for (int k0 = 0; k0 < K; k0 += 8) {
-      uint32_t bh[2], bl[2];
-      deepfm::split(b(k0 + tig, n0 + gid), bh[0], bl[0]);
-      deepfm::split(b(k0 + tig + 4, n0 + gid), bh[1], bl[1]);
-#pragma unroll
-      for (int mb = 0; mb < 4; ++mb) {
-        const int r = m0 + 16 * mb + gid;
-        uint32_t ah[4], al[4];
-        deepfm::split(a(r, k0 + tig), ah[0], al[0]);
-        deepfm::split(a(r + 8, k0 + tig), ah[1], al[1]);
-        deepfm::split(a(r, k0 + tig + 4), ah[2], al[2]);
-        deepfm::split(a(r + 8, k0 + tig + 4), ah[3], al[3]);
-        deepfm::mma3(acc[mb], ah, al, bh, bl);
-      }
-    }
-#pragma unroll
-    for (int mb = 0; mb < 4; ++mb) {
-      const int r = m0 + 16 * mb + gid, cc = n0 + 2 * tig;
-      epi(r, cc, acc[mb][0]);
-      epi(r, cc + 1, acc[mb][1]);
-      epi(r + 8, cc, acc[mb][2]);
-      epi(r + 8, cc + 1, acc[mb][3]);
-    }
-  }
-}
-
-// entry i of this CTA's partial: set on its first tile, added to after
-__device__ __forceinline__ void add_part(float* p, float v, bool first) { __stcg(p, first ? v : __ldcg(p) + v); }
-
 __global__ void __launch_bounds__(THREADS, 1) k_deepctr_wdl_tower(b200_deepctr_wdl_args_t a, Work w, int ntiles,
                                                                  int train) {
   extern __shared__ __align__(16) float sm[];
@@ -266,24 +167,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_deepctr_wdl_tower(b200_deepctr_w
     if (t < TILE) {
       float s = 0.f;
       if (t < n) {
-        for (int j = 0; j < NF; ++j) s += __ldg(P + O_LIN + (int64_t)j * ROWS + row_of(__ldg(a.ids + j * B + base + t)));
+        for (int j = 0; j < NF; ++j) s += __ldg(P + O_LIN + (int64_t)j * ROWS + Rows::row(__ldg(a.ids + j * B + base + t)));
         for (int i = 0; i < ND; ++i) s = fmaf(X[t * XS + NS + i], __ldg(D + P_WLIN + i), s);
       }
       ls[t] = s;
     }
-    // h1 = relu(x W0 + b0)
-    warp_gemm(64, N1, 120, [&](int m, int k) { return X[m * XS + k]; },
-              [&](int k, int c) { return k < F ? __ldg(D + P_W0 + k * N1 + c) : 0.f; },
-              [&](int m, int c, float v) { A1[m * S1 + c] = fmaxf(v + __ldg(D + P_B0 + c), 0.f); });
-    __syncthreads();
-    warp_gemm(64, N2, N1, [&](int m, int k) { return A1[m * S1 + k]; },
-              [&](int k, int c) { return __ldg(D + P_W1 + k * N2 + c); },
-              [&](int m, int c, float v) { A2[m * S2 + c] = fmaxf(v + __ldg(D + P_B1 + c), 0.f); });
-    __syncthreads();
-    warp_gemm(64, N3, N2, [&](int m, int k) { return A2[m * S2 + k]; },
-              [&](int k, int c) { return __ldg(D + P_W2 + k * N3 + c); },
-              [&](int m, int c, float v) { A3[m * S3 + c] = fmaxf(v + __ldg(D + P_B2 + c), 0.f); });
-    __syncthreads();
+    deepctr::dnn_forward<Dnn>(X, A1, A2, A3, D);
     // z, four threads per sample (16 units each, then a fixed shuffle tree); the loss and dz
     {
       const int r = t >> 2, q = t & 3;
@@ -322,74 +211,27 @@ __global__ void __launch_bounds__(THREADS, 1) k_deepctr_wdl_tower(b200_deepctr_w
       float s = 0.f;
       if (e < N3) {
         for (int r = 0; r < TILE; ++r) s = fmaf(A3[r * S3 + e], dzs[r], s);
-        add_part(mine + P_WD + e, s, first);
+        deepctr::add_part(mine + P_WD + e, s, first);
       } else if (e < N3 + ND) {
         for (int r = 0; r < TILE; ++r) s = fmaf(X[r * XS + NS + e - N3], dzs[r], s);
-        add_part(mine + P_WLIN + e - N3, s, first);
+        deepctr::add_part(mine + P_WLIN + e - N3, s, first);
       } else if (e == N3 + ND) {
         for (int r = 0; r < TILE; ++r) s += dzs[r];
-        add_part(mine + P_GB, s, first);
+        deepctr::add_part(mine + P_GB, s, first);
       } else {
         for (int r = 0; r < TILE; ++r) s += ls[r];
-        add_part(mine + P_BCE, s, first);
+        deepctr::add_part(mine + P_BCE, s, first);
       }
     }
     __syncthreads();
-    // dh3 = dz wd [h3 > 0], in place
-    for (int i = t; i < TILE * N3; i += THREADS) {
-      const int r = i / N3, c = i % N3;
-      A3[r * S3 + c] = A3[r * S3 + c] > 0.f ? dzs[r] * __ldg(D + P_WD + c) : 0.f;
-    }
-    __syncthreads();
-    if (t < N3) {
-      float s = 0.f;
-      for (int r = 0; r < TILE; ++r) s += A3[r * S3 + t];
-      add_part(mine + P_B2 + t, s, first);
-    }
-    // dW2 = h2^T dh3
-    warp_gemm(N2, N3, TILE, [&](int m, int k) { return A2[k * S2 + m]; }, [&](int k, int c) { return A3[k * S3 + c]; },
-              [&](int m, int c, float v) { add_part(mine + P_W2 + m * N3 + c, v, first); });
-    __syncthreads();
-    // dh2 = (dh3 W2^T) [h2 > 0], in place
-    warp_gemm(64, N2, N3, [&](int m, int k) { return A3[m * S3 + k]; },
-              [&](int k, int c) { return __ldg(D + P_W2 + c * N3 + k); },
-              [&](int m, int c, float v) { A2[m * S2 + c] = A2[m * S2 + c] > 0.f ? v : 0.f; });
-    __syncthreads();
-    if (t < N2) {
-      float s = 0.f;
-      for (int r = 0; r < TILE; ++r) s += A2[r * S2 + t];
-      add_part(mine + P_B1 + t, s, first);
-    }
-    // dW1 = h1^T dh2
-    warp_gemm(N1, N2, TILE, [&](int m, int k) { return A1[k * S1 + m]; }, [&](int k, int c) { return A2[k * S2 + c]; },
-              [&](int m, int c, float v) { add_part(mine + P_W1 + m * N2 + c, v, first); });
-    __syncthreads();
-    // dh1 = (dh2 W1^T) [h1 > 0], in place
-    warp_gemm(64, N1, N2, [&](int m, int k) { return A2[m * S2 + k]; },
-              [&](int k, int c) { return __ldg(D + P_W1 + c * N2 + k); },
-              [&](int m, int c, float v) { A1[m * S1 + c] = A1[m * S1 + c] > 0.f ? v : 0.f; });
-    __syncthreads();
-    {
-      float s = 0.f;  // THREADS == N1: thread t owns db0[t]
-      for (int r = 0; r < TILE; ++r) s += A1[r * S1 + t];
-      add_part(mine + P_B0 + t, s, first);
-    }
-    // dW0 = x^T dh1 (x's columns past F are zero and not stored)
-    warp_gemm(128, N1, TILE, [&](int m, int k) { return X[k * XS + m]; }, [&](int k, int c) { return A1[k * S1 + c]; },
-              [&](int m, int c, float v) {
-                if (m < F) add_part(mine + P_W0 + m * N1 + c, v, first);
-              });
-    // dx of the sparse columns = dh1 W0^T, and dz, per sample
-    warp_gemm(64, NS, N1, [&](int m, int k) { return A1[m * S1 + k]; },
-              [&](int k, int c) { return __ldg(D + P_W0 + c * N1 + k); },
-              [&](int m, int c, float v) {
-                if (m < n) __stcg(w.dx + (base + m) * NS + c, v);
-              });
+    // the DNN's weight gradients, and dx of the sparse columns per sample
+    deepctr::dnn_backward<Dnn>(X, A1, A2, A3, dzs, D, mine, first, [&](int m, int c, float v) {
+      if (m < n) __stcg(w.dx + (base + m) * NS + c, v);
+    });
     if (t < n) __stcg(w.dz + base + t, dzs[t]);
     __syncthreads();
   }
 }
-static_assert(THREADS == N1, "one thread per unit of h1 for db0");
 
 // one warp per (table, row): 2 lambda W + the row's occurrences in perm order, for the deep and the linear row
 __global__ void __launch_bounds__(THREADS) k_deepctr_wdl_tables(b200_deepctr_wdl_args_t a, Work w) {
@@ -450,14 +292,13 @@ __global__ void __launch_bounds__(THREADS) k_deepctr_wdl_reduce(b200_deepctr_wdl
                                                                 int tblocks) {
   const float* __restrict__ D = a.params + O_DNN;
   for (int i = blockIdx.x * THREADS + threadIdx.x; i < N_DNN; i += gridDim.x * THREADS) {
-    float s = 0.f;
-    for (int c = 0; c < grid; ++c) s += __ldcg(w.parts + (size_t)c * Q + i);
+    float s = deepctr::cta_order_sum(w.parts, Q, grid, i);
     if (i < P_W0) s = fmaf(2.f * LAMBDA, __ldg(D + i), s);
     a.grads[O_DNN + i] = s;
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    float bce = 0.f, sq = 0.f;
-    for (int c = 0; c < grid; ++c) bce += __ldcg(w.parts + (size_t)c * Q + P_BCE);
+    const float bce = deepctr::cta_order_sum(w.parts, Q, grid, P_BCE);
+    float sq = 0.f;
     for (int c = 0; c < tblocks; ++c) sq += __ldcg(w.tparts + c);
     for (int i = 0; i < ND; ++i) sq = fmaf(__ldg(D + P_WLIN + i), __ldg(D + P_WLIN + i), sq);
     *a.loss = bce / (float)a.B + LAMBDA * sq;

@@ -23,6 +23,7 @@ struct CensusSqlflow {};  // b200_census_sqlflow.h
 struct Frappe {};    // b200_frappe.h
 struct FcDnn {};     // b200_fc_dnn.h
 struct DeepctrWdl {};  // b200_deepctr_wdl.h
+struct DeepctrDeepfm {};  // b200_deepctr_deepfm.h
 struct Metrics {};   // b200_metrics.h
 
 // What an exported *_launch_count reads; entry points of several host threads add to it.

@@ -26,12 +26,7 @@ class AsyncEngine:
     `push_dense_segs` and `push_rows_segs`, and defines _step(*inputs), which ends in _push()."""
 
     def __init__(self, group, batch, lr, register, lr_schedule=None):
-        name = type(self).__name__
-        if not getattr(group, "use_async", True):
-            raise ValueError("%s trains async only: a sync-SGD group needs the drop-in trainer" % name)
-        if getattr(group, "lr_staleness_modulation", False):
-            raise ValueError("%s pushes without model versions: a group with lr_staleness_modulation needs the "
-                             "drop-in trainer" % name)
+        self._check_group(group)
         self.B = int(batch)
         if self.B < 1:
             raise ValueError("batch size must be >= 1, not %d" % self.B)
@@ -45,6 +40,15 @@ class AsyncEngine:
         self.lr_schedule = None
         if lr_schedule is not None:
             self.set_lr_schedule(lr_schedule)
+
+    def _check_group(self, group):
+        """ValueError for a group the engine cannot push to."""
+        name = type(self).__name__
+        if not getattr(group, "use_async", True):
+            raise ValueError("%s trains async only: a sync-SGD group needs the drop-in trainer" % name)
+        if getattr(group, "lr_staleness_modulation", False):
+            raise ValueError("%s pushes without model versions: a group with lr_staleness_modulation needs the "
+                             "drop-in trainer" % name)
 
     def _check_batch(self, *tensors):
         """Check a batch, one tensor per declared input, against the declaration."""
