@@ -1,11 +1,12 @@
-"""The Wide & Deep and DCN engines on the owner-computes exchange (torchrun, one rank per GPU; B200_SHARED_GPU=1 puts
+"""The Wide & Deep, DCN and xDeepFM engines on the owner-computes exchange (torchrun, one rank per GPU; B200_SHARED_GPU=1 puts
 every rank on cuda:0 as its own process).  For each model, every rank:
   - conditions its first batch on the known initial state (the engine's seeded rows and tower), so that no sample
     sits within rounding of a ReLU kink;
   - runs one eager step and, right after the tower, copies what the exchange pulled into bet_w / bet_d, the plan's
     dedup, the dense parameters and the tower's outputs;
   - checks the pulled rows against the initial rows and the tower's loss, logits, flat_grads and gsum_w / gsum_d
-    against the float64 reference on those rows (oracle/wide_deep_oracle.py, oracle/dcn_oracle.py);
+    against the float64 reference on those rows (oracle/wide_deep_oracle.py, oracle/dcn_oracle.py,
+    oracle/xdeepfm_oracle.py);
   - trains a few more steps, eagerly and from its CUDA graph, and the loss falls."""
 import os
 import sys
@@ -18,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from elasticdl_b200.ps import PSGroup  # noqa: E402
-from oracle import dcn_oracle, wide_deep_oracle  # noqa: E402
+from oracle import dcn_oracle, wide_deep_oracle, xdeepfm_oracle  # noqa: E402
 
 ADAM = ("Adam", "learning_rate=0.001;beta_1=0.9;beta_2=0.999;epsilon=1e-07;amsgrad=false;")
 ROWS = [11, 5000, 60000, 9, 300]
@@ -29,6 +30,8 @@ def _reference(model):
     """(reference(inputs...), oracle module) of a model."""
     if model == "dcn":
         return dcn_oracle.dcn_reference, dcn_oracle
+    if model == "xdeepfm":
+        return xdeepfm_oracle.xdeepfm_reference, xdeepfm_oracle
     return wide_deep_oracle.wide_deep_reference, wide_deep_oracle
 
 
@@ -79,7 +82,7 @@ def check_model(model, world, rank, local, dev, n_sm):
 
     def after_tower():
         for k in ("bet_w", "bet_d", "inv", "n_unique", "uniq", "flat_params", "loss_buf", "logits_buf", "flat_grads",
-                  "gsum_w", "gsum_d"):
+                  "gsum_w", "gsum_d", "scratch"):
             snap[k] = getattr(eng, k).clone()
 
     torch.cuda.synchronize(dev)  # this rank's rows and dense parameters are set before any peer reads them
@@ -95,7 +98,12 @@ def check_model(model, world, rank, local, dev, n_sm):
         u = int(s_nu[g])
         assert torch.equal(got_w[g, :u], bw[g, :u]) and torch.equal(got_d[g, :u], bd[g, :u]), (model, rank, g)
     assert torch.equal(snap["flat_params"], params0), (model, rank)
-    ref = ref_fn(s_inv, s_nu, got_w, got_d, dense, labels, snap["flat_params"])
+    inputs = (s_inv, s_nu, got_w, got_d, dense, labels, snap["flat_params"])
+    ref = ref_fn(*inputs)
+    if model == "xdeepfm":
+        from tests.test_gpu_xdeepfm_tower import reference_with_kernel_masks
+
+        ref = reference_with_kernel_masks(inputs, ref, snap["scratch"], "%s rank %d step 1" % (model, rank))
     got = {"loss": snap["loss_buf"], "logits": snap["logits_buf"], "grads": snap["flat_grads"],
            "gsum_wide": snap["gsum_w"].view(G, B), "gsum_deep": snap["gsum_d"].view(G, B, 8)}
     rs = R.check(got, ref, label="%s rank %d step 1" % (model, rank), n_sm=n_sm)
@@ -126,7 +134,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
     lines = []
-    for model in ("wide_deep", "dcn"):
+    for model in ("wide_deep", "dcn", "xdeepfm"):
         l0, l1, l2, worst = check_model(model, world, rank, local, dev, n_sm)
         lines.append("%s loss %.4f -> %.4f -> %.4f (graph), step 1 worst err/bound %.3f" % (model, l0, l1, l2, worst))
     dist.barrier()

@@ -40,13 +40,13 @@ def _condition(group, eng, ids, dense, labels, seed, dense_params=None):
     """Redraw, in place, the dense rows of the samples whose float64 pre-activation lies near a ReLU kink under the
     state the PS holds now (dense parameters: `dense_params` where given): their fp32 mask may flip, which no
     rounding bound covers.  Returns the float64 reference of the conditioned batch (_ps_reference)."""
-    gen = torch.Generator(device=DEV).manual_seed(seed)
+    gen = torch.Generator(device=dense.device).manual_seed(seed)
     for _ in range(40):
         _, ref = _ps_reference(group, eng, ids, dense, labels, dense_params)
         near = T.near_relu_kink(ref)
         if not bool(near.any()):
             return ref
-        dense[near] = torch.randn((int(near.sum()), T.ND), generator=gen, device=DEV)
+        dense[near] = torch.randn((int(near.sum()), T.ND), generator=gen, device=dense.device)
     raise AssertionError("conditioning did not converge")
 
 
