@@ -15,6 +15,17 @@ def check_tensor(t, name, dtype, shape, device):
                          % (name, dtype, shape, device, got))
 
 
+def truncated_normal(shape, std, gen, device):
+    """TF's truncated_normal initializer: a normal of stddev `std`, every draw outside two stddevs redrawn (not
+    rescaled).  `gen` is a torch.Generator on `device`."""
+    x = torch.randn(shape, generator=gen, device=device)
+    while True:
+        bad = x.abs() > 2
+        if not bool(bad.any()):
+            return x * std
+        x[bad] = torch.randn(int(bad.sum()), generator=gen, device=device)
+
+
 class AsyncEngine:
     """The part of one async worker on the parameter-server step that the census and frappe engines share.
 

@@ -21,7 +21,7 @@ import torch
 from elasticdl_b200 import _lib
 from elasticdl_b200._lib import DeepctrDeepfmArgs, check
 from elasticdl_b200.common.hash_utils import string_to_id
-from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor
+from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor, truncated_normal
 
 FIELDS, DENSE, ROWS, DIM = 26, 13, 1000, 4   # B200_DEEPCTR_DEEPFM_FIELDS, _DENSE, _ROWS, _DIM
 F = FIELDS * DIM + DENSE                     # 117
@@ -67,16 +67,6 @@ def flat_views(flat):
     return {n: flat[OFFSETS[n]:OFFSETS[n] + int(np.prod(s))].view(s) for n, s in PARAMS}
 
 
-def _truncated(shape, std, gen, device):
-    """A normal of stddev `std` redrawn outside two stddevs."""
-    x = torch.randn(shape, generator=gen, device=device)
-    while True:
-        bad = x.abs() > 2
-        if not bool(bad.any()):
-            return x * std
-        x[bad] = torch.randn(int(bad.sum()), generator=gen, device=device)
-
-
 def initial_params(seed, device):
     """The recalled initialisers: embedding tables truncated_normal(stddev = 1/sqrt(4)) (embedding_column's
     default), DNN and logit kernels glorot_normal (Keras' truncated normal of stddev sqrt(2 / (in + out))), biases
@@ -85,10 +75,10 @@ def initial_params(seed, device):
     flat = torch.zeros(N_PARAMS, dtype=torch.float32, device=device)
     for n, v in flat_views(flat).items():
         if n in EMB_NAMES:
-            v.copy_(_truncated(v.shape, 1.0 / np.sqrt(DIM), gen, device))
+            v.copy_(truncated_normal(v.shape, 1.0 / np.sqrt(DIM), gen, device))
         elif n.startswith("dnn/") and "kernel" in n:
-            v.copy_(_truncated(v.shape, float(np.sqrt(2.0 / (v.shape[0] + v.shape[1]))) / 0.87962566103423978, gen,
-                               device))
+            v.copy_(truncated_normal(v.shape, float(np.sqrt(2.0 / (v.shape[0] + v.shape[1]))) / 0.87962566103423978,
+                                     gen, device))
     return flat
 
 

@@ -1,18 +1,23 @@
 """The model zoo's embedding-column DNNs on the parameter-server step: census_dnn_model
-(model_zoo/census_dnn_model/census_functional_api.py:19-55 with census_feature_columns.py:19-62) and
-heart_functional_api (model_zoo/heart_functional_api/heart_functional_api.py:19-96).
+(model_zoo/census_dnn_model/census_functional_api.py:19-55 with census_feature_columns.py:19-62),
+heart_functional_api (model_zoo/heart_functional_api/heart_functional_api.py:19-96) and census_model_sqlflow's
+DNNClassifier (model_zoo/census_model_sqlflow/dnn/census_functional.py:28-70 with census_feature_column.py:35-67).
 
-Both are raw columns -> DenseFeatures -> Dense(16, relu) -> Dense(16, relu) -> Dense(1, sigmoid).  DenseFeatures
-holds numeric_column (pass-through), bucketized_column (a left-closed one-hot) and ElasticDL's embedding_column
-(feature_column/feature_column.py:24-221) over categorical_column_with_hash_bucket.  The trainer registers every
-embedding column as a PS embedding table named dense_features/<key>_embedding/embedding_weights:0 with the
-"uniform" initializer whatever the column's own initializer is (worker/ps_trainer.py:76-92, 200-211), so its rows
-are created when first pulled.  One layout table per model says where each column sits in x; the tower kernel
-(csrc/fc_dnn_tower.cu) reads nothing else.
+All three are raw columns -> DenseFeatures -> Dense(16, relu) -> Dense(16, relu) -> Dense(1, sigmoid).
+DenseFeatures holds numeric_column (pass-through), bucketized_column (a left-closed one-hot) and an embedding_column
+over categorical_column_with_hash_bucket.  Where the column is ElasticDL's (feature_column/feature_column.py:24-221:
+census_dnn_model, heart), the trainer registers it as a PS embedding table named
+dense_features/<key>_embedding/embedding_weights:0 with the "uniform" initializer whatever the column's own
+initializer is (worker/ps_trainer.py:76-92, 200-211), so its rows are created when first pulled.  Where it is
+TF's (census_model_sqlflow), the PS strategy swaps it for ElasticDL's only above 2 MB
+(common/model_handler.py:98-127): a smaller table stays a Keras variable of that name, a dense PS parameter the
+worker initialises, updated by the Indexed kernels on the batch's rows only (Q36).  One layout table per model says
+where each column sits in x and which kind each table is; the tower kernel (csrc/fc_dnn_tower.cu) reads the same
+rows and writes the same row gradients for both kinds.
 
 The step: pull_dense (the MLP) -> FeatureTransform (FarmHash buckets, Discretization) -> empty strings to the fill
 id 0 -> per-table dedup -> one pull_rows of the batch's unique rows -> the tower -> push_dense + push_rows ->
-push_end.  Quirks Q16-Q20 of DESIGN.md section 4 are what the layouts reproduce.
+push_end.  Quirks Q16-Q20 and Q36 of DESIGN.md section 4 are what the layouts reproduce.
 """
 import ctypes
 
@@ -22,10 +27,11 @@ import torch
 from elasticdl_b200 import _lib
 from elasticdl_b200._lib import FcDnnArgs, FcLayout, check
 from elasticdl_b200.common.hash_utils import string_to_id
-from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor
+from elasticdl_b200.workloads.async_engine import AsyncEngine, check_tensor, truncated_normal
 from elasticdl_b200.workloads.census_features import STRING_WIDTH, synthetic_raw_batch
 
 NUMERIC, BUCKET, EMBEDDING = 0, 1, 2  # B200_FC_NUMERIC, B200_FC_BUCKET, B200_FC_EMBEDDING
+PS_TABLE, DENSE_TABLE = "ps", "dense"  # a table's kind: a hashed PS embedding table, or a dense PS parameter
 HIDDEN = 16
 TILE = 64  # B200_FC_DNN_TILE
 
@@ -51,15 +57,23 @@ class Layout:
     inputs.  tables: [(key, hash buckets, dim)], table k hashing string column string_keys.index(key).  buckets:
     [(key, boundaries)], Discretization of a numeric column.  columns: DenseFeatures' concatenation order, as
     [(column name, kind, key)] -- quirk Q17: sorted by column name, recalled from TF's feature_column_v2 and not
-    verified here.  loss_mean: True = the gradients are batch means, False = batch sums (Q16)."""
+    verified here.  loss_mean: True = the gradients are batch means, False = batch sums (Q16).  table_kinds: per
+    table, PS_TABLE (default: a hashed PS table with "uniform" rows created when pulled) or DENSE_TABLE (a dense
+    [rows, dim] PS parameter initialised from TF's embedding_column default, truncated_normal(0, 1/sqrt(dim)),
+    first writer wins, and updated on the pushed rows only: Q36)."""
 
-    def __init__(self, name, numeric_keys, string_keys, tables, buckets, columns, loss_mean, optimizer):
+    def __init__(self, name, numeric_keys, string_keys, tables, buckets, columns, loss_mean, optimizer,
+                 table_kinds=None):
         self.name = name
         self.numeric_keys, self.string_keys = tuple(numeric_keys), tuple(string_keys)
         self.tables, self.buckets, self.columns = list(tables), list(buckets), list(columns)
         self.loss_mean = bool(loss_mean)
         self.optimizer = optimizer  # (PS optimizer type, its argument string, lr) of the model zoo entry
         self.table_names = [table_name(k) for k, _, _ in self.tables]
+        self.table_kinds = list(table_kinds) if table_kinds is not None else [PS_TABLE] * len(self.tables)
+        if len(self.table_kinds) != len(self.tables) or not set(self.table_kinds) <= {PS_TABLE, DENSE_TABLE}:
+            raise ValueError("table_kinds must give %r or %r for each of the %d tables, not %r"
+                             % (PS_TABLE, DENSE_TABLE, len(self.tables), table_kinds))
         blocks, off = [], 0
         for _, kind, key in self.columns:
             if kind == NUMERIC:
@@ -82,7 +96,7 @@ class Layout:
     def spec(self):
         """The layout as plain data (oracle/fc_dnn_oracle.py takes it)."""
         return {"F": self.F, "blocks": list(self.blocks), "tables": [(r, d) for _, r, d in self.tables],
-                "loss_mean": self.loss_mean}
+                "loss_mean": self.loss_mean, "table_kinds": list(self.table_kinds)}
 
     def _c_layout(self):
         c = FcLayout()
@@ -124,6 +138,14 @@ class Layout:
                 v.copy_((torch.rand(v.shape, generator=gen, device=device) * 2 - 1) * lim)
         return flat
 
+    def initial_tables(self, seed):
+        """The DENSE_TABLE tables' initial values, {name: float32 [rows, dim] on the CPU}: TF's embedding_column
+        default truncated_normal(mean 0, stddev 1/sqrt(dim)), draws outside two stddevs redrawn, from one CPU
+        generator seeded `seed` and drawn in table order (the same values on every device)."""
+        gen = torch.Generator().manual_seed(int(seed))
+        return {n: truncated_normal((r, d), 1.0 / np.sqrt(d), gen, "cpu")
+                for n, kind, (_, r, d) in zip(self.table_names, self.table_kinds, self.tables) if kind == DENSE_TABLE}
+
 
 CENSUS_CATEGORICAL = ["workclass", "education", "marital-status", "occupation", "relationship", "race", "sex",
                       "native-country"]
@@ -154,10 +176,20 @@ HEART = Layout(
              ("thalach", NUMERIC, "thalach"), ("trestbps", NUMERIC, "trestbps")],
     loss_mean=True,
     optimizer=("SGD", "learning_rate=1e-06;momentum=0.0;nesterov=false;", 1e-6))
-LAYOUTS = {"census_dnn_model": CENSUS_DNN, "heart_functional_api": HEART}
+# census_model_sqlflow/dnn: census_feature_column.py:35-53, TF's embedding_column(categorical_column_with_hash_bucket(
+# key, 64), dimension=16) after the four numeric_columns, so the same DenseFeatures as census_dnn_model; loss
+# census_functional.py:51-53 (binary_crossentropy(expand_dims(labels, 1), p): per-sample, never reduced, Q16);
+# optimizer :56-57 (Adam() defaults).  Its 64 x 16 tables (4 KB) stay Keras variables under the PS strategy (Q36).
+CENSUS_SQLFLOW_DNN = Layout(
+    "census_model_sqlflow_dnn", CENSUS_NUMERIC, CENSUS_CATEGORICAL,
+    tables=[(k, 64, 16) for k in CENSUS_CATEGORICAL], buckets=[], columns=CENSUS_DNN.columns,
+    loss_mean=False, optimizer=CENSUS_DNN.optimizer, table_kinds=[DENSE_TABLE] * len(CENSUS_CATEGORICAL))
+LAYOUTS = {"census_dnn_model": CENSUS_DNN, "heart_functional_api": HEART,
+           "census_model_sqlflow_dnn": CENSUS_SQLFLOW_DNN}
 for _l in LAYOUTS.values():
     assert [c for c, _, _ in _l.columns] == sorted(c for c, _, _ in _l.columns)  # Q17
 assert (CENSUS_DNN.F, CENSUS_DNN.n_mlp, HEART.F, HEART.n_mlp) == (132, 2417, 25, 705)
+assert (CENSUS_SQLFLOW_DNN.F, CENSUS_SQLFLOW_DNN.n_mlp) == (132, 2417)
 
 
 def layout_of(model):
@@ -201,12 +233,13 @@ def synthetic_heart_batch(B, seed, device, empty_fraction=0.05):
 
 def eval_metrics_fn(model):
     """The model's eval_metrics_fn as an EvaluationMetrics dict over the outputs {"logits", "probs"}.
-    census_dnn_model (census_functional_api.py:42-48): accuracy of round(p); tf.round rounds half to even, so
-    round(p) = 1 iff p > 0.5 iff the logit > 0.  heart_functional_api (heart_functional_api.py:89-96): argmax of
+    census_dnn_model (census_functional_api.py:42-48) and census_model_sqlflow_dnn (census_functional.py:60-66):
+    accuracy of round(p) against the int label; tf.round rounds half to even, so round(p) = 1 iff p > 0.5 iff the
+    logit > 0.  heart_functional_api (heart_functional_api.py:89-96): argmax of
     the [B, 1] output over axis 1 is always 0, so its "accuracy" is the share of label-0 samples (Q20)."""
     from elasticdl_b200.common.evaluation_utils import zoo_eval_metrics
 
-    if layout_of(model) is CENSUS_DNN:
+    if layout_of(model) in (CENSUS_DNN, CENSUS_SQLFLOW_DNN):
         return {"logits": {"accuracy": zoo_eval_metrics(0.0)["logits"]["accuracy"]}}
 
     def heart_accuracy(labels, predictions):
@@ -311,16 +344,20 @@ def fc_dnn_tower(model, numeric, ids, strings, inv, n_unique, rows, labels, flat
 
 
 class FeatureColumnDNNEngine(AsyncEngine):
-    """One async worker of census_dnn_model or heart_functional_api on the parameter-server step.
+    """One async worker of census_dnn_model, heart_functional_api or census_model_sqlflow_dnn on the
+    parameter-server step.
 
-    group: an async PSGroup, as AsyncEngine takes it.  model: "census_dnn_model" or "heart_functional_api" (or
-    a Layout).  register=True registers the MLP's six dense parameters (initial values first-writer-wins, as
-    PushModel does) and the embedding-column tables as hashed "uniform" tables; register=False attaches to a
-    group.clone_view() of a group where another engine registered them, for another worker thread.
+    group: an async PSGroup, as AsyncEngine takes it.  model: one of LAYOUTS (or a Layout).  register=True
+    registers the MLP's six dense parameters and the embedding-column tables, a PS_TABLE as a hashed "uniform"
+    table, a DENSE_TABLE as a dense [rows, dim] parameter (initial values of both dense kinds first-writer-wins, as
+    PushModel does: Layout.initial_mlp(seed) and initial_tables(seed)); register=False attaches to a
+    group.clone_view() of a group where another engine registered them, for another worker thread.  Both table
+    kinds go through the same pull_rows and push_rows launches; on a dense parameter push_rows is the Indexed
+    update of the batch's unique rows and their slots (Q36).
     step(numeric float32 [n, B], strings uint8 [m, B, 32], labels float32 [B]) runs pull_dense -> the feature
     transform -> empty strings to id 0 -> the per-table dedup -> one pull_rows of the unique rows -> the tower ->
     push_begin -> push_dense -> push_rows (counts on the device) -> push_end, with no host read, and returns the
-    loss on the device (a batch sum for census_dnn_model, a mean for heart_functional_api: Q16).  capture() /
+    loss on the device (a batch sum for the census models, a mean for heart_functional_api: Q16).  capture() /
     replay() run the same step as one CUDA graph over static inputs.  lr_schedule: as AsyncEngine takes it."""
 
     def __init__(self, group, model, batch, lr, seed=0, register=True, lr_schedule=None):
@@ -331,14 +368,18 @@ class FeatureColumnDNNEngine(AsyncEngine):
         self.inputs = [("numeric", torch.float32, (len(L.numeric_keys), B)),
                        ("strings", torch.uint8, (len(L.string_keys), B, STRING_WIDTH)),
                        ("labels", torch.float32, (B,))]
-        self.owner = {n: string_to_id(n, g.n_shards) for n, _ in L.mlp}
+        self.owner = {n: string_to_id(n, g.n_shards)
+                      for n in MLP_NAMES + [t for t, kind in zip(L.table_names, L.table_kinds) if kind == DENSE_TABLE]}
         if register:
-            for n, (_, rows, dim) in zip(L.table_names, L.tables):
-                g.register_table(n, dim, "uniform", expected_rows=max(4 * rows, 1024))
+            for n, kind, (_, rows, dim) in zip(L.table_names, L.table_kinds, L.tables):
+                if kind == PS_TABLE:
+                    g.register_table(n, dim, "uniform", expected_rows=max(4 * rows, 1024))
+                else:
+                    g.register_dense(n, (rows, dim), self.owner[n])
             for n, s in L.mlp:
                 g.register_dense(n, s, self.owner[n])
             g.commit()
-            g.init_dense(L.flat_views(L.initial_mlp(seed, dev)).items())
+            g.init_dense(list(L.flat_views(L.initial_mlp(seed, dev)).items()) + list(L.initial_tables(seed).items()))
         self.tids = {n: g.lookup(n)[0] for n in L.table_names + MLP_NAMES}  # PSNotFound if unregistered
         self.flat = torch.zeros(L.n_mlp, dtype=torch.float32, device=dev)
         self.views = L.flat_views(self.flat)
@@ -435,11 +476,14 @@ def twin_features(model, numeric, strings, transform=None):
 
 
 class FeatureColumnDNN(torch.nn.Module):
-    """The same model as a torch module for the drop-in ParameterServerTrainer: one elasticdl_b200.layers.Embedding
-    per embedding column under the reference's table name (hashed "uniform" PS tables), empty-string rows zeroed,
-    the three Dense layers as Keras-named parameters (dense/kernel:0 [F, 16], ...) so that the trainer registers
-    the same PS parameters the engine does.  forward(twin_features(...)) returns the probability [B]; the loss is
-    the Keras clipped binary cross-entropy, summed (census_dnn_model) or averaged (heart_functional_api)."""
+    """The same model as a torch module for the drop-in ParameterServerTrainer: per embedding column, a PS_TABLE is
+    an elasticdl_b200.layers.Embedding under the reference's table name (a hashed "uniform" PS table) and a
+    DENSE_TABLE a torch.nn.Embedding(rows, dim) whose weight is also this module's parameter of the table's name,
+    so that ParameterServerModelHandler keeps it as a DenseTableEmbedding (at most 2 MB) and the trainer pulls and
+    pushes its rows by id under that name (Q36).  Empty-string rows are zeroed, and the three Dense layers are
+    Keras-named parameters (dense/kernel:0 [F, 16], ...), so that the trainer registers the same PS parameters, with
+    the same update kinds, as the engine does.  forward(twin_features(...)) returns the probability [B]; the loss is
+    the Keras clipped binary cross-entropy, summed (the census models) or averaged (heart_functional_api)."""
 
     def __init__(self, model, lr=None, optimizer=None):
         super().__init__()
@@ -447,13 +491,18 @@ class FeatureColumnDNN(torch.nn.Module):
 
         L = self.layout = layout_of(model)
         self.tables = torch.nn.ModuleList()
-        for key, _, dim in L.tables:
-            e = Embedding(dim, embeddings_initializer="uniform", name="%s_embedding" % key)
-            e.set_embedding_weight_name(table_name(key))
+        for kind, (key, rows, dim) in zip(L.table_kinds, L.tables):
+            if kind == PS_TABLE:
+                e = Embedding(dim, embeddings_initializer="uniform", name="%s_embedding" % key)
+                e.set_embedding_weight_name(table_name(key))
+            else:  # registered here first, so named_parameters() gives the weight the table's name
+                e = torch.nn.Embedding(rows, dim)
+                self.register_parameter(table_name(key), e.weight)
             self.tables.append(e)
         for n, s in L.mlp:
             self.register_parameter(n, torch.nn.Parameter(torch.zeros(s)))
         self.load_mlp(L.initial_mlp(0, "cpu"))
+        self.load_tables(L.initial_tables(0))
         lr = L.optimizer[2] if lr is None else lr
         opt = torch.optim.Adam if (optimizer or L.optimizer[0]).lower() == "adam" else torch.optim.SGD
         self.optimizer = opt([getattr(self, n) for n in MLP_NAMES], lr=lr)
@@ -464,6 +513,12 @@ class FeatureColumnDNN(torch.nn.Module):
         with torch.no_grad():
             for n in MLP_NAMES:
                 getattr(self, n).copy_(v[n])
+
+    def load_tables(self, tables):
+        """Copy {table name: [rows, dim]} into the DENSE_TABLE weights."""
+        with torch.no_grad():
+            for n, v in tables.items():
+                getattr(self, n).copy_(v)
 
     def dense_features(self, features):
         L = self.layout

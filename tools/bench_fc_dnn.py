@@ -39,7 +39,7 @@ def power_limit():
 def batches(L, B, n, seed):
     out = []
     for s in range(n):
-        if L is M.CENSUS_DNN:
+        if L is not M.HEART:
             numeric, strings = M.synthetic_census_batch(B, seed + s, DEV)
             labels = (torch.rand(B, generator=torch.Generator(device=DEV).manual_seed(seed + s), device=DEV)
                       < 0.25).float()
