@@ -233,7 +233,9 @@ int launch_tile_tower(const b200_deepfm_args_t* args, void* stream, int what, si
   long long grid = (long long)d.sms * 2;
   if (grid > ntile) grid = ntile;
   if (what & 1) {
-    prep(dim3(4, BACKWARD ? a.G : 1), st, a, w1x, (int)grid);
+    // 16 blocks per id group: the prep is on the step's critical path, and most of it is zeroing the live rows of
+    // the per-unique-id sums (up to 2 x 25 000 float4 stores for one group), which 4 blocks ran as long loops
+    prep(dim3(16, BACKWARD ? a.G : 1), st, a, w1x, (int)grid);
     if (int rc = E::launched("tile tower prep", launches)) return rc;
   }
   if (!(what & 2)) return 0;

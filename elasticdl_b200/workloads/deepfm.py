@@ -542,6 +542,25 @@ class DeepFMPSEngine:
         self.loss_cursor = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.logits_buf = torch.empty(B, **f32)
         self.zero_versions = [0] * group.n_shards
+        # tail_prep (one shard, tile tower, direct unpaired tables, not xDeepFM, whose prologue also rewrites the
+        # CIN's scratch): a lookahead step prepares the NEXT one beside its own row push -- dense pull, then the
+        # tower prologue -- so the next step opens with its tower.  The prologue zeroes what a step accumulates
+        # into, and callers read this step's accumulators after it, so the two plans of the pipeline accumulate
+        # into two sets (_accs): step i trains into its plan's set and zeroes the other plan's, which step i - 1
+        # filled, over the live rows that step recorded (_acc_rows) -- the dedup of batch i + 1 is rewriting that
+        # plan's counts meanwhile.  gsum_w / gsum_d / flat_grads / loss_buf name the set of the last step run.
+        # With more shards the other ranks' dense pushes must land before the pull: pull and prologue stay at
+        # the head, as they do for step() and for the first lookahead step after anything else ran
+        # (_ready: the last step was a lookahead step that prepared the next).
+        self.tail_prep = (self.tower_kind == "tile" and group.n_shards == 1 and self.exchange == "direct"
+                          and not self.paired and model != "xdeepfm")
+        self._ready = False
+        self._ACC = ("gsum_w", "gsum_d", "flat_grads", "loss_buf")
+        self._accs = [{k: getattr(self, k) for k in self._ACC}]
+        if self.tail_prep:
+            self._accs.append({k: torch.zeros_like(v) for k, v in self._accs[0].items()})
+        self._acc_rows = [torch.zeros(G, dtype=torch.int32, device=dev) for _ in self._accs]
+        self._plan_acc = [0]
 
         self.loss_fn = torch.nn.BCEWithLogitsLoss()
         # everything addressed through one (uniq, inv, n_unique) triple is a "plan"; the lookahead
@@ -572,14 +591,18 @@ class DeepFMPSEngine:
             self.capture_ahead()
 
     _PLAN_ATTRS = ("uniq", "inv", "n_unique", "pull_segs", "push_segs", "pull_pair", "push_pair", "tower_args",
-                   "tower_rows", "pull_names", "push_names")
+                   "tower_rows", "pull_names", "push_names", "push_dense_segs")
 
-    def _make_plan(self):
+    def _make_plan(self, acc=0):
+        """A plan accumulating into set `acc`; the accumulators named on the engine stay what they were."""
         dev, G, B = self.device, self.G, self.B
+        named = {k: getattr(self, k) for k in self._ACC}
+        self.__dict__.update(self._accs[acc])
         self.uniq = torch.empty(G * B, dtype=torch.int64, device=dev)
         self.inv = torch.empty(G * B, dtype=torch.int32, device=dev)
         self.n_unique = torch.empty(G, dtype=torch.int32, device=dev)
         self._build_segs()
+        self.__dict__.update(named)
         return {k: getattr(self, k) for k in self._PLAN_ATTRS}
 
     def _use(self, p):
@@ -662,13 +685,16 @@ class DeepFMPSEngine:
             setattr(r, fam + "_param_off", off)
         return r
 
-    def step(self, ids, dense, labels, ev=None, after_tower=None):
+    def step(self, ids, dense, labels, ev=None, after_tower=None, next_plan=None):
         """ids int64 [G, B] (group-major), dense fp32 [B, 13], labels fp32 [B] -- all on the device.
         Returns the loss (device scalar).  ev: optional dict name -> list; CUDA-event pairs are
-        recorded around the named PS kernels on the launching stream."""
+        recorded around the named PS kernels on the launching stream.  next_plan: the plan the next step
+        trains on (lookahead pipeline); with tail_prep this step prepares it (see __init__)."""
         g, lib, h = self.group, self.group.lib, self.group._h
         G, B, D = self.G, self.B, self.D
         st = g._stream()
+        ready, self._ready = self._ready, False  # until this step has prepared the next one
+        self.__dict__.update(self._accs[self._plan_acc[self.cur]])
 
         def mark(name):
             if ev is None:
@@ -686,9 +712,10 @@ class DeepFMPSEngine:
         # push_end) that do not depend on the row kernels beside them.  With
         # `branch` they run on a second stream -- inside a captured graph these become parallel branches --
         # while the main stream carries unique -> pull -> tower -> push rows:
-        #   aux:  pull_dense -> push_begin -> tower prologue  | joined before the tower
-        #   aux:  push_dense                                   | beside the row push, joined before push_end
+        #   aux:  pull_dense -> tower prologue -> push_begin  | the tower waits for the prologue
+        #   aux:  push_dense (-> pull_dense -> prologue of the next step: tail_prep)  | beside the row push
         branch = self.tower_kind == "tile" and ev is None
+        at_tail = branch and self.tail_prep and next_plan is not None
         main = torch.cuda.current_stream(self.device)
         if branch:
             if self.aux is None:
@@ -704,9 +731,12 @@ class DeepFMPSEngine:
         if branch:
             self.aux.wait_stream(main)  # n_unique of this batch, parameters of the previous step
             with torch.cuda.stream(self.aux):
-                arr, n = self.pull_dense_segs
-                check(lib.b200ps_pull_dense(h, arr, n, g._stream()))
-                self._tower_call(self.calls.prologue, a, g._stream())
+                if not (at_tail and ready):
+                    if at_tail:  # entering the pipeline: no stale row in either set (the tails zero live rows)
+                        self._zero_accs()
+                    arr, n = self.pull_dense_segs
+                    check(lib.b200ps_pull_dense(h, arr, n, g._stream()))
+                    self._tower_call(self.calls.prologue, a, g._stream())
                 ev_prep = torch.cuda.Event()
                 ev_prep.record(self.aux)  # the tower waits for this, not for push_begin behind it
                 g.push_begin(self.lr, self.zero_versions)
@@ -758,6 +788,8 @@ class DeepFMPSEngine:
                 arr, n = dense_segs
                 check(lib.b200ps_push_dense(h, arr, n, g._stream()))
                 self._publish_loss(loss, g._stream())
+                if at_tail:
+                    self._prepare_next(a, next_plan, g._stream())
         else:
             g.push_begin(self.lr, self.zero_versions)
             arr, n = dense_segs
@@ -781,7 +813,27 @@ class DeepFMPSEngine:
             main.wait_stream(self.aux)
         g.push_end(sync=False)
         self.steps += 1
+        self._ready = at_tail
         return loss.detach().reshape(())
+
+    def _zero_accs(self):
+        """Both accumulator sets to 0 on the current stream."""
+        for acc in self._accs:
+            for t in acc.values():
+                t.zero_()
+
+    def _prepare_next(self, a, q, st):
+        """The head of the step on plan q, on `st` after this step's dense push (tail_prep): the dense pull, the
+        live rows of this step's set recorded, then the prologue over plan q's set -- its live rows are the ones
+        recorded by the step that last filled it."""
+        g = self.group
+        arr, n = self.pull_dense_segs
+        check(g.lib.b200ps_pull_dense(g._h, arr, n, st))
+        self._acc_rows[self._plan_acc[self.cur]].copy_(self.n_unique)
+        nxt = type(a).from_buffer_copy(self.plans[q]["tower_args"])
+        nxt.dense, nxt.labels = a.dense, a.labels  # checked, not read, by a prologue
+        nxt.n_unique = self._acc_rows[self._plan_acc[q]].data_ptr()
+        self._tower_call(self.calls.prologue, nxt, st)
 
     def _tower_call(self, fn, args, st):
         """One tower entry point on `args` (DeepFMArgs); RuntimeError with its return code and
@@ -821,7 +873,8 @@ class DeepFMPSEngine:
     def _ensure_plans(self):
         if len(self.plans) == 1:
             cur = self.cur
-            self.plans.append(self._make_plan())
+            self.plans.append(self._make_plan(len(self._accs) - 1))
+            self._plan_acc.append(len(self._accs) - 1)
             self._use(cur)
             self.side = torch.cuda.Stream(device=self.device)
 
@@ -832,6 +885,7 @@ class DeepFMPSEngine:
         reference's dataset.prefetch(1) work, elasticdl/python/worker/worker.py:334)."""
         self._ensure_plans()
         self._unique_into(ids)
+        self._ready = False  # the first step pulls what the PS holds now
 
     def step_ahead(self, dense, labels, next_ids, ev=None):
         """One training step on the prepared batch + the dedup of `next_ids` (int64 or int32 [G, B],
@@ -852,7 +906,7 @@ class DeepFMPSEngine:
                 self._unique_into(next_ids)
             self._use(p)
 
-        loss = self.step(None, dense, labels, ev=ev, after_tower=fork)
+        loss = self.step(None, dense, labels, ev=ev, after_tower=fork, next_plan=1 - p)
         main.wait_stream(self.side)  # join
         self._use(1 - p)
         return loss
@@ -870,16 +924,17 @@ class DeepFMPSEngine:
                              for _ in range(2)]
         views = [packed_views(b, G, B, self.widths) for b in self.s_packed]
         torch.cuda.synchronize(dev)
-        start, steps = self.cur, self.steps
+        start, steps, ready = self.cur, self.steps, self._ready
         self.graphs_ahead = [None, None]
         for p in (start, 1 - start):
             assert self.cur == p
             gr = torch.cuda.CUDAGraph()
+            self._ready = True  # the graphs open with the tower; step_ahead_graph runs the head of the first
             with torch.cuda.graph(gr):
                 self.step_ahead(views[p][1], views[p][2], views[1 - p][0])
             self.graphs_ahead[p] = gr
         self._use(start)
-        self.steps = steps  # capture does not execute
+        self.steps, self._ready = steps, ready  # capture does not execute
         return self.graphs_ahead
 
     def _fill(self, dst, batch):
@@ -904,13 +959,22 @@ class DeepFMPSEngine:
             self.capture_ahead()
         self._fill(self.s_packed[self.cur], batch)
         self._unique_into(packed_views(self.s_packed[self.cur], self.G, self.B, self.widths)[0])
+        self._ready = False  # the first step pulls what the PS holds now
 
     def step_ahead_graph(self, *next_batch):
         """step_ahead through the captured graphs: trains on the batch loaded by the previous call (or
         prepare_packed) while `next_batch` -- (packed,) or (ids, dense, labels) -- is loaded and its ids
         are deduplicated.  Inputs may be pinned-host or device tensors."""
         self._fill(self.s_packed[1 - self.cur], next_batch)
-        self.graphs_ahead[self.cur].replay()
+        p = self.cur
+        if self.tail_prep and not self._ready:  # the head the graphs leave out
+            self._zero_accs()
+            arr, n = self.pull_dense_segs
+            check(self.group.lib.b200ps_pull_dense(self.group._h, arr, n, self.group._stream()))
+            self._tower_call(self.calls.prologue, self.tower_args, self.group._stream())
+        self.graphs_ahead[p].replay()
+        self._ready = self.tail_prep
+        self.__dict__.update(self._accs[self._plan_acc[p]])
         self._use(1 - self.cur)
         self.steps += 1
         return self.loss_buf.reshape(())
@@ -925,10 +989,12 @@ class DeepFMPSEngine:
         dev, G, B = self.device, self.G, self.B
         self.s_one = torch.zeros(packed_nbytes(G, B, self.widths), dtype=torch.uint8, device=dev)
         torch.cuda.synchronize(dev)
+        ready = self._ready
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.step(*packed_views(self.s_one, G, B, self.widths))
         self.steps -= 1  # capture does not execute
+        self._ready = ready
         return self.graph
 
     def step_graph(self, *batch):
@@ -936,6 +1002,7 @@ class DeepFMPSEngine:
         or device tensors."""
         self._fill(self.s_one, batch)
         self.graph.replay()
+        self._ready = False
         self.steps += 1
         return self.loss_buf.reshape(())
 
@@ -976,6 +1043,7 @@ class DeepFMPSEngine:
         dedup workspace and (uniq, inv, n_unique) plan, so a prepared lookahead batch stays intact."""
         g, lib, h = self.group, self.group.lib, self.group._h
         st = g._stream()
+        self._ready = False  # the forward tower runs its own prologue and takes the tile counter
         if self._predict_state is None:
             cur = self.cur
             ws = torch.zeros(lib.b200ps_unique_workspace(self.G, self.B), dtype=torch.uint8, device=self.device)
