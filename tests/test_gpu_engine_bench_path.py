@@ -107,6 +107,12 @@ def _check_step(group, eng, t, p, dedup, ref, pre, sample, label):
     got = {"loss": eng.loss_buf, "logits": eng.logits_buf, "grads": eng.flat_grads,
            "gsum_wide": eng.gsum_w.view(G, B), "gsum_deep": eng.gsum_d.view(G, B, D)}
     T.check(got, ref, families=T.FAMILIES, label=what, n_sm=_n_sm())
+    _check_push(group, eng, t, dedup, pre, sample, what)
+
+
+def _check_push(group, eng, t, dedup, pre, sample, what):
+    """Checks 3-4 of step t, whatever the model's tower."""
+    G, B, D = eng.G, eng.B, eng.D
     # 3. push: oracle Adam (step t) on the gradient rows the engine pushed, from the pre-step state, bit for bit
     tabs, dense0, snap0 = pre
     assert snap0 == [(t - 1, t - 1, True)], (what, snap0)
